@@ -40,7 +40,15 @@ def measured_peak_hbm():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3, not a measured rate)"
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Writes what the timed path returned in its last step as <out_dir>/<name>.npy (float64 holds every
+    hop count and -1 exactly), so that two builds can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 class ClockSampler(threading.Thread):
@@ -189,7 +197,11 @@ def main():
     ap.add_argument("--alpha", type=int, default=0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the c3 / c5 sub-records (R-MAT-24 / R-MAT-26)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's result columns (lengths, valid) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes what the GPU path computed; the reference arm has no such output")
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3
 
@@ -320,6 +332,11 @@ def main():
     ms_total = float(ms.item())
     value = total_pairs * args.steps / (ms_total / 1e3)
     last_dev = d_len[(nsteps - 1) & 1].cpu().numpy()
+    if args.dump_outputs and rank == 0:
+        # a caller of the timed path gets the length column (-1 = NULL) and the validity column; with several
+        # ranks d_val holds only this rank's rows, the assembled lengths carry the validity of all of them
+        last_valid = d_val.cpu().numpy() if world == 1 else (last_dev >= 0)
+        dump_outputs(args.dump_outputs, {"lengths": last_dev, "valid": last_valid})
 
     # ---- e2e: host buffers through the C ABI (H2D pairs + D2H results inside), result assembly for N > 1
     sharded = sharding.ShardedLengths(csr, dev, pgq.Options(args.lanes, args.direction, args.alpha)) if world > 1 else None
@@ -377,13 +394,6 @@ def main():
         W_total, expand_ms = acc["edges_traversed"], acc["expand_ms"]
         expand_launches = acc["push_levels"] + acc["pull_levels"]
         achieved = (W_total * 4.0 / 1e9) / (expand_ms / 1e3) if expand_ms > 0 else 0.0
-        traffic, traffic_src = None, None
-        try:
-            with open(os.path.join(ROOT, "profiles", "dominant_kernel_traffic.json")) as f:
-                tj = json.load(f)
-                traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("source")
-        except Exception:
-            pass
         pull_l = max(acc["pull_levels"], 1)
         dominant = {"kernel": "k_pull_fused (bottom-up level: expansion + update)", "launches_per_step": acc["pull_levels"] / steps,
                     "ms": acc["pull_ms"] / pull_l, "alg_bytes": acc["pull_edges"] * 4 // pull_l,
@@ -402,7 +412,7 @@ def main():
             "gpu_launches": acc["kernel_launches"],
             "clocks": clocks,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src,
+                         "frac": achieved / peak, "traffic": None, "traffic_source": None,
                          "kernel": "frontier expansion, all launches of a step (k_pull_fused / k_expand_push*)",
                          "dominant": dominant,
                          "algorithmic_bytes_per_step": W_total * 4 // steps,

@@ -1,6 +1,6 @@
 """Build + ctypes binding of libduckpgq_b200.so (the C ABI declared in include/duckpgq_b200.h).
 
-The library is compiled in-tree (duckpgq_extension_b200/lib/) for sm_100a only.  There is no CPU
+The library is compiled in-tree (duckpgq_extension_b200/lib/) for sm_90a (H100) only.  There is no CPU
 fallback: if the shared library is missing or cannot be loaded, load() raises.
 """
 from __future__ import annotations
@@ -20,7 +20,7 @@ SOURCES = ["pgq_csr.cu", "pgq_bfs.cu", "pgq_api.cu", "pgq_cheapest.cu", "pgq_mul
 HEADERS = ["pgq_internal.h", "pgq_tile.cuh", "pgq_pull.cuh"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "-cudart", "static",
 ]
 
@@ -41,7 +41,7 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """nvcc -gencode arch=compute_100a,code=sm_100a ... -> duckpgq_extension_b200/lib/libduckpgq_b200.so"""
+    """nvcc -gencode arch=compute_90a,code=sm_90a ... ->duckpgq_extension_b200/lib/libduckpgq_b200.so"""
     if not force and not needs_build():
         return LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)

@@ -1,6 +1,6 @@
 // pgq_cheapest.cu -- cheapest_path_length on the device CSR: the batched Bellman-Ford of
 // cheapest_path_length.cpp:12-136 (TemplatedBatchBellmanFord: one lane per row, all lanes of an edge
-// relaxed together, sweeps until nothing changes).  sm_100a only.
+// relaxed together, sweeps until nothing changes).  sm_90a only.
 //
 // The reference relaxes in place, sequentially, in CSR order; the distances it ends with are the least
 // fixed point of  d[n] = min(d[n], d[v] + w(v,n))  -- for int64 exactly, for double because fl(a + w)

@@ -1,7 +1,7 @@
 // pgq_csr.cu -- device-resident CSR: context/workspace plumbing, the device-side CSR build that
 // replaces create_csr_vertex / create_csr_edge (reference: src/core/functions/scalar/csr_creation.cpp),
 // the transposed (in-edge) CSC used by the bottom-up step, and the row-head metadata of the
-// edge-tiled kernels.  sm_100a only.
+// edge-tiled kernels.  sm_90a only.
 #include <algorithm>
 #include <atomic>
 #include <cstdarg>
@@ -101,8 +101,8 @@ extern "C" int pgq_ctx_create(int device, pgq_ctx **out) {
 	PGQ_CUDA(cudaSetDevice(device));
 	cudaDeviceProp prop;
 	PGQ_CUDA(cudaGetDeviceProperties(&prop, device));
-	if (prop.major < 10) {
-		return pgq_fail(PGQ_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_100a only", device,
+	if (prop.major != 9 || prop.minor != 0) { // sm_90a code runs on compute capability 9.0 and nothing else
+		return pgq_fail(PGQ_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device,
 		                prop.major, prop.minor);
 	}
 	pgq_ctx *ctx = new (std::nothrow) pgq_ctx();
@@ -201,8 +201,49 @@ static int ws_take(pgq_ctx *ctx, Workspace **out, bool block) {
 		ctx->cv.notify_one();
 		return pgq_fail(ws ? PGQ_ERR_CUDA : PGQ_ERR_OOM, "workspace creation failed: %s", cudaGetErrorString(e));
 	}
+	ws->ctx = ctx;
 	*out = ws;
 	return PGQ_OK;
+}
+
+// Gives the device memory of the context that no call is using back to the driver: the buffers of the pooled
+// (idle) workspaces and the cache of freed CSR buffers.  Called when an allocation fails, so that a graph that
+// fills most of the device (R-MAT-26 takes 40 GB of an 80 GB H100) is not refused for scratch that earlier
+// calls left behind.  (cudaFree waits for the work still queued on those buffers.)
+static void ctx_release_idle(pgq_ctx *ctx) {
+	std::vector<void *> drop;
+	{
+		std::lock_guard<std::mutex> g(ctx->mu);
+		for (Workspace *w : ctx->free_ws) {
+			for (int i = 0; i < PGQ_WS_SLOTS; i++) {
+				if (w->buf[i]) {
+					drop.push_back(w->buf[i]);
+				}
+				w->buf[i] = nullptr;
+				w->cap[i] = 0;
+			}
+			w->clean_from = -1; // its lane-mask arrays are gone
+		}
+		for (auto &kv : ctx->buf_cache) {
+			drop.push_back(kv.second);
+		}
+		ctx->buf_cache.clear();
+		ctx->buf_cache_bytes = 0;
+	}
+	for (void *q : drop) {
+		cudaFree(q);
+	}
+}
+
+// cudaMalloc that, when the device is full, releases the context's idle memory and tries once more
+static cudaError_t ctx_malloc(pgq_ctx *ctx, void **p, size_t bytes) {
+	cudaError_t e = cudaMalloc(p, bytes);
+	if (e != cudaSuccess && ctx) {
+		cudaGetLastError();
+		ctx_release_idle(ctx);
+		e = cudaMalloc(p, bytes);
+	}
+	return e;
 }
 
 int pgq_ws_acquire(pgq_ctx *ctx, Workspace **out) {
@@ -230,7 +271,7 @@ int pgq_ws_grow(Workspace *ws, int slot, size_t bytes, size_t keep_bytes, cudaSt
 	if (ws->cap[slot] < bytes) {
 		const size_t want = std::max(bytes * 2, (size_t)4096);
 		void *bigger = nullptr;
-		cudaError_t e = cudaMalloc(&bigger, want);
+		cudaError_t e = ctx_malloc(ws->ctx, &bigger, want);
 		if (e != cudaSuccess) {
 			cudaGetLastError();
 			return pgq_fail(PGQ_ERR_OOM, "device allocation of %zu bytes failed: %s", want, cudaGetErrorString(e));
@@ -271,7 +312,7 @@ int pgq_ws_reserve(Workspace *ws, int slot, size_t bytes, void **out) {
 		if (e != cudaSuccess) {
 			cudaGetLastError();
 			want = bytes;
-			e = cudaMalloc(&ws->buf[slot], want);
+			e = ctx_malloc(ws->ctx, &ws->buf[slot], want);
 		}
 		if (e != cudaSuccess) {
 			cudaGetLastError();
@@ -859,23 +900,7 @@ static int dev_alloc(pgq_csr *csr, void **p, size_t bytes) {
 		}
 	}
 	if (!*p) {
-		cudaError_t e = cudaMalloc(p, bytes);
-		if (e != cudaSuccess) { // give the cached buffers back to the driver and try once more
-			cudaGetLastError();
-			std::vector<void *> drop;
-			{
-				std::lock_guard<std::mutex> g(ctx->mu);
-				for (auto &kv : ctx->buf_cache) {
-					drop.push_back(kv.second);
-				}
-				ctx->buf_cache.clear();
-				ctx->buf_cache_bytes = 0;
-			}
-			for (void *q : drop) {
-				cudaFree(q);
-			}
-			e = cudaMalloc(p, bytes);
-		}
+		cudaError_t e = ctx_malloc(ctx, p, bytes);
 		if (e != cudaSuccess) {
 			cudaGetLastError();
 			*p = nullptr;
@@ -1033,7 +1058,7 @@ static int build_pull_graph(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	PGQ_TRY(pgq_ws_reserve(ws, 9, row_bytes, (void **)&long_flag));
 	PGQ_TRY(pgq_ws_reserve(ws, 10, row_bytes, (void **)&short_flag));
 	PGQ_TRY(pgq_ws_reserve(ws, 1, pgq_scan_tmp_elems(std::max<int64_t>(n_rows, m / 32) + 2) * sizeof(int32_t), (void **)&scan_tmp));
-	k_pull_classify<<<grid_for(n_rows + 1, 256, 148 * 8), 256, 0, s>>>(csr->in.off, n_rows, long_deg, long_flag, short_flag);
+	k_pull_classify<<<grid_for(n_rows + 1, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->in.off, n_rows, long_deg, long_flag, short_flag);
 	PGQ_CUDA(cudaGetLastError());
 	PGQ_TRY(pgq_scan_exclusive_i32(long_deg, long_deg, n_rows + 1, scan_tmp, s));
 	PGQ_TRY(pgq_scan_exclusive_i32(long_flag, long_flag, n_rows + 1, scan_tmp, s));
@@ -1062,11 +1087,11 @@ static int build_pull_graph(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	if (g.n_rows > 0) {
 		int32_t *off_by_rank;
 		PGQ_TRY(pgq_ws_reserve(ws, 11, (size_t)(g.n_rows + 2) * sizeof(int32_t), (void **)&off_by_rank));
-		k_pull_long_fill<<<grid_for(n_rows * 32, 256, 148 * 16), 256, 0, s>>>(csr->in.off, csr->in.adj, n_rows, long_deg,
+		k_pull_long_fill<<<grid_for(n_rows * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->in.off, csr->in.adj, n_rows, long_deg,
 		                                                                long_flag, g.adj, g.row, off_by_rank);
 		const int32_t m_long = (int32_t)g.m;
 		PGQ_CUDA(cudaMemcpyAsync(off_by_rank + g.n_rows, &m_long, sizeof(int32_t), cudaMemcpyHostToDevice, s));
-		k_pull_long_meta<<<grid_for(g.n_rows, 256, 148 * 8), 256, 0, s>>>(off_by_rank, g.n_rows, g.head, g.chunk_rank);
+		k_pull_long_meta<<<grid_for(g.n_rows, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(off_by_rank, g.n_rows, g.head, g.chunk_rank);
 		PGQ_CUDA(cudaGetLastError());
 		PGQ_CUDA(cudaStreamSynchronize(s)); // (m_long lives on this frame)
 	}
@@ -1080,10 +1105,10 @@ static int build_pull_graph(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 		PGQ_TRY(pgq_ws_reserve(ws, 6, std::max(kv, ws->cap[6]), (void **)&key_b));
 		PGQ_TRY(pgq_ws_reserve(ws, 7, std::max(kv, ws->cap[7]), (void **)&val_a));
 		PGQ_TRY(pgq_ws_reserve(ws, 12, kv, (void **)&val_b));
-		k_pull_short_list<<<grid_for(n_rows, 256, 148 * 8), 256, 0, s>>>(csr->in.off, n_rows, short_flag, key_a, val_a);
+		k_pull_short_list<<<grid_for(n_rows, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->in.off, n_rows, short_flag, key_a, val_a);
 		PGQ_CUDA(cudaGetLastError());
 		PGQ_TRY(radix_sort_pairs(ws, key_a, key_b, val_a, val_b, g.n_short, 5, s, &key_res, &val_res));
-		k_pull_slice_width<<<grid_for(g.n_slices + 1, 256, 148 * 8), 256, 0, s>>>(key_res, g.n_short, g.n_slices, g.s_off);
+		k_pull_slice_width<<<grid_for(g.n_slices + 1, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(key_res, g.n_short, g.n_slices, g.s_off);
 		PGQ_CUDA(cudaGetLastError());
 		PGQ_TRY(pgq_scan_exclusive_i32(g.s_off, g.s_off, g.n_slices + 1, scan_tmp, s));
 		int32_t total = 0;
@@ -1091,7 +1116,7 @@ static int build_pull_graph(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 		PGQ_CUDA(cudaStreamSynchronize(s));
 		g.s_total = total;
 		PGQ_TRY(dev_alloc(csr, (void **)&g.s_adj, (size_t)std::max<int64_t>(g.s_total, 1) * sizeof(int32_t)));
-		k_pull_short_fill<<<grid_for(g.n_slices * 32, 256, 148 * 16), 256, 0, s>>>(csr->in.off, csr->in.adj, val_res, g.n_short,
+		k_pull_short_fill<<<grid_for(g.n_slices * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->in.off, csr->in.adj, val_res, g.n_short,
 		                                                                    g.n_slices, g.s_off, g.s_adj, g.s_row);
 		PGQ_CUDA(cudaGetLastError());
 	} else {
@@ -1125,7 +1150,7 @@ static int finish_csr(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	PGQ_TRY(pgq_ws_reserve(ws, 1, pgq_scan_tmp_elems(n + 1) * sizeof(int32_t), (void **)&scan_tmp));
 	PGQ_CUDA(cudaMemsetAsync(csr->in.off, 0, (size_t)(n + 1) * sizeof(int32_t), s));
 	if (m > 0) {
-		k_histogram<<<grid_for(m, 256, 148 * 16), 256, 0, s>>>(csr->out.adj, m, csr->in.off);
+		k_histogram<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->out.adj, m, csr->in.off);
 		PGQ_CUDA(cudaGetLastError());
 	}
 	PGQ_TRY(pgq_scan_exclusive_i32(csr->in.off, csr->in.off, n + 1, scan_tmp, s));
@@ -1137,7 +1162,7 @@ static int finish_csr(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 		while (end_bit < 31 && ((int64_t)1 << end_bit) < n) {
 			end_bit++;
 		}
-		k_edge_rows<<<grid_for(csr->out.nchunks * 32, 256, 148 * 16), 256, 0, s>>>(csr->out, m, rowid);
+		k_edge_rows<<<grid_for(csr->out.nchunks * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->out, m, rowid);
 		PGQ_CUDA(cudaGetLastError());
 		int32_t *keys_a, *keys_res, *vals_res;
 		PGQ_TRY(pgq_ws_reserve(ws, 7, (size_t)m * sizeof(int32_t), (void **)&keys_a));
@@ -1210,7 +1235,7 @@ static int upload_narrow(Workspace *ws, const int64_t *host, int64_t count, int6
 	for (int64_t o = 0; o < count; o += piece) {
 		int64_t c = std::min(piece, count - o);
 		PGQ_CUDA(cudaMemcpyAsync(tmp, host + o, (size_t)c * sizeof(int64_t), cudaMemcpyHostToDevice, s));
-		k_narrow<<<grid_for(c, 256, 148 * 8), 256, 0, s>>>(tmp, d_out + o, c, lo, hi, d_err);
+		k_narrow<<<grid_for(c, 256, (int64_t)ws->ctx->sm_count * 8), 256, 0, s>>>(tmp, d_out + o, c, lo, hi, d_err);
 		PGQ_CUDA(cudaGetLastError());
 		PGQ_CUDA(cudaStreamSynchronize(s)); // tmp is reused by the next piece
 	}
@@ -1485,13 +1510,13 @@ static int finalize_from_rows(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	PGQ_CUDA(cudaMemsetAsync(outdeg, 0, (size_t)(n + 1) * sizeof(int32_t), s));
 	PGQ_CUDA(cudaMemsetAsync(indeg, 0, (size_t)(n + 1) * sizeof(int32_t), s));
 	if (m > 0) {
-		k_histogram<<<grid_for(m, 256, 148 * 16), 256, 0, s>>>(csr->st_src, m, outdeg);
-		k_histogram<<<grid_for(m, 256, 148 * 16), 256, 0, s>>>(csr->st_dst, m, indeg);
+		k_histogram<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->st_src, m, outdeg);
+		k_histogram<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->st_dst, m, indeg);
 	}
 	// the degrees must equal the counts given to create_csr_vertex (the reference trusts them and
 	// scatters out of place otherwise)
 	if (csr->have_counts && n > 0) {
-		k_compare_i32<<<grid_for(n, 256, 148 * 8), 256, 0, s>>>(outdeg, csr->st_cnt, n, d_err);
+		k_compare_i32<<<grid_for(n, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(outdeg, csr->st_cnt, n, d_err);
 	}
 	// internal numbering: one stable sort by (class, descending degree)
 	int64_t class_size[4] = {0, 0, 0, 0};
@@ -1505,10 +1530,10 @@ static int finalize_from_rows(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 		PGQ_TRY(pgq_ws_reserve(ws, 11, (size_t)(n + 2) * sizeof(int32_t), (void **)&val_b));
 		PGQ_TRY(pgq_ws_reserve(ws, 3, 256, (void **)&d_cls));
 		PGQ_CUDA(cudaMemsetAsync(d_cls, 0, 4 * sizeof(int), s));
-		k_vertex_keys<<<grid_for(n, 256, 148 * 8), 256, 0, s>>>(outdeg, indeg, n, key_a, val_a, d_cls);
+		k_vertex_keys<<<grid_for(n, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(outdeg, indeg, n, key_a, val_a, d_cls);
 		PGQ_CUDA(cudaGetLastError());
 		PGQ_TRY(radix_sort_pairs(ws, key_a, key_b, val_a, val_b, n, 24, s, &key_res, &val_res));
-		k_invert_perm<<<grid_for(n, 256, 148 * 8), 256, 0, s>>>(val_res, n, csr->perm, csr->inv);
+		k_invert_perm<<<grid_for(n, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(val_res, n, csr->perm, csr->inv);
 		PGQ_CUDA(cudaGetLastError());
 		int h_cls[4] = {0, 0, 0, 0};
 		PGQ_CUDA(cudaMemcpyAsync(h_cls, d_cls, 4 * sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -1528,9 +1553,9 @@ static int finalize_from_rows(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	// row offsets of the internal out-CSR = CsrInitializeEdge's prefix sum (csr_creation.cpp:57-59)
 	PGQ_CUDA(cudaMemsetAsync(csr->out.off, 0, (size_t)(n + 1) * sizeof(int32_t), s));
 	if (m > 0) {
-		k_apply_perm<<<grid_for(m, 256, 148 * 16), 256, 0, s>>>(csr->st_src, m, csr->perm);
-		k_apply_perm<<<grid_for(m, 256, 148 * 16), 256, 0, s>>>(csr->st_dst, m, csr->perm);
-		k_histogram<<<grid_for(m, 256, 148 * 16), 256, 0, s>>>(csr->st_src, m, csr->out.off);
+		k_apply_perm<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->st_src, m, csr->perm);
+		k_apply_perm<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->st_dst, m, csr->perm);
+		k_histogram<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->st_src, m, csr->out.off);
 	}
 	PGQ_TRY(pgq_scan_exclusive_i32(csr->out.off, csr->out.off, n + 1, scan_tmp, s));
 	if (m > 0) {
@@ -1542,14 +1567,14 @@ static int finalize_from_rows(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 		while (end_bit < 31 && ((int64_t)1 << end_bit) < n) {
 			end_bit++;
 		}
-		k_iota<<<grid_for(m, 256, 148 * 8), 256, 0, s>>>(perm_in, m);
+		k_iota<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(perm_in, m);
 		PGQ_CUDA(cudaGetLastError());
 		// (st_src is staging and may be clobbered: the out-degree histogram above already used it)
 		PGQ_TRY(radix_sort_pairs(ws, csr->st_src, keys_out, perm_in, perm_out, m, end_bit, s, &keys_res, &perm_out));
 		if (csr->st_w) {
 			PGQ_TRY(dev_alloc(csr, (void **)&csr->w_bits, (size_t)m * sizeof(int64_t)));
 		}
-		k_gather_edges<<<grid_for(m, 256, 148 * 16), 256, 0, s>>>(perm_out, csr->st_dst, csr->st_eid, csr->st_w, m,
+		k_gather_edges<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(perm_out, csr->st_dst, csr->st_eid, csr->st_w, m,
 		                                                       csr->out.adj, csr->edge_ids, csr->w_bits);
 		PGQ_CUDA(cudaGetLastError());
 	}
@@ -1703,12 +1728,12 @@ extern "C" int pgq_csr_build_device(pgq_ctx *ctx, int64_t n, int64_t m, const in
 		if (m > 0) {
 			cudaMemcpyAsync(csr->st_src, d_src, (size_t)m * sizeof(int32_t), cudaMemcpyDeviceToDevice, s);
 			cudaMemcpyAsync(csr->st_dst, d_dst, (size_t)m * sizeof(int32_t), cudaMemcpyDeviceToDevice, s);
-			k_range_check_i32<<<grid_for(m, 256, 148 * 16), 256, 0, s>>>(csr->st_src, m, n, d_err);
-			k_range_check_i32<<<grid_for(m, 256, 148 * 16), 256, 0, s>>>(csr->st_dst, m, n, d_err);
+			k_range_check_i32<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->st_src, m, n, d_err);
+			k_range_check_i32<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->st_dst, m, n, d_err);
 			if (d_eid) {
 				cudaMemcpyAsync(csr->st_eid, d_eid, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToDevice, s);
 			} else {
-				k_iota64<<<grid_for(m, 256, 148 * 8), 256, 0, s>>>(csr->st_eid, m);
+				k_iota64<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->st_eid, m);
 			}
 		}
 		int flag = 0;
@@ -1779,11 +1804,11 @@ extern "C" int pgq_csr_upload(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t 
 			break;
 		}
 		if (m > 0) {
-			k_rows_from_offsets<<<grid_for(n * 32, 256, 148 * 16), 256, 0, s>>>(off_tmp, n, csr->st_src);
+			k_rows_from_offsets<<<grid_for(n * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(off_tmp, n, csr->st_src);
 			if (edge_ids) {
 				cudaMemcpyAsync(csr->st_eid, edge_ids, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, s);
 			} else {
-				k_iota64<<<grid_for(m, 256, 148 * 8), 256, 0, s>>>(csr->st_eid, m);
+				k_iota64<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->st_eid, m);
 			}
 		}
 		st = finalize_from_rows(csr, ws, s);
@@ -1822,10 +1847,10 @@ extern "C" int pgq_csr_download(pgq_csr *csr, int64_t *v_out, int64_t *e_out, in
 		tmp_id = nullptr;
 		if (edge_ids_out &&
 		    (st = pgq_ws_reserve(ws, 5, (size_t)std::max<int64_t>(m, 1) * sizeof(int64_t), (void **)&tmp_id)) != PGQ_OK) break;
-		k_orig_degrees<<<grid_for(n + 1, 256, 148 * 8), 256, 0, s>>>(csr->out.off, csr->perm, n, orig_off);
+		k_orig_degrees<<<grid_for(n + 1, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->out.off, csr->perm, n, orig_off);
 		if ((st = pgq_scan_exclusive_i32(orig_off, orig_off, n + 1, scan_tmp, s)) != PGQ_OK) break;
 		if (m > 0 && (e_out || edge_ids_out)) {
-			k_orig_rows<<<grid_for(n * 32, 256, 148 * 16), 256, 0, s>>>(csr->out.off, csr->out.adj, csr->edge_ids, csr->perm,
+			k_orig_rows<<<grid_for(n * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->out.off, csr->out.adj, csr->edge_ids, csr->perm,
 			                                                       csr->inv, orig_off, n, e_out ? tmp_e : nullptr,
 			                                                       edge_ids_out ? tmp_id : nullptr);
 			if (e_out) {
@@ -1837,7 +1862,7 @@ extern "C" int pgq_csr_download(pgq_csr *csr, int64_t *v_out, int64_t *e_out, in
 			cudaStreamSynchronize(s);
 		}
 		if (v_out) {
-			k_widen<<<grid_for(n + 1, 256, 148 * 8), 256, 0, s>>>(orig_off, tmp_e, n + 1);
+			k_widen<<<grid_for(n + 1, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(orig_off, tmp_e, n + 1);
 			cudaMemcpyAsync(v_out, tmp_e, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
 			cudaStreamSynchronize(s);
 			v_out[n + 1] = v_out[n]; // the reference's padding slot
@@ -1900,10 +1925,10 @@ extern "C" int pgq_csr_download_weights(pgq_csr *csr, void *w_out) {
 		if ((st = pgq_ws_reserve(ws, 0, (size_t)(n + 2) * sizeof(int32_t), (void **)&orig_off)) != PGQ_OK) break;
 		if ((st = pgq_ws_reserve(ws, 1, pgq_scan_tmp_elems(n + 1) * sizeof(int32_t), (void **)&scan_tmp)) != PGQ_OK) break;
 		if ((st = pgq_ws_reserve(ws, 5, (size_t)std::max<int64_t>(m, 1) * sizeof(int64_t), (void **)&tmp_w)) != PGQ_OK) break;
-		k_orig_degrees<<<grid_for(n + 1, 256, 148 * 8), 256, 0, s>>>(csr->out.off, csr->perm, n, orig_off);
+		k_orig_degrees<<<grid_for(n + 1, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->out.off, csr->perm, n, orig_off);
 		if ((st = pgq_scan_exclusive_i32(orig_off, orig_off, n + 1, scan_tmp, s)) != PGQ_OK) break;
 		if (m > 0) {
-			k_orig_rows<<<grid_for(n * 32, 256, 148 * 16), 256, 0, s>>>(csr->out.off, csr->out.adj, csr->w_bits, csr->perm,
+			k_orig_rows<<<grid_for(n * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->out.off, csr->out.adj, csr->w_bits, csr->perm,
 			                                                       csr->inv, orig_off, n, nullptr, tmp_w);
 			cudaMemcpyAsync(w_out, tmp_w, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
 		}

@@ -80,6 +80,7 @@ struct PullGraph {
 #define PGQ_WS_SLOTS 32
 // Scratch of one path-function call (mask arrays etc.), pooled per context and grown on demand.
 struct Workspace {
+	pgq_ctx *ctx = nullptr; // the context whose pool it belongs to
 	void *buf[PGQ_WS_SLOTS] = {};
 	size_t cap[PGQ_WS_SLOTS] = {};
 	cudaStream_t stream = nullptr; // owned stream for host-pointer calls
@@ -98,7 +99,7 @@ struct Workspace {
 
 struct pgq_ctx {
 	int device = 0;
-	int sm_count = 148;
+	int sm_count = 132; // H100 SXM; set from the device properties by pgq_ctx_create
 	std::mutex mu;
 	std::condition_variable cv;
 	std::vector<Workspace *> free_ws;

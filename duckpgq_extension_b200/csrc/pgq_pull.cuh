@@ -89,9 +89,7 @@ __device__ __forceinline__ void ld_mask_rw(const u64 *base, int64_t idx, u64 (&m
 	} else {
 #pragma unroll
 		for (int i = 0; i < W; i += 4) {
-			asm volatile("ld.global.v4.u64 {%0,%1,%2,%3}, [%4];"
-			             : "=l"(m[i]), "=l"(m[i + 1]), "=l"(m[i + 2]), "=l"(m[i + 3])
-			             : "l"(p + i));
+			PGQ_LD4("", p + i, m[i], m[i + 1], m[i + 2], m[i + 3]);
 		}
 	}
 }
@@ -104,25 +102,30 @@ __device__ __forceinline__ void ld_mask_hint(const u64 *__restrict__ base, int64
 	const u64 *p = base + idx * W;
 	if constexpr (W == 4 && HINT == 1) {
 		if (hot) {
-			asm volatile("ld.global.nc.L1::evict_last.v4.u64 {%0,%1,%2,%3}, [%4];"
-			             : "=l"(m[0]), "=l"(m[1]), "=l"(m[2]), "=l"(m[3])
-			             : "l"(p));
+			PGQ_LD4(".nc.L1::evict_last", p, m[0], m[1], m[2], m[3]);
 		} else {
-			asm volatile("ld.global.nc.L1::no_allocate.v4.u64 {%0,%1,%2,%3}, [%4];"
-			             : "=l"(m[0]), "=l"(m[1]), "=l"(m[2]), "=l"(m[3])
-			             : "l"(p));
+			PGQ_LD4(".nc.L1::no_allocate", p, m[0], m[1], m[2], m[3]);
 		}
-	} else if constexpr (W >= 4 && HINT == 2) { // (experiment: L2 eviction priorities on top, 256-bit loads only)
+	} else if constexpr (W >= 4 && HINT == 2) { // (experiment: L2 eviction priorities on top, 32 B masks and wider only)
+		// sm_90 takes an L2 eviction priority only as a cache policy (createpolicy) handed to the load
+		u64 pol;
+		if (hot) {
+			asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+		} else {
+			asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+		}
 #pragma unroll
 		for (int i = 0; i < W; i += 4) {
 			if (hot) {
-				asm volatile("ld.global.nc.L1::evict_last.L2::evict_last.v4.b64 {%0,%1,%2,%3}, [%4];"
-				             : "=l"(m[i]), "=l"(m[i + 1]), "=l"(m[i + 2]), "=l"(m[i + 3])
-				             : "l"(p + i));
+				asm volatile("ld.global.nc.L1::evict_last.L2::cache_hint.v2.u64 {%0,%1}, [%4], %5;\n\t"
+				             "ld.global.nc.L1::evict_last.L2::cache_hint.v2.u64 {%2,%3}, [%4+16], %5;"
+				             : "=&l"(m[i]), "=&l"(m[i + 1]), "=&l"(m[i + 2]), "=&l"(m[i + 3])
+				             : "l"(p + i), "l"(pol));
 			} else {
-				asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v4.b64 {%0,%1,%2,%3}, [%4];"
-				             : "=l"(m[i]), "=l"(m[i + 1]), "=l"(m[i + 2]), "=l"(m[i + 3])
-				             : "l"(p + i));
+				asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%0,%1}, [%4], %5;\n\t"
+				             "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%2,%3}, [%4+16], %5;"
+				             : "=&l"(m[i]), "=&l"(m[i + 1]), "=&l"(m[i + 2]), "=&l"(m[i + 3])
+				             : "l"(p + i), "l"(pol));
 			}
 		}
 	} else if constexpr (HINT == 3) { // hub masks staged in shared memory (k_pull_fused_hub), all others bypass L1
@@ -146,9 +149,7 @@ __device__ __forceinline__ void ld_mask_hint(const u64 *__restrict__ base, int64
 		} else {
 #pragma unroll
 			for (int i = 0; i < W; i += 4) {
-				asm volatile("ld.global.nc.L1::no_allocate.v4.u64 {%0,%1,%2,%3}, [%4];"
-				             : "=l"(m[i]), "=l"(m[i + 1]), "=l"(m[i + 2]), "=l"(m[i + 3])
-				             : "l"(p + i));
+				PGQ_LD4(".nc.L1::no_allocate", p + i, m[i], m[i + 1], m[i + 2], m[i + 3]);
 			}
 		}
 	} else {

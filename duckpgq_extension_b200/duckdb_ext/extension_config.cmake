@@ -1,4 +1,4 @@
-# DuckDB extension list for the combined build: the UNMODIFIED reference first, then the B200
+# DuckDB extension list for the combined build: the UNMODIFIED reference first, then the GPU
 # override (LoadAllExtensions loads in list order, duckdb/extension/generated_extension_loader.cpp.in:14-26).
 if(NOT DEFINED PGQ_REFERENCE_DIR)
   set(PGQ_REFERENCE_DIR "/root/reference")

@@ -1,4 +1,4 @@
-// duckpgq_b200 -- the DuckDB-side shim of the B200 path-finding hot path.
+// duckpgq_b200 -- the DuckDB-side shim of the H100 path-finding hot path.
 //
 // Loaded after the unmodified `duckpgq` extension, it re-registers -- same names, same argument types,
 // so ExtensionLoader::RegisterFunction (ALTER_ON_CONFLICT) replaces the CPU callbacks -- the scalar

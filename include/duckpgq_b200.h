@@ -1,5 +1,5 @@
 /*
- * duckpgq_b200.h -- C ABI of the B200-native path-finding hot path of DuckPGQ.
+ * duckpgq_b200.h -- C ABI of the H100-native (sm_90a) path-finding hot path of DuckPGQ.
  *
  * This is the drop-in boundary: the shared library libduckpgq_b200.so exports exactly these
  * symbols (plain pointers + sizes, caller-owned buffers, int status codes, no C++/torch types,

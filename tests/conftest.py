@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: the library is built for sm_90a)")
 
 
 def _cuda_device_count() -> int:
@@ -32,7 +32,7 @@ def pytest_collection_modifyitems(config, items):
     (`-m gpu` / `-m "not gpu"` select as before)."""
     if _cuda_device_count() > 0:
         return
-    skip = pytest.mark.skip(reason="no CUDA device visible: gpu-marked tests run on the B200 box")
+    skip = pytest.mark.skip(reason="no CUDA device visible: gpu-marked tests need an H100")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -1,6 +1,6 @@
 """bench.py's reference arm on CPU (small graph): the JSON line carries every key the bench contract names,
-and only rank 0 prints under a multi-rank launch.  (The GPU arm needs a B200; its line is checked by the
-driver.)  Uses oracle/_ref when it is built, else the C restatement -- both are allowed for this arm."""
+and only rank 0 prints under a multi-rank launch.  (The GPU arm needs an H100; its line is checked by
+running bench.py there.)  Uses oracle/_ref when it is built, else the C restatement -- both are allowed for this arm."""
 import json
 import os
 import subprocess
@@ -35,3 +35,21 @@ def test_reference_arm_line():
 
 def test_reference_arm_other_ranks_stay_silent():
     assert run_bench({"RANK": "1", "LOCAL_RANK": "1", "WORLD_SIZE": "2"}) == ""
+
+
+def test_dump_outputs_files_and_dtypes(tmp_path):
+    import numpy as np
+    import bench
+    lengths = np.array([0, 3, -1, 7], dtype=np.int64)
+    valid = np.array([1, 1, 0, 1], dtype=np.uint8)
+    bench.dump_outputs(str(tmp_path / "out"), {"lengths": lengths, "valid": valid})
+    assert sorted(os.listdir(tmp_path / "out")) == ["lengths.npy", "valid.npy"]
+    for name, a in (("lengths", lengths), ("valid", valid)):
+        got = np.load(tmp_path / "out" / f"{name}.npy")
+        assert got.dtype == np.float64 and np.array_equal(got, a)
+
+
+def test_dump_outputs_is_refused_by_the_reference_arm(tmp_path):
+    out = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--dump-outputs",
+                          str(tmp_path / "d")], capture_output=True, text=True, timeout=120, cwd=ROOT)
+    assert out.returncode != 0 and "--dump-outputs" in out.stderr and not (tmp_path / "d").exists()

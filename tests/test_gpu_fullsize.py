@@ -26,7 +26,7 @@ def check_paths_valid(v, e, ids, ps, pd, paths, lengths, valid):
 
 
 def test_c2_rmat22_1024_pairs(gpu_ctx):
-    """configs[1]: RMAT scale-22 (4M v / 64M e), 1024 hashed pairs, 1 x B200."""
+    """configs[1]: RMAT scale-22 (4M v / 64M e), 1024 hashed pairs, 1 x H100."""
     n, src, dst = datagen.rmat_edges_cached(22)
     csr = pgq.DeviceCSR.build(gpu_ctx, n, src, dst)
     ps, pd = datagen.hashed_pairs(1024, n)

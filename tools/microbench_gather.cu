@@ -1,9 +1,9 @@
-// Micro-benchmark (development aid): cost of random sector gathers through the LSU on B200.
-//   A: one lane reads one 32 B record with LDG.256           (32 records / warp instruction)
+// Micro-benchmark (development aid): cost of random sector gathers through the LSU on H100.
+//   A: one lane reads one 32 B record with two LDG.128 back to back (the mask loads of csrc/; sm_90 has no LDG.256)
 //   B: two adjacent lanes read the halves of one 32 B record  (16 records / warp instruction, LDG.128)
 //   C: one lane reads one 16 B record with LDG.128
 //   D: one lane reads one  8 B record with LDG.64
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/mb tools/microbench_gather.cu && /tmp/mb
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/mb tools/microbench_gather.cu && /tmp/mb
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -26,7 +26,8 @@ __global__ void __launch_bounds__(256) k(const u64 *__restrict__ tab, const uint
 			uint32_t r = idx[i] & mask;
 			if (MODE == 0) {
 				u64 a, b, c, d;
-				asm volatile("ld.global.nc.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(tab + (int64_t)r * 4));
+				asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%4];\n\tld.global.nc.v2.u64 {%2,%3}, [%4+16];"
+				             : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(tab + (int64_t)r * 4));
 				acc |= a ^ b ^ c ^ d;
 			} else if (MODE == 2) {
 				const ulonglong2 v = __ldg(reinterpret_cast<const ulonglong2 *>(tab + (int64_t)r * 2));
@@ -49,17 +50,17 @@ int main() {
 		size_t bytes = (size_t)mb << 20;
 		cudaMalloc(&tab, bytes); cudaMemset(tab, 1, bytes);
 		cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
-		const char *names[4] = {"A LDG.256 32B/lane", "B 2 lanes x LDG.128 (32B rec)", "C LDG.128 16B/lane", "D LDG.64 8B/lane"};
+		const char *names[4] = {"A 2 x LDG.128 32B/lane", "B 2 lanes x LDG.128 (32B rec)", "C LDG.128 16B/lane", "D LDG.64 8B/lane"};
 		for (int mode = 0; mode < 4; mode++) {
 			uint32_t recbytes = mode <= 1 ? 32 : (mode == 2 ? 16 : 8);
 			uint32_t mask = (uint32_t)(bytes / recbytes) - 1;
 			float best = 1e9;
 			for (int rep = 0; rep < 5; rep++) {
 				cudaEventRecord(a);
-				if (mode == 0) k<0><<<148 * 8, 256>>>(tab, idx, n, mask, out);
-				if (mode == 1) k<1><<<148 * 8, 256>>>(tab, idx, n, mask, out);
-				if (mode == 2) k<2><<<148 * 8, 256>>>(tab, idx, n, mask, out);
-				if (mode == 3) k<3><<<148 * 8, 256>>>(tab, idx, n, mask, out);
+				if (mode == 0) k<0><<<132 * 8, 256>>>(tab, idx, n, mask, out);
+				if (mode == 1) k<1><<<132 * 8, 256>>>(tab, idx, n, mask, out);
+				if (mode == 2) k<2><<<132 * 8, 256>>>(tab, idx, n, mask, out);
+				if (mode == 3) k<3><<<132 * 8, 256>>>(tab, idx, n, mask, out);
 				cudaEventRecord(b); cudaEventSynchronize(b);
 				float ms; cudaEventElapsedTime(&ms, a, b); if (ms < best) best = ms;
 			}
