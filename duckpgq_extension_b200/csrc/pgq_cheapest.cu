@@ -2,12 +2,21 @@
 // cheapest_path_length.cpp:12-136 (TemplatedBatchBellmanFord: one lane per row, all lanes of an edge
 // relaxed together, sweeps until nothing changes).  sm_90a only.
 //
-// The reference relaxes in place, sequentially, in CSR order; the distances it ends with are the least
-// fixed point of  d[n] = min(d[n], d[v] + w(v,n))  -- for int64 exactly, for double because fl(a + w)
-// is monotone in a -- and do not depend on the relaxation order.  The device relaxes in parallel with
-// atomicMin and re-sweeps only the vertices whose distances improved, to the same fixed point,
-// bit for bit.  "Unreachable" is the reference's own sentinel max/2 (l.15), added to like any other
-// number (no guard, as UpdateOneLane l.29-36 has none).
+// The reference relaxes in place, sequentially, in CSR order, from EVERY vertex, reached or not; the
+// distances it ends with are the greatest fixed point of  d[n] = min(d[n], d[v] + w(v,n))  below its start
+// values -- for int64 exactly, for double because fl(a + w) is monotone in a -- and do not depend on the
+// relaxation order.  The device relaxes in parallel with atomicMin and sweeps only the dirty vertices,
+// those whose distance in some lane changed since they were last relaxed, to the same fixed point, bit
+// for bit.  "Unreachable" is the reference's own sentinel max/2 (l.15), added to like any other number
+// (no guard, as UpdateOneLane l.29-36 has none), so a weight below zero can improve on it: an unreached
+// vertex relaxes max/2 + w into its neighbour, which then holds a valid, huge cost (BIGINT: any w < 0;
+// DOUBLE: -inf, or w below about -1.5e292).  A batch therefore starts with only its sources dirty when
+// every weight is >= 0, and with every vertex dirty when some weight is below zero (pgq_csr::neg_weights,
+// found when the CSR is finalized): the first sweep then relaxes from the unreached vertices as the
+// reference does, and a row's result does not depend on the other rows of its batch.
+// A NaN sum is never better (new_dist < n_dist is false), so an edge of NaN weight never relaxes; without
+// that test a NaN with the sign bit set would win every atomicMin.  A negative cycle anywhere in the graph,
+// reachable or not, keeps improving for ~2^62 sweeps here as in the reference: there is no cap.
 #include <algorithm>
 #include <cstring>
 
@@ -78,15 +87,18 @@ __global__ void __launch_bounds__(256) k_bf_sweep(int64_t n, int L, const int32_
 			for (int e = e0; e < e1; e++) {
 				const int u = adj[e];
 				u64 nk;
+				bool is_nan = false;
 				if (F64) {
-					nk = f64_key(key_f64(dk) + __longlong_as_double(w_bits[e]));
+					const double c = key_f64(dk) + __longlong_as_double(w_bits[e]);
+					is_nan = c != c; // new_dist < n_dist is false for a NaN (UpdateOneLane l.31)
+					nk = f64_key(c);
 				} else {
 					nk = (u64)((long long)dk + w_bits[e]);
 				}
 				u64 *slot = &dist[(int64_t)u * L + g + lane];
 				bool better;
 				if (F64) {
-					better = nk < *reinterpret_cast<volatile u64 *>(slot) && nk < atomicMin(slot, nk);
+					better = !is_nan && nk < *reinterpret_cast<volatile u64 *>(slot) && nk < atomicMin(slot, nk);
 				} else {
 					better = (long long)nk < *reinterpret_cast<volatile long long *>(slot) &&
 					         (long long)nk < atomicMin(reinterpret_cast<long long *>(slot), (long long)nk);
@@ -164,7 +176,8 @@ static int run_bf(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, 
 		const int cnt = (int)std::min<int64_t>(L, p - b0);
 		k_bf_init<F64><<<(unsigned)std::min<int64_t>((dist_elems + 255) / 256, (int64_t)sms * 16), 256, 0, s>>>(
 		    (int64_t)dist_elems, dist);
-		PGQ_CUDA(cudaMemsetAsync(dirty, 0, dirty_bytes, s));
+		// a weight below zero can improve on max/2: then the first sweep relaxes from every vertex (see the top)
+		PGQ_CUDA(cudaMemsetAsync(dirty, csr->neg_weights ? 0xff : 0, dirty_bytes, s));
 		k_bf_sources<F64><<<(cnt + 127) / 128, 128, 0, s>>>((int)b0, cnt, L, d_src, d_sv, csr->perm, n, dist, dirty,
 		                                                   flags + 1);
 		st->batches++;

@@ -635,6 +635,17 @@ __global__ void k_gather_edges(const int32_t *__restrict__ perm, const int32_t *
 	}
 }
 
+// flag = 1 if some weight is below zero; BIGINT or DOUBLE bits (-0.0 and NaNs of either sign are not below zero)
+__global__ void k_any_negative_weight(const int64_t *__restrict__ w, int64_t count, bool f64, int *flag) {
+	bool neg = false;
+	for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
+		neg |= f64 ? __longlong_as_double(w[i]) < 0.0 : w[i] < 0;
+	}
+	if (neg) {
+		*flag = 1;
+	}
+}
+
 // offsets must be non-decreasing, start at 0 and end at m
 __global__ void k_check_offsets(const int32_t *__restrict__ off, int64_t n, int64_t m, int *err) {
 	for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -1577,6 +1588,16 @@ static int finalize_from_rows(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 		k_gather_edges<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(perm_out, csr->st_dst, csr->st_eid, csr->st_w, m,
 		                                                       csr->out.adj, csr->edge_ids, csr->w_bits);
 		PGQ_CUDA(cudaGetLastError());
+		if (csr->w_bits) {
+			int *d_neg, neg = 0;
+			PGQ_TRY(pgq_ws_reserve(ws, 3, 256, (void **)&d_neg));
+			PGQ_CUDA(cudaMemsetAsync(d_neg, 0, sizeof(int), s));
+			k_any_negative_weight<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->w_bits, m,
+			                                                                                     csr->weight_type == 2, d_neg);
+			PGQ_CUDA(cudaGetLastError());
+			PGQ_TRY(read_flag(d_neg, s, &neg));
+			csr->neg_weights = neg != 0;
+		}
 	}
 	PGQ_TRY(finish_csr(csr, ws, s));
 	PGQ_CUDA(cudaStreamSynchronize(s));

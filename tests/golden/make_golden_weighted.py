@@ -140,6 +140,45 @@ def main():
     src = np.concatenate([np.arange(0, 149), rng.integers(0, 150, 40)])
     dst = np.concatenate([np.arange(1, 150), rng.integers(0, 150, 40)])
     save("chain150_f64", n, src, dst, rng.random(len(src)) + 0.5, rng.integers(0, n, 200), rng.integers(0, n, 200))
+    # negative BIGINT weights on a DAG (no cycle can form: every edge runs from a lower to a higher rank of a random
+    # permutation).  The reference relaxes from unreached vertices too, so a target that only an unreached vertex
+    # reaches at a negative cost gets max/2 + that cost, a valid result; half of the pairs start at low ranks so
+    # that many targets are reachable from their source as well
+    n = 400
+    src, dst, rank = dag_edges(rng, n, 1200)
+    ps, pd = dag_pairs(rng, rank, 300)
+    save("dagneg_i64", n, src, dst, rng.integers(-50, 51, len(src)), ps, pd)
+    # dyadic doubles k/1024 (every path sum is exact), plus one -1e300 edge out of a vertex without in-edges: every
+    # row whose target that edge reaches ends near 8.99e307 instead of NULL
+    n = 300
+    src, dst, rank = dag_edges(rng, n, 900)
+    w = rng.integers(-(1 << 20) + 1, 1 << 20, len(src)) / 1024.0
+    tail = int(np.argmin(rank))
+    head = int(np.argsort(rank)[n // 10])
+    src, dst, w = np.append(src, tail), np.append(dst, head), np.append(w, -1e300)
+    ps, pd = dag_pairs(rng, rank, 300)
+    save("dagdyadic_f64", n, src, dst, w, ps, pd)
+
+
+def dag_edges(rng, n, m):
+    """m random edges (plus a tenth as parallel twins), each oriented from the lower to the higher rank of a random
+    permutation, self-loops dropped: a DAG, so negative weights cannot form a negative cycle."""
+    rank = rng.permutation(n)
+    a, b = rng.integers(0, n, m), rng.integers(0, n, m)
+    a, b = a[a != b], b[a != b]
+    fwd = rank[a] < rank[b]
+    src, dst = np.where(fwd, a, b), np.where(fwd, b, a)
+    twin = rng.integers(0, len(src), len(src) // 10)
+    return np.concatenate([src, src[twin]]), np.concatenate([dst, dst[twin]]), rank
+
+
+def dag_pairs(rng, rank, p):
+    """p pairs: the first half uniform, the second half from the lowest quarter of the ranks to the highest half."""
+    n = len(rank)
+    by_rank = np.argsort(rank)
+    h = p // 2
+    return (np.concatenate([rng.integers(0, n, h), by_rank[rng.integers(0, n // 4, p - h)]]),
+            np.concatenate([rng.integers(0, n, h), by_rank[rng.integers(n // 2, n, p - h)]]))
 
 
 if __name__ == "__main__":
