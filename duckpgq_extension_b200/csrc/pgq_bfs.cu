@@ -1816,7 +1816,15 @@ static int run_batch(Run &r, const CallCtx &cc, LevelStatus *d_st, LevelStatus *
 	if (r.seq == 0) {
 		*reinterpret_cast<volatile int *>(&h_st->seq) = 0; // forget whatever an earlier call left behind
 	}
-	const int direction = opts ? opts->direction : 0;
+	// PGQ_B200_SCHEDULE (tests): the kind of every level, whatever the heuristic would pick.  Character (iter - 1) % len
+	// decides level iter: b bottom-up (top-down on an edgeless graph), p top-down, t k_tail where it is eligible
+	// (top-down otherwise), a the heuristic.  Overrides opts->direction.
+	const char *schedule = getenv("PGQ_B200_SCHEDULE");
+	const size_t sched_len = schedule ? strlen(schedule) : 0;
+	if (schedule && strspn(schedule, "bpta") != sched_len) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "PGQ_B200_SCHEDULE may only hold the characters b, p, t and a");
+	}
+	const int direction = sched_len ? 0 : (opts ? opts->direction : 0);
 	const int64_t alpha = (opts && opts->alpha > 0) ? opts->alpha : 5; // a pushed edge costs ~5x a pulled one (measured)
 	const int64_t wide_grid = (int64_t)r.sms * 8;
 	const int pull_variant = getenv("PGQ_B200_PULL") ? atoi(getenv("PGQ_B200_PULL")) : 0;
@@ -1891,10 +1899,16 @@ static int run_batch(Run &r, const CallCtx &cc, LevelStatus *d_st, LevelStatus *
 	int batch_pulls = 0;     // fused bottom-up levels this batch has run
 	int64_t pull_cost = m;   // gathers the next bottom-up level costs at most: what the last one issued
 	int iter = 1;
+	// Path mode records the level that discovers a vertex in a uint16 array (0xFFFF = unvisited) and supports depths up
+	// to 0xFFFD.  A level 0xFFFE still runs: with reference batching a batch ends only at the level that finds its
+	// frontier empty, and that level records nothing.  If it finds vertices, the call fails (checked after each level).
+	const auto too_deep = [&]() {
+		return PATH && iter >= 0xFFFE && h_st->pub_vertices > 0
+		           ? pgq_fail(PGQ_ERR_UNSUPPORTED, "BFS deeper than 65533 levels is not supported in path mode")
+		           : PGQ_OK;
+	};
 	for (;; iter++) {
-		if (PATH && iter >= 0xFFFE) {
-			return pgq_fail(PGQ_ERR_UNSUPPORTED, "BFS deeper than 65533 levels is not supported in path mode");
-		}
+		const char forced = sched_len ? schedule[(size_t)(iter - 1) % sched_len] : 'a';
 		const int64_t fe = (int64_t)h_st->pub_edges;
 		const int64_t fv = (int64_t)h_st->pub_vertices;
 		// without an item list its length is bounded by one item per vertex + one per 256 edges
@@ -1905,9 +1919,16 @@ static int run_batch(Run &r, const CallCtx &cc, LevelStatus *d_st, LevelStatus *
 		// a tiny frontier is expanded by k_tail whatever the direction heuristic says (on a tiny GRAPH
 		// every frontier is "large" relative to m, yet three launches + a round trip per level cost
 		// far more than the work)
-		const bool tail = use_tail && direction != 2 && n_items <= PGQ_TAIL_ITEMS && fe <= PGQ_TAIL_EDGES;
-		// (finished rows and early exits only ever grow: the gathers of the last bottom-up level bound the next one's)
-		const bool pull = !tail && m > 0 && ((direction == 2) || (direction == 0 && fe * alpha > pull_cost));
+		const bool tail_fits = use_tail && n_items <= PGQ_TAIL_ITEMS && fe <= PGQ_TAIL_EDGES;
+		bool tail, pull;
+		if (forced == 'a') {
+			tail = tail_fits && direction != 2;
+			// (finished rows and early exits only ever grow: the gathers of the last bottom-up level bound the next one's)
+			pull = !tail && m > 0 && ((direction == 2) || (direction == 0 && fe * alpha > pull_cost));
+		} else {
+			tail = forced == 't' && tail_fits;
+			pull = forced == 'b' && m > 0;
+		}
 		if (!pull && !items_valid) {
 			// top-down after bottom-up: build the frontier's item list from its masks, clean the other array
 			k_frontier_items<W><<<upd_grid, 256, 0, s>>>(n_reach, visit, cand, csr->out.off, items, d_st, hd_st, ++r.seq);
@@ -1927,7 +1948,14 @@ static int run_batch(Run &r, const CallCtx &cc, LevelStatus *d_st, LevelStatus *
 		if (tail) {
 			int max_levels = PGQ_TAIL_MAX;
 			if (PATH) {
-				max_levels = std::min(max_levels, 0xFFFE - iter); // >= 1: iter < 0xFFFE was checked above
+				max_levels = std::min(max_levels, 0xFFFF - iter); // >= 1: no level after 0xFFFE runs (too_deep)
+			}
+			if (sched_len) { // not into a level the schedule gives to b or p
+				int run = 1;
+				while (run < max_levels && strchr("ta", schedule[(size_t)(iter - 1 + run) % sched_len])) {
+					run++;
+				}
+				max_levels = run;
 			}
 			k_tail<W, PATH><<<1, 1024, 0, s>>>(csr->out.off, csr->out.adj, seen, visit, cand, items, items_next, n_items,
 			                                  tlist, tbits, level, d_st, active, max_levels, chk);
@@ -1951,6 +1979,7 @@ static int run_batch(Run &r, const CallCtx &cc, LevelStatus *d_st, LevelStatus *
 			}
 			iter += done - 1;
 			saturated += h_st->pub_sat;
+			PGQ_TRY(too_deep());
 			if (h_st->pub_vertices == 0) {
 				break;
 			}
@@ -2050,6 +2079,7 @@ static int run_batch(Run &r, const CallCtx &cc, LevelStatus *d_st, LevelStatus *
 				pull_cost = (int64_t)h_st->pub_gathers + m / 256 + 1;
 			}
 		}
+		PGQ_TRY(too_deep());
 		if (h_st->pub_vertices == 0) { // no change, iterativelength.cpp:115-117
 			break;
 		}
