@@ -76,23 +76,36 @@ struct LevelStatus {
 // The host decides the next kernel from the frontier statistics of the finished level.  Instead of a
 // D2H copy + stream synchronisation per level, the last thread of a level writes the few numbers
 // straight into pinned, device-mapped host memory and then bumps a sequence number the host spins on.
-__device__ __forceinline__ void publish_to_host(LevelStatus *host_st, const LevelStatus *st, int seq, int tail_levels) {
-	host_st->pub_vertices = st->pub_vertices;
-	host_st->pub_edges = st->pub_edges;
-	host_st->pub_items = st->pub_items;
-	host_st->pub_remaining = st->pub_remaining;
-	host_st->pub_sat = st->pub_sat;
-	host_st->pub_gathers = st->pub_gathers;
+__device__ __forceinline__ void signal_host(LevelStatus *host_st, int seq) {
+	__threadfence_system();
+	*reinterpret_cast<volatile int *>(&host_st->seq) = seq;
+}
+
+// The fields the host reads after every level; the caller then publishes them with signal_host.
+__device__ __forceinline__ void publish_fields(LevelStatus *host_st, u64 vertices, u64 edges, int items, int remaining,
+                                               int sat, u64 gathers, const u64 (&live)[8], int tail_levels) {
+	host_st->pub_vertices = vertices;
+	host_st->pub_edges = edges;
+	host_st->pub_items = items;
+	host_st->pub_remaining = remaining;
+	host_st->pub_sat = sat;
+	host_st->pub_gathers = gathers;
 	host_st->tail_levels = tail_levels;
+#pragma unroll
 	for (int i = 0; i < 8; i++) {
-		host_st->pub_live[i] = st->pub_live[i];
+		host_st->pub_live[i] = live[i];
 	}
+}
+
+// publish_fields from the pub_* fields of the device copy (+ the per-level counts of a k_tail launch)
+__device__ __forceinline__ void publish_to_host(LevelStatus *host_st, const LevelStatus *st, int seq, int tail_levels) {
+	publish_fields(host_st, st->pub_vertices, st->pub_edges, st->pub_items, st->pub_remaining, st->pub_sat,
+	               st->pub_gathers, st->pub_live, tail_levels);
 	for (int i = 0; i < tail_levels; i++) {
 		host_st->tail_fv[i] = st->tail_fv[i];
 		host_st->tail_fe[i] = st->tail_fe[i];
 	}
-	__threadfence_system();
-	*reinterpret_cast<volatile int *>(&host_st->seq) = seq;
+	signal_host(host_st, seq);
 }
 
 // ---- mask loads: one vertex mask = 8*W bytes; W = 4 is exactly one 32 B sector ----------------------
@@ -709,36 +722,72 @@ __device__ __forceinline__ void finish_level(LevelStatus *st, const u64 *seen, c
 	}
 	__threadfence();
 	const int batch_n = st->batch_n;
-	for (int j = threadIdx.x; j < batch_n; j += blockDim.x) {
-		const int row = a.batch_rows[j];
-		const int l = a.lm.row_lane[row] - a.b0;
-		const int64_t d = a.lm.pdst[row];
-		const bool found = (__ldcg(&seen[d * W + (l >> 6)]) >> (l & 63)) & 1ull;
-		if (PATH) {
-			if (!found) {
-				atomicAdd(&s_remaining, 1);
+	// R rows per thread and round, their loads issued side by side: one block walks all rows of the batch (up to 1024
+	// at 256 threads), and each row is a chain of three dependent loads
+	constexpr int R = 4;
+	for (int j0 = threadIdx.x; j0 < batch_n; j0 += R * blockDim.x) {
+		int row[R];
+		bool found[R], answered[R];
+#pragma unroll
+		for (int r = 0; r < R; r++) {
+			const int j = j0 + r * blockDim.x;
+			row[r] = j < batch_n ? a.batch_rows[j] : -1;
+		}
+#pragma unroll
+		for (int r = 0; r < R; r++) {
+			found[r] = false;
+			answered[r] = true;
+			if (row[r] >= 0) {
+				const int l = a.lm.row_lane[row[r]] - a.b0;
+				const int64_t d = a.lm.pdst[row[r]];
+				found[r] = (__ldcg(&seen[d * W + (l >> 6)]) >> (l & 63)) & 1ull;
+				if (!PATH) {
+					answered[r] = *reinterpret_cast<volatile uint8_t *>(a.out_valid + row[r]);
+				}
 			}
-		} else if (!*reinterpret_cast<volatile uint8_t *>(a.out_valid + row)) {
-			if (found) {
-				a.out_len[row] = a.iter;
-				a.out_valid[row] = 1;
-			} else {
-				atomicAdd(&s_remaining, 1);
+		}
+#pragma unroll
+		for (int r = 0; r < R; r++) {
+			if (row[r] < 0) {
+				continue;
+			}
+			if (PATH) {
+				if (!found[r]) {
+					atomicAdd(&s_remaining, 1);
+				}
+			} else if (!answered[r]) {
+				if (found[r]) {
+					a.out_len[row[r]] = a.iter;
+					a.out_valid[row[r]] = 1;
+				} else {
+					atomicAdd(&s_remaining, 1);
+				}
 			}
 		}
 	}
 	__syncthreads();
 	if (threadIdx.x == 0) {
-		st->pub_vertices = atomicAdd(&st->acc_vertices, 0ull);
-		st->pub_edges = atomicAdd(&st->acc_edges, 0ull);
-		st->pub_items = atomicAdd(&st->acc_items, 0);
-		st->pub_sat = atomicAdd(&st->acc_sat, 0);
-		st->pub_remaining = s_remaining;
+		// Every block took its ticket behind a fence after its last accumulator update, so L2 loads see the sums.  The
+		// loads are issued side by side, and the values go to the host from registers: one atomic read per field, each
+		// waiting for the store before it, made this single thread a chain of some twenty memory round trips per level.
+		const u64 fv = __ldcg(&st->acc_vertices), fe = __ldcg(&st->acc_edges), gathers = __ldcg(&st->acc_gathers);
+		const int items = __ldcg(&st->acc_items), sat = __ldcg(&st->acc_sat);
+		u64 live[8];
+#pragma unroll
 		for (int i = 0; i < 8; i++) {
-			st->pub_live[i] = atomicAdd(&st->acc_live[i], 0ull);
+			live[i] = __ldcg(&st->acc_live[i]);
+		}
+		st->pub_vertices = fv;
+		st->pub_edges = fe;
+		st->pub_items = items;
+		st->pub_sat = sat;
+		st->pub_remaining = s_remaining;
+		st->pub_gathers = gathers;
+#pragma unroll
+		for (int i = 0; i < 8; i++) {
+			st->pub_live[i] = live[i];
 			st->acc_live[i] = 0;
 		}
-		st->pub_gathers = atomicAdd(&st->acc_gathers, 0ull);
 		st->acc_gathers = 0;
 		for (int i = 0; i < 4; i++) {
 			st->pull_ticket[i] = 0;
@@ -749,7 +798,8 @@ __device__ __forceinline__ void finish_level(LevelStatus *st, const u64 *seen, c
 		st->acc_sat = 0;
 		st->n_touched = 0;
 		st->blocks_done = 0;
-		publish_to_host(a.host_st, st, a.seq, 0);
+		publish_fields(a.host_st, fv, fe, items, s_remaining, sat, gathers, live, 0);
+		signal_host(a.host_st, a.seq);
 	}
 }
 
@@ -938,19 +988,29 @@ __global__ void __launch_bounds__(256) k_update_sparse(const int32_t *__restrict
 
 #include "pgq_pull.cuh"
 
-// The rows that cross a range boundary of k_pull_fused (at most one per range): their OR was combined
-// with atomicOr in cand; apply the level update, and clear them in the array that becomes cand in the
-// next level (a bottom-up level overwrites every exclusive row, so only these must be zero beforehand).
-// The last block ends the level (finish_level).
+// Behind a fused bottom-up level, one launch (the last block ends the level, finish_level):
+//  * The rows that cross a range boundary of k_pull_fused (at most one per range): their OR was combined with
+//    atomicOr in cand; apply the level update, and clear them in the array that becomes cand in the next level (a
+//    bottom-up level overwrites every exclusive row, so only these must be zero beforehand).  A thread per row; in path
+//    mode a warp per row (long rows gain hundreds of bits per level there, which the 32 lanes record together).
+//  * Fused bottom-up levels neither gather for nor write finished rows.  A row is marked finished in the level that
+//    finds every live lane in its seen mask; the frontier bits it gained in that level (in cand) and in the level
+//    before (in visit) are still in the two mask arrays and each must disappear once it has been read as a frontier:
+//    when `words` > 0, the rows whose bit appeared in the bitmap since the snapshot taken two levels ago are zeroed in
+//    the array that was the level's frontier (old_visit), and the snapshot is refreshed.  (Top-down
+//    levels in between clean up after themselves; a stale snapshot only zeroes more rows than necessary, and a finished
+//    row's frontier entry may always be zeroed once the level that read it is over.)  A crossing row this launch marks
+//    may be missing from the snapshot it writes: its entry in old_visit is cleared by the first part anyway, and a bit
+//    missing from a snapshot only makes a later level zero that row once more.
 template <int W, bool PATH>
-__global__ void __launch_bounds__(256) k_pull_finish(const PullArgs<W> a, u64 *old_visit, CheckArgs chk) {
-	// a warp per shared row (they are long rows: in path mode they gain hundreds of bits per level, which the 32
-	// lanes record together); every lane computes the update, lane 0 stores it
+__global__ void __launch_bounds__(256) k_pull_finish(const PullArgs<W> a, u64 *old_visit, uint32_t *snap, int64_t words,
+                                                     CheckArgs chk) {
+	constexpr int T = PATH ? 32 : 1; // threads per crossing row
 	const int lane = threadIdx.x & 31;
-	const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-	const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+	const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	const int64_t nthreads = (int64_t)gridDim.x * blockDim.x;
 	PullTotals<W> tot;
-	for (int64_t i = warp; i < a.nranges; i += nwarps) {
+	for (int64_t i = tid / T; i < a.nranges; i += nthreads / T) {
 		const int k = a.shared_row[i]; // rank of a long row
 		if (k < 0) {
 			continue;
@@ -967,8 +1027,10 @@ __global__ void __launch_bounds__(256) k_pull_finish(const PullArgs<W> a, u64 *o
 			sn[w] |= val[w];
 			now_sat &= ((~sn[w]) & a.live.w[w]) == 0;
 		}
-		__syncwarp(); // (all lanes have read the row before lane 0 rewrites it)
-		if (lane == 0) {
+		if (PATH) {
+			__syncwarp(); // (all lanes have read the row before lane 0 rewrites it)
+		}
+		if (!PATH || lane == 0) {
 			st_mask<W>(a.cand, row, val);
 			if (any_new) {
 				st_mask<W>(a.seen, row, sn);
@@ -1000,47 +1062,45 @@ __global__ void __launch_bounds__(256) k_pull_finish(const PullArgs<W> a, u64 *o
 			}
 		}
 	}
-	pull_totals_flush<W>(tot, a.st);
-	finish_level<W, PATH>(a.st, a.seen, chk);
-}
-
-// Fused bottom-up levels neither gather for nor write finished rows.  A row is marked finished in the level that
-// finds every live lane in its seen mask; the frontier bits it gained in that level (in cand) and in the level before
-// (in visit) are still in the two mask arrays and each must disappear once it has been read as a frontier: after every
-// level this kernel zeroes, in the array that was the level's frontier, the rows whose bit appeared in the bitmap
-// since the snapshot taken two levels ago, and refreshes that snapshot.  (Top-down levels in between clean up after
-// themselves; a stale snapshot only zeroes more rows than necessary, and a finished row's frontier entry may always
-// be zeroed once the level that read it is over.)
-template <int W>
-__global__ void __launch_bounds__(256) k_pull_zero(const PullArgs<W> a, u64 *old_visit, uint32_t *snap, int64_t words) {
-	for (int64_t w = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; w < words; w += (int64_t)gridDim.x * blockDim.x) {
-		const uint32_t cur = a.satbits[w];
-		uint32_t delta = cur & ~snap[w];
-		if (cur != snap[w]) {
-			snap[w] = cur;
-		}
-		while (delta) {
-			const int b = __ffs(delta) - 1;
-			delta &= delta - 1;
-			const int64_t idx = w * 32 + b;
-			int row = -1;
-			if (idx < a.short_base) {
-				if (idx < a.g.n_rows) {
-					row = a.g.row[idx];
-				}
-			} else if (idx - a.short_base < a.g.n_short) {
-				row = a.g.s_row[idx - a.short_base];
+	// A warp takes 32 bitmap words, a lane each, then visits only the words with new bits: lane l handles bit l of
+	// such a word, so the rank -> row lookups are coalesced.  (Whole warps: nthreads is a multiple of 32.)
+	for (int64_t w0 = (tid >> 5) * 32; w0 < words; w0 += nthreads) {
+		const int64_t w = w0 + lane;
+		uint32_t delta = 0;
+		if (w < words) {
+			const uint32_t cur = a.satbits[w];
+			const uint32_t old = snap[w];
+			delta = cur & ~old;
+			if (cur != old) {
+				snap[w] = cur;
 			}
-			if (row >= 0) {
-				u64 zero[W];
-#pragma unroll
-				for (int i = 0; i < W; i++) {
-					zero[i] = 0;
+		}
+		for (unsigned todo = __ballot_sync(FULL_MASK, delta != 0); todo; todo &= todo - 1) {
+			const int j = __ffs(todo) - 1;
+			const uint32_t d = __shfl_sync(FULL_MASK, delta, j);
+			if ((d >> lane) & 1u) {
+				const int64_t idx = (w0 + j) * 32 + lane;
+				int row = -1;
+				if (idx < a.short_base) {
+					if (idx < a.g.n_rows) {
+						row = a.g.row[idx];
+					}
+				} else if (idx - a.short_base < a.g.n_short) {
+					row = a.g.s_row[idx - a.short_base];
 				}
-				st_mask<W>(old_visit, row, zero);
+				if (row >= 0) {
+					u64 zero[W];
+#pragma unroll
+					for (int i = 0; i < W; i++) {
+						zero[i] = 0;
+					}
+					st_mask<W>(old_visit, row, zero);
+				}
 			}
 		}
 	}
+	pull_totals_flush<W>(tot, a.st);
+	finish_level<W, PATH>(a.st, a.seen, chk);
 }
 
 // After bottom-up levels the frontier exists only as masks.  When the next level runs top-down (or in
@@ -1839,7 +1899,7 @@ static int run_batch(Run &r, const CallCtx &cc, LevelStatus *d_st, LevelStatus *
 	// finished-rows bitmap: the long rows by rank, then (word-aligned) the short rows by sorted position
 	const int64_t short_base = (csr->pull.n_rows + 31) / 32 * 32;
 	const size_t sat_words = (size_t)(short_base + csr->pull.n_slices * 32) / 32 + 2;
-	// (behind the bitmap: its snapshots of one and two levels ago, k_pull_zero)
+	// (behind the bitmap: its snapshots of one and two levels ago, k_pull_finish)
 	const size_t sat_bytes = 3 * sat_words * sizeof(uint32_t);
 	uint32_t *satbits = nullptr;
 	int32_t *shared_rows = nullptr;
@@ -2020,14 +2080,14 @@ static int run_batch(Run &r, const CallCtx &cc, LevelStatus *d_st, LevelStatus *
 			PGQ_TRY((launch_pull_fused<W, PATH>(pull_variant, r.sms, s, pa, batch_pulls > 0))); // (EXIT variant: from the 2nd on)
 			batch_pulls++;
 			PGQ_CUDA(cudaEventRecord(eb, s));
-			k_pull_finish<W, PATH><<<grid_cap((nranges + 7) / 8, wide_grid), 256, 0, s>>>(pa, visit, chk);
-			if (skip_finished) {
-				// rows that were marked finished in this level or the one before: their entry in the array that was
-				// this level's frontier is zeroed now (nobody writes a finished row any more)
-				k_pull_zero<W><<<grid_cap(((int64_t)sat_words + 255) / 256, wide_grid), 256, 0, s>>>(
-				    pa, visit, satbits + sat_words * (1 + (iter & 1)), (int64_t)sat_words);
-				r.st.kernel_launches++;
-			}
+			// (grid-stride loops over a thread per crossing row -- a warp in path mode -- and, when finished rows are
+			// skipped, a lane per bitmap word; the snapshot alternates with the level's parity.  Every block takes a
+			// ticket of finish_level, so the grid stays at most 8 blocks per SM: on the H100, with a thread per bitmap
+			// bit, a cap of 32 blocks per SM ran the bench 4 % slower)
+			const int64_t zero_words = skip_finished ? (int64_t)sat_words : 0;
+			const int64_t finish_threads = std::max<int64_t>(nranges * (PATH ? 32 : 1), zero_words);
+			k_pull_finish<W, PATH><<<grid_cap((finish_threads + 255) / 256, wide_grid), 256, 0, s>>>(
+			    pa, visit, satbits + sat_words * (1 + (iter & 1)), zero_words, chk);
 			if (iter == 1) { // the sources may lie outside the rows a bottom-up level rewrites
 				k_clear_items<W><<<grid_cap((n_items + 255) / 256, 64), 256, 0, s>>>(items, n_items, visit);
 				r.st.kernel_launches++;

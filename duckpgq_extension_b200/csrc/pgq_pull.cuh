@@ -29,7 +29,7 @@
 //
 // Finished rows: a search whose frontier has died out can never add a bit anywhere, so a destination
 // that every LIVE lane has seen is finished for good; it is marked in a bitmap and from then on is
-// neither gathered for nor written (k_pull_zero, pgq_bfs.cu, clears the two frontier entries it leaves
+// neither gathered for nor written (k_pull_finish, pgq_bfs.cu, clears the two frontier entries it leaves
 // behind), a range / slice whose rows are all finished costs one bitmap test, and a chunk inside a
 // finished row is not even read.  (Undirected social graphs saturate after 3-4 levels; on directed
 // R-MAT the levels behind the peak have 13 % and 0.1 % of the gathers left.)
@@ -59,7 +59,7 @@ struct PullArgs {
 	int iter;
 	int skip;
 	// Finished rows are not written at all.  Their entries in the two mask buffers are zeroed behind the level by
-	// k_pull_zero (bits newly set in the bitmap since the snapshot of two levels ago), so a range / slice whose rows
+	// k_pull_finish (bits newly set in the bitmap since the snapshot of two levels ago), so a range / slice whose rows
 	// are all finished costs one or two loads of the bitmap and nothing else.
 	LaneMask<W> live;
 };
@@ -175,7 +175,7 @@ __device__ __forceinline__ bool sat_bit(const uint32_t *bits, int64_t k) {
 template <int W, bool PATH, bool HAVE_SEEN = false>
 __device__ __forceinline__ void pull_update_row(const PullArgs<W> &a, int row, u64 (&val)[W], bool finished,
                                                 int64_t satpos, PullTotals<W> &tot, u64 *seen_row = nullptr) {
-	if (finished) { // (both mask buffers hold zeros for it, or k_pull_zero is about to see to that)
+	if (finished) { // (both mask buffers hold zeros for it, or k_pull_finish is about to see to that)
 #pragma unroll
 		for (int i = 0; i < W; i++) {
 			val[i] = 0;
