@@ -538,8 +538,8 @@ __global__ void __launch_bounds__(RS_THREADS) k_rs_scatter(const int32_t *__rest
 
 // Sorts by the low `end_bit` bits of the keys.  (keys_a, vals_a) hold the input and are clobbered;
 // the result is in (*keys_res, *vals_res), which is either the a or the b pair.
-static int radix_sort_pairs(Workspace *ws, int32_t *keys_a, int32_t *keys_b, int32_t *vals_a, int32_t *vals_b,
-                            int64_t count, int end_bit, cudaStream_t s, int32_t **keys_res, int32_t **vals_res) {
+int radix_sort_pairs(Workspace *ws, int32_t *keys_a, int32_t *keys_b, int32_t *vals_a, int32_t *vals_b, int64_t count,
+                     int end_bit, cudaStream_t s, int32_t **keys_res, int32_t **vals_res) {
 	const int nblocks = (int)((count + RS_TILE - 1) / RS_TILE);
 	const int64_t hist_elems = (int64_t)RS_BINS * nblocks;
 	int32_t *hist, *scan_tmp;

@@ -164,6 +164,13 @@ struct pgq_csr {
 	int64_t *w_bits = nullptr;
 	bool neg_weights = false; // some weight is below zero (a NaN is not): cheapest_path_length relaxes from every vertex
 	std::unordered_map<void *, size_t> allocs; // every device buffer of this CSR with its size (buffer cache)
+	// pagerank / weakly_connected_component of all n + 2 entries, computed on the first call under `mu` and kept
+	// on the host (pgq_analytics.cu); pgq_csr_clone does not copy them
+	bool pr_done = false;
+	int64_t pr_iters = 0;
+	std::vector<double> pr_rank;
+	bool wcc_done = false;
+	std::vector<int64_t> wcc_label;
 };
 
 // ---- helpers implemented in pgq_csr.cu ---------------------------------------------------------
@@ -175,6 +182,9 @@ int pgq_ws_reserve(Workspace *ws, int slot, size_t bytes, void **out);
 int pgq_ws_pinned(Workspace *ws, size_t bytes, void **out);
 int pgq_scan_exclusive_i32(const int32_t *in, int32_t *out, int64_t count, int32_t *block_tmp, cudaStream_t s);
 size_t pgq_scan_tmp_elems(int64_t count);
+// stable LSD radix sort of (int32 key, int32 value) pairs by the low end_bit bits; uses workspace slots 14 and 15
+int radix_sort_pairs(Workspace *ws, int32_t *keys_a, int32_t *keys_b, int32_t *vals_a, int32_t *vals_b, int64_t count,
+                     int end_bit, cudaStream_t s, int32_t **keys_res, int32_t **vals_res);
 
 // ---- BFS drivers implemented in pgq_bfs.cu -----------------------------------------------------
 int pgq_bfs_lengths_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,

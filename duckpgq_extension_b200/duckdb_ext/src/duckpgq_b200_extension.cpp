@@ -7,6 +7,9 @@
 //   create_csr_vertex / create_csr_edge (3 overloads) / delete_csr   csr_creation.cpp:86-238, csr_deletion.cpp:10-29
 //   iterativelength / iterativelength2 / shortestpath                iterativelength.cpp:148-152, shortest_path.cpp:212-217
 //   cheapest_path_length                                             cheapest_path_length.cpp:162-166
+//   local_clustering_coefficient / pagerank / weakly_connected_component (the reference's binds, device callbacks)
+//                                                                    local_clustering_coefficient.cpp:14-83,
+//                                                                    pagerank.cpp:14-120, weakly_connected_component.cpp:37-113
 //
 // The MATCH rewriter calls all of them BY NAME in the SQL it generates (match.cpp:476-487,657-671,
 // compressed_sparse_row.cpp:132-251), so every SQL/PGQ query keeps the reference's parser, binder and
@@ -17,8 +20,8 @@
 // forwarded to the device build (pgq_csr_add_*; asynchronous pinned staging, no upload at query time).
 // What happens to the HOST arrays is a mode (PGQ_B200_HOST_CSR):
 //   skip   (default) the reference's scatter into the int64 host arrays is not run at all; the functions
-//          of the reference that read the host CSR (pagerank, weakly_connected_component,
-//          local_clustering_coefficient, reachability, csr_get_w_type, get_csr_v / _e / _w / _ptr, ...) are
+//          of the reference that read the host CSR (reachability, csr_get_w_type, iterativelength_bidirectional,
+//          get_csr_v / _e / _w / _ptr) are
 //          wrapped: the wrapper first materialises the host arrays from the device copy (pgq_csr_download,
 //          the reference's own layout), then calls the captured reference callback;
 //   mirror the captured reference callback runs for every chunk as well (host and device CSR side by side).
@@ -45,6 +48,9 @@
 
 #include "duckpgq/core/functions/function_data/cheapest_path_length_function_data.hpp"
 #include "duckpgq/core/functions/function_data/iterative_length_function_data.hpp"
+#include "duckpgq/core/functions/function_data/local_clustering_coefficient_function_data.hpp"
+#include "duckpgq/core/functions/function_data/pagerank_function_data.hpp"
+#include "duckpgq/core/functions/function_data/weakly_connected_component_function_data.hpp"
 #include "duckpgq/core/utils/compressed_sparse_row.hpp"
 #include "duckpgq/core/utils/duckpgq_utils.hpp"
 
@@ -62,7 +68,7 @@ namespace duckdb {
 static std::mutex g_ctx_lock;
 static pgq_ctx *g_ctx = nullptr;
 static std::atomic<int64_t> g_calls_lengths {0}, g_calls_paths {0}, g_calls_cheapest {0}, g_pairs {0}, g_uploads {0},
-    g_device_builds {0}, g_chunks {0}, g_materialized {0};
+    g_device_builds {0}, g_chunks {0}, g_materialized {0}, g_calls_lcc {0}, g_calls_pagerank {0}, g_calls_wcc {0};
 
 [[noreturn]] static void ThrowStatus(int status) {
 	string msg = pgq_last_error();
@@ -773,6 +779,105 @@ static void CheapestPathLengthB200Function(DataChunk &args, ExpressionState &sta
 	duckpgq_state->csr_to_delete.insert(info.csr_id); // cheapest_path_length.cpp:160
 }
 
+// ---- local_clustering_coefficient / pagerank / weakly_connected_component ---------------------------------------
+// Registered through WrapScalar, so the signatures and binds are the reference's; the reference callback is not
+// called.  The device CSR is found like a path function's (the device build, or an upload of the host CSR).
+static pgq_csr *ForAnalytics(ClientContext &context, int32_t csr_id, const char *not_initialized) {
+	auto duckpgq_state = GetDuckPGQState(context);
+	auto csr_entry = duckpgq_state->csr_list.find(csr_id); // e.g. pagerank.cpp:17-24
+	if (csr_entry == duckpgq_state->csr_list.end()) {
+		throw ConstraintException("CSR not found. Is the graph populated?");
+	}
+	CSR &host = *csr_entry->second;
+	auto b200 = GetB200State(context);
+	auto entry = b200->Find(csr_id);
+	// initialized_e: in mode `skip` the host arrays stay empty, and edges that reached the device build count
+	const bool edges = host.initialized_e || (entry && entry->edges_started);
+	if (!(host.initialized_v && edges)) {
+		throw ConstraintException(not_initialized);
+	}
+	return b200->ForPathFunction(csr_id, host, static_cast<int64_t>(host.vsize) - 2);
+}
+
+// The source column (args.data[1]) as contiguous ids + validity.
+struct SourceColumn {
+	vector<int64_t> src;
+	vector<uint8_t> valid;
+	SourceColumn(DataChunk &args) {
+		Column<int64_t> col(args.data[1], args.size());
+		src.assign(col.data, col.data + args.size());
+		valid.resize(args.size());
+		for (idx_t i = 0; i < args.size(); i++) {
+			valid[i] = col.RowIsValid(i) ? 1 : 0;
+		}
+	}
+};
+
+template <class T>
+static void WriteAnalyticsResult(Vector &result, const vector<T> &out, const vector<uint8_t> &out_valid) {
+	result.SetVectorType(VectorType::FLAT_VECTOR);
+	auto result_data = FlatVector::GetDataMutable<T>(result);
+	auto &result_validity = FlatVector::ValidityMutable(result);
+	for (idx_t i = 0; i < out.size(); i++) {
+		result_data[i] = out[i];
+		if (!out_valid[i]) {
+			result_validity.SetInvalid(i);
+		}
+	}
+}
+
+static void LocalClusteringCoefficientB200(const scalar_function_t &, DataChunk &args, ExpressionState &state,
+                                           Vector &result) {
+	auto &info = state.expr.Cast<BoundFunctionExpression>().BindInfo()->Cast<LocalClusteringCoefficientFunctionData>();
+	pgq_csr *csr = ForAnalytics(info.context, info.csr_id,
+	                            "Need to initialize CSR before doing local clustering coefficient.");
+	SourceColumn src(args);
+	vector<float> out(args.size());
+	vector<uint8_t> out_valid(args.size());
+	int st = pgq_local_clustering_coefficient(csr, static_cast<int64_t>(args.size()), src.src.data(), src.valid.data(),
+	                                          out.data(), out_valid.data(), nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_lcc++;
+	WriteAnalyticsResult(result, out, out_valid);
+	GetDuckPGQState(info.context)->csr_to_delete.insert(info.csr_id); // local_clustering_coefficient.cpp:71
+}
+
+static void PageRankB200(const scalar_function_t &, DataChunk &args, ExpressionState &state, Vector &result) {
+	auto &info = state.expr.Cast<BoundFunctionExpression>().BindInfo()->Cast<PageRankFunctionData>();
+	pgq_csr *csr = ForAnalytics(info.context, info.csr_id, "Need to initialize CSR before running PageRank.");
+	SourceColumn src(args);
+	vector<double> out(args.size());
+	vector<uint8_t> out_valid(args.size());
+	int st = pgq_pagerank(csr, static_cast<int64_t>(args.size()), src.src.data(), src.valid.data(), out.data(),
+	                      out_valid.data(), nullptr, nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_pagerank++;
+	WriteAnalyticsResult(result, out, out_valid);
+	GetDuckPGQState(info.context)->csr_to_delete.insert(info.csr_id); // pagerank.cpp:110
+}
+
+static void WeaklyConnectedComponentB200(const scalar_function_t &, DataChunk &args, ExpressionState &state,
+                                         Vector &result) {
+	auto &info = state.expr.Cast<BoundFunctionExpression>().BindInfo()->Cast<WeaklyConnectedComponentFunctionData>();
+	pgq_csr *csr = ForAnalytics(info.context, info.csr_id,
+	                            "Need to initialize CSR before doing weakly connected components.");
+	SourceColumn src(args);
+	vector<int64_t> out(args.size());
+	vector<uint8_t> out_valid(args.size());
+	int st = pgq_weakly_connected_component(csr, static_cast<int64_t>(args.size()), src.src.data(), src.valid.data(),
+	                                        out.data(), out_valid.data(), nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_wcc++;
+	WriteAnalyticsResult(result, out, out_valid);
+	GetDuckPGQState(info.context)->csr_to_delete.insert(info.csr_id); // weakly_connected_component.cpp:103
+}
+
 // ---- introspection: proves which implementation served the query ------------------------------------------
 // duckpgq_b200_stats() -> 'iterativelength_calls=..,shortestpath_calls=..,pairs=..,csr_uploads=..,...'
 static void B200StatsFunction(DataChunk &args, ExpressionState &state, Vector &result) {
@@ -782,7 +887,10 @@ static void B200StatsFunction(DataChunk &args, ExpressionState &state, Vector &r
 	              ",pairs=" + std::to_string(g_pairs.load()) + ",csr_uploads=" + std::to_string(g_uploads.load()) +
 	              ",csr_device_builds=" + std::to_string(g_device_builds.load()) +
 	              ",csr_chunks=" + std::to_string(g_chunks.load()) +
-	              ",host_csr_materialisations=" + std::to_string(g_materialized.load());
+	              ",host_csr_materialisations=" + std::to_string(g_materialized.load()) +
+	              ",local_clustering_coefficient_calls=" + std::to_string(g_calls_lcc.load()) +
+	              ",pagerank_calls=" + std::to_string(g_calls_pagerank.load()) +
+	              ",weakly_connected_component_calls=" + std::to_string(g_calls_wcc.load());
 	result.SetVectorType(VectorType::CONSTANT_VECTOR);
 	ConstantVector::GetData<string_t>(result)[0] = StringVector::AddString(result, text);
 }
@@ -847,10 +955,13 @@ static void LoadInternal(ExtensionLoader &loader) {
 	WrapScalar(loader, "create_csr_edge", CreateCsrEdgeB200);
 	WrapScalar(loader, "delete_csr", DeleteCsrB200);
 	// reference functions that read the host CSR
-	for (auto name : {"pagerank", "weakly_connected_component", "local_clustering_coefficient", "reachability",
-	                  "csr_get_w_type", "iterativelength_bidirectional"}) {
+	for (auto name : {"reachability", "csr_get_w_type", "iterativelength_bidirectional"}) {
 		WrapScalar(loader, name, HostConsumerB200);
 	}
+	// the other consumers of the CSR: on the device
+	WrapScalar(loader, "local_clustering_coefficient", LocalClusteringCoefficientB200);
+	WrapScalar(loader, "pagerank", PageRankB200);
+	WrapScalar(loader, "weakly_connected_component", WeaklyConnectedComponentB200);
 	WrapTable<0>(loader, "get_csr_v");
 	WrapTable<1>(loader, "get_csr_e");
 	WrapTable<2>(loader, "get_csr_w");

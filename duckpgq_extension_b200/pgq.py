@@ -135,13 +135,16 @@ class DeviceCSR:
         self._h = handle
         self.n = n
         self.initialized_v = True
+        self.initialized_e = True  # CsrInitializeEdge has run (csr_creation.cpp:43-61): False until create()'s edges come
 
     # ---- construction ---------------------------------------------------------------------------
     @classmethod
     def create(cls, ctx: Context, n: int) -> "DeviceCSR":
         h = C.c_void_p()
         _check(ctx._lib.pgq_csr_create(ctx._h, n, C.byref(h)))
-        return cls(ctx, h, n)
+        csr = cls(ctx, h, n)
+        csr.initialized_e = False
+        return csr
 
     @classmethod
     def build(cls, ctx: Context, n: int, src, dst, edge_id=None) -> "DeviceCSR":
@@ -180,6 +183,7 @@ class DeviceCSR:
 
     def add_edges(self, edge_size: int, edge_size_count: int, src, dst, edge_id, weight=None):
         src, dst, edge_id = _i64(src), _i64(dst), _i64(edge_id)
+        self.initialized_e = True
         if weight is None:
             _check(self._lib.pgq_csr_add_edges(self._h, edge_size, edge_size_count, src.shape[0], _p64(src), _p64(dst),
                                                _p64(edge_id)))
@@ -222,6 +226,45 @@ class DeviceCSR:
 
     def finalize(self):
         _check(self._lib.pgq_csr_finalize(self._h))
+
+    # ---- the other consumers of the CSR (ids n and n + 1 are the reference's two entries behind the vertices) ---
+    def local_clustering_coefficient(self, src, src_valid=None):
+        """-> (float32 coefficients, valid uint8, stats dict).  An id outside [0, n) raises (PGQ_ERR_RANGE)."""
+        src = _i64(src)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        out = np.zeros(max(p, 1), dtype=np.float32)
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        st = _native.PgqStats()
+        _check(self._lib.pgq_local_clustering_coefficient(self._h, p, _p64(src), _pu8(sv),
+                                                          out.ctypes.data_as(C.POINTER(C.c_float)), _pu8(ov),
+                                                          C.byref(st)))
+        return out[:p], ov[:p], st.as_dict()
+
+    def pagerank(self, src, src_valid=None):
+        """-> (float64 ranks, valid uint8, iterations, stats dict).  Computed on the first call, cached after."""
+        src = _i64(src)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        out = np.zeros(max(p, 1), dtype=np.float64)
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        it = C.c_int64(0)
+        st = _native.PgqStats()
+        _check(self._lib.pgq_pagerank(self._h, p, _p64(src), _pu8(sv), out.ctypes.data_as(C.POINTER(C.c_double)),
+                                      _pu8(ov), C.byref(it), C.byref(st)))
+        return out[:p], ov[:p], int(it.value), st.as_dict()
+
+    def weakly_connected_component(self, src, src_valid=None):
+        """-> (int64 component ids, valid uint8, stats dict).  Computed on the first call, cached after."""
+        src = _i64(src)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        out = np.zeros(max(p, 1), dtype=np.int64)
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        st = _native.PgqStats()
+        _check(self._lib.pgq_weakly_connected_component(self._h, p, _p64(src), _pu8(sv), _p64(out), _pu8(ov),
+                                                        C.byref(st)))
+        return out[:p], ov[:p], st.as_dict()
 
     # ---- introspection (get_csr_v / get_csr_e, pgq_scan.cpp:84-111) ------------------------------
     def info(self):
@@ -440,6 +483,49 @@ def shortestpath(state: DuckPGQState, csr_id: int, v_size: int, src, dst, src_va
     paths, _ = csr.shortestpath(src, dst, src_valid, options)
     state.csr_to_delete.add(csr_id)  # shortest_path.cpp:206
     return paths
+
+
+_NOT_INITIALIZED_TEXT = {  # the binds' texts: local_clustering_coefficient.cpp:22, pagerank.cpp:23,
+    "lcc": "Need to initialize CSR before doing local clustering coefficient.",  # weakly_connected_component.cpp:47
+    "pagerank": "Need to initialize CSR before running PageRank.",
+    "wcc": "Need to initialize CSR before doing weakly connected components.",
+}
+
+
+def _lookup_for_analytics(state: DuckPGQState, csr_id: int, what: str) -> DeviceCSR:
+    csr = state.csr_list.get(csr_id)
+    if csr is None:
+        raise ConstraintException(PGQ_ERR_INVALID_ID, "CSR not found. Is the graph populated?")
+    if not (csr.initialized_v and csr.initialized_e):  # e.g. pagerank.cpp:22-24
+        raise ConstraintException(PGQ_ERR_NOT_INITIALIZED, _NOT_INITIALIZED_TEXT[what])
+    csr.finalize()
+    return csr
+
+
+def local_clustering_coefficient(state: DuckPGQState, csr_id: int, src, src_valid=None):
+    """local_clustering_coefficient(INT, BIGINT) -> FLOAT (local_clustering_coefficient.cpp:14-70):
+    (coefficients, valid)."""
+    csr = _lookup_for_analytics(state, csr_id, "lcc")
+    out, valid, _ = csr.local_clustering_coefficient(src, src_valid)
+    state.csr_to_delete.add(csr_id)  # l.71
+    return out, valid
+
+
+def pagerank(state: DuckPGQState, csr_id: int, src, src_valid=None):
+    """pagerank(INT, BIGINT) -> DOUBLE (pagerank.cpp:14-107): (ranks, valid)."""
+    csr = _lookup_for_analytics(state, csr_id, "pagerank")
+    out, valid, _, _ = csr.pagerank(src, src_valid)
+    state.csr_to_delete.add(csr_id)
+    return out, valid
+
+
+def weakly_connected_component(state: DuckPGQState, csr_id: int, src, src_valid=None):
+    """weakly_connected_component(INT, BIGINT) -> BIGINT (weakly_connected_component.cpp:37-104):
+    (component ids, valid)."""
+    csr = _lookup_for_analytics(state, csr_id, "wcc")
+    out, valid, _ = csr.weakly_connected_component(src, src_valid)
+    state.csr_to_delete.add(csr_id)
+    return out, valid
 
 
 def delete_csr(state: DuckPGQState, csr_id: int) -> bool:

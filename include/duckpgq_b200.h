@@ -194,6 +194,34 @@ int pgq_cheapest_path_length(pgq_csr *csr, int64_t n_pairs, const int64_t *src, 
                              const uint8_t *src_valid, const uint8_t *dst_valid, void *out_cost, uint8_t *out_valid,
                              pgq_stats *stats);
 
+/* ---- the other consumers of the CSR ------------------------------------------------------------------------
+ * Host pointers in and out.  As in the reference, "v_size" is n + 2: the two entries n and n + 1 behind the
+ * vertices have no edges and take part where the reference lets them.  Results are bit-identical to the reference's.
+ *
+ * pgq_local_clustering_coefficient <- LocalClusteringCoefficientFunction local_clustering_coefficient.cpp:41-70
+ *   out[i] = (float)count / (k * (k - 1.0f)) with k the out-degree of src[i] and count the entries of its
+ *   neighbours' lists (neighbours with multiplicity) that are neighbours of src[i]; 0 when k < 2.  A NULL source
+ *   gives NULL.  An id outside [0, n) fails the call with PGQ_ERR_RANGE (the reference reads out of bounds).
+ *   Computed per call.  stats: kernel_launches, h2d/d2h bytes, total_ms.
+ * pgq_pagerank <- PageRankFunction pagerank.cpp:31-84
+ *   out[i] = the rank of entry src[i], valid for src[i] in [0, n + 2); NULL source or any other id -> NULL.
+ *   *iterations (nullable) = the iteration count of the computation (the reference's iteration_count).
+ * pgq_weakly_connected_component <- WeaklyConnectedComponentFunction weakly_connected_component.cpp:37-104
+ *   out[i] = the reference's component id (the root of src[i] in its Link forest) for src[i] in [0, n + 2);
+ *   NULL source or any other id -> NULL.
+ * PageRank and the component ids are computed for all entries on the first call for a CSR (concurrent first
+ * callers wait for it) and answered from a host copy afterwards.  stats of the call that computed them:
+ * levels = PageRank iterations / Boruvka rounds, kernel_launches, d2h_bytes, total_ms (device time of the
+ * computation) and, for pgq_pagerank, expand_ms = device time of the serial dangling-rank fold over all
+ * iterations.  A call answered from the copy reports zeros.
+ */
+int pgq_local_clustering_coefficient(pgq_csr *csr, int64_t n_rows, const int64_t *src, const uint8_t *src_valid,
+                                     float *out, uint8_t *out_valid, pgq_stats *stats);
+int pgq_pagerank(pgq_csr *csr, int64_t n_rows, const int64_t *src, const uint8_t *src_valid, double *out,
+                 uint8_t *out_valid, int64_t *iterations, pgq_stats *stats);
+int pgq_weakly_connected_component(pgq_csr *csr, int64_t n_rows, const int64_t *src, const uint8_t *src_valid,
+                                   int64_t *out, uint8_t *out_valid, pgq_stats *stats);
+
 /* Device-resident form of pgq_iterativelength: all pointers are device pointers on the CSR's
  * device, the work is enqueued on `stream` (a cudaStream_t passed as void*; NULL = the legacy
  * default stream) and has completed when the call returns.  Used when the pairs already live in
