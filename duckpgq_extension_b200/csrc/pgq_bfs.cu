@@ -2454,6 +2454,20 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 	if (rc != PGQ_OK) {
 		return rc;
 	}
+	// The reference's batch loop (iterativelength.cpp:84-113, shortest_path.cpp:93-125) starts one batch more when
+	// its last batch filled every lane (or no row took a lane) and rows that take no lane follow: that batch finds no
+	// lane and ends at once.  Count it, so that the counters of the reference's batch composition stay the reference's.
+	// (Only at an explicit lane width: with lanes = auto the last batch is narrowed to what it holds, so "full" says
+	// nothing about the reference's batches.)
+	if (ref_batching && opts && opts->lanes && p > 0 && shard_count <= 1 &&
+	    (batches.empty() || batches.back().take == batches.back().lanes)) {
+		int32_t last = 0;
+		PGQ_CUDA(cudaMemcpyAsync(&last, aa.row_lane + p - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaStreamSynchronize(s));
+		if (last < 0) {
+			r.st.batches++;
+		}
+	}
 	if (PATH) {
 		// list offsets over ALL rows in row order, then move every walked path to its place
 		int64_t *d_total;
