@@ -1027,7 +1027,7 @@ static int read_flag(int *d_flag, cudaStream_t s, int *value) {
 	return PGQ_OK;
 }
 
-// Builds head / nzrow / chunk_rank for a direction whose off[] and adj[] are in place.
+// Builds head / nzrow / chunk_rank of the out-CSR once its off[] and adj[] are in place.
 static int build_dir_metadata(pgq_csr *csr, DirGraph &g, Workspace *ws, cudaStream_t s) {
 	int64_t n = csr->n, m = csr->m;
 	g.nchunks = (m + PGQ_CHUNK - 1) / PGQ_CHUNK;
@@ -1086,7 +1086,7 @@ static int build_pull_graph(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	g.n_slices = (g.n_short + 31) / 32;
 	// ---- long part
 	const size_t head_words = (size_t)std::max<int64_t>(g.nchunks, 1) * PGQ_STEPS;
-	// (padded to whole ranges of 1024 positions: the bottom-up kernel fetches a range with one 4 KB bulk copy)
+	// (padded with -1 to whole ranges of 1024 positions)
 	const size_t adj_elems = (size_t)((std::max<int64_t>(g.m, 1) + 1023) / 1024) * 1024;
 	PGQ_TRY(dev_alloc(csr, (void **)&g.adj, adj_elems * sizeof(int32_t)));
 	PGQ_CUDA(cudaMemsetAsync(g.adj + adj_elems - 1024, 0xFF, 1024 * sizeof(int32_t), s));
@@ -1183,7 +1183,6 @@ static int finish_csr(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 			PGQ_CUDA(cudaMemcpyAsync(csr->in.adj, vals_res, (size_t)m * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
 		}
 	}
-	PGQ_TRY(build_dir_metadata(csr, csr->in, ws, s));
 	PGQ_TRY(build_pull_graph(csr, ws, s));
 	PGQ_CUDA(cudaStreamSynchronize(s));
 	static std::atomic<uint64_t> next_uid {1};

@@ -46,7 +46,9 @@ int pgq_fail(int status, const char *fmt, ...);
 #define PGQ_CHUNK 256
 #define PGQ_STEPS 8
 
-// One direction of the graph: the out-CSR (row = source) or the in-CSC (row = destination).
+// One direction of the graph: the out-CSR (row = source) or the in-CSC (row = destination).  Only the out-CSR has
+// head / nzrow / chunk_rank (the edge-tiled CSR build kernels walk it); the in-CSC is off / adj alone, and nnz /
+// nchunks are 0 there.
 struct DirGraph {
 	int32_t *off = nullptr;        // [n+1] row offsets
 	int32_t *adj = nullptr;        // [m]   neighbour ids

@@ -40,6 +40,7 @@ static int clone_array(pgq_csr *dst, int dst_dev, T **out, const T *src, int src
 	return PGQ_OK;
 }
 
+// (the in-CSC has no head / nzrow / chunk_rank: clone_array leaves a null array null)
 static int clone_dir(pgq_csr *dst, int dd, DirGraph &out, const DirGraph &in, int sd, int64_t n, int64_t m, cudaStream_t s) {
 	out.nnz = in.nnz;
 	out.nchunks = in.nchunks;

@@ -34,8 +34,9 @@
 // finished row is not even read.  (Undirected social graphs saturate after 3-4 levels; on directed
 // R-MAT the levels behind the peak have 13 % and 0.1 % of the gathers left.)
 //
-// EXIT (tuning variant 17, not the default): a row stops gathering inside a level once the lanes that
-// can still gain it are covered.  Halves the gathers of the level behind the peak and saves no time.
+// A row is always gathered to its end: stopping inside a row once the lanes that can still gain it are covered
+// halved the gathers of the level behind the peak but saved no time, since the level is bound by the latency chains
+// of its warps, not by the gathers alone.
 #pragma once
 
 #define PGQ_RANGE_CHUNKS 4
@@ -46,7 +47,6 @@ struct PullArgs {
 	PullGraph g;
 	int64_t nranges;      // ranges of the long part
 	int32_t gather_limit; // sources >= this cannot hold frontier bits in this level
-	int32_t hub_limit;    // HINT variant: masks of sources below this are kept in L1 (evict_last), all others bypass it
 	const u64 *visit;     // current frontier masks (read only)
 	u64 *seen;
 	u64 *cand;            // becomes the next frontier's visit array
@@ -94,75 +94,6 @@ __device__ __forceinline__ void ld_mask_rw(const u64 *base, int64_t idx, u64 (&m
 	}
 }
 
-// Mask gather with an L1 policy: the internal numbering puts the most gathered vertices first, so "u < hub_limit"
-// are the few thousand masks that serve a quarter of all gathers -- they are asked to stay in L1 (evict_last) while
-// every other mask, read about once per SM and level, does not allocate a line (no_allocate).
-template <int W, int HINT>
-__device__ __forceinline__ void ld_mask_hint(const u64 *__restrict__ base, int64_t idx, u64 (&m)[W], bool hot) {
-	const u64 *p = base + idx * W;
-	if constexpr (W == 4 && HINT == 1) {
-		if (hot) {
-			PGQ_LD4(".nc.L1::evict_last", p, m[0], m[1], m[2], m[3]);
-		} else {
-			PGQ_LD4(".nc.L1::no_allocate", p, m[0], m[1], m[2], m[3]);
-		}
-	} else if constexpr (W >= 4 && HINT == 2) { // (experiment: L2 eviction priorities on top, 32 B masks and wider only)
-		// sm_90 takes an L2 eviction priority only as a cache policy (createpolicy) handed to the load
-		u64 pol;
-		if (hot) {
-			asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-		} else {
-			asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-		}
-#pragma unroll
-		for (int i = 0; i < W; i += 4) {
-			if (hot) {
-				asm volatile("ld.global.nc.L1::evict_last.L2::cache_hint.v2.u64 {%0,%1}, [%4], %5;\n\t"
-				             "ld.global.nc.L1::evict_last.L2::cache_hint.v2.u64 {%2,%3}, [%4+16], %5;"
-				             : "=&l"(m[i]), "=&l"(m[i + 1]), "=&l"(m[i + 2]), "=&l"(m[i + 3])
-				             : "l"(p + i), "l"(pol));
-			} else {
-				asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%0,%1}, [%4], %5;\n\t"
-				             "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%2,%3}, [%4+16], %5;"
-				             : "=&l"(m[i]), "=&l"(m[i + 1]), "=&l"(m[i + 2]), "=&l"(m[i + 3])
-				             : "l"(p + i), "l"(pol));
-			}
-		}
-	} else if constexpr (HINT == 3) { // hub masks staged in shared memory (k_pull_fused_hub), all others bypass L1
-		if (hot) {
-			extern __shared__ __align__(128) unsigned char pull_smem[];
-			const u64 *q = reinterpret_cast<const u64 *>(pull_smem) + idx * W;
-			if constexpr (W == 1) {
-				m[0] = q[0];
-			} else {
-#pragma unroll
-				for (int i = 0; i < W; i += 2) {
-					const ulonglong2 t = *reinterpret_cast<const ulonglong2 *>(q + i);
-					m[i] = t.x;
-					m[i + 1] = t.y;
-				}
-			}
-		} else if constexpr (W == 1) {
-			asm volatile("ld.global.nc.L1::no_allocate.u64 %0, [%1];" : "=l"(m[0]) : "l"(p));
-		} else if constexpr (W == 2) {
-			asm volatile("ld.global.nc.L1::no_allocate.v2.u64 {%0,%1}, [%2];" : "=l"(m[0]), "=l"(m[1]) : "l"(p));
-		} else {
-#pragma unroll
-			for (int i = 0; i < W; i += 4) {
-				PGQ_LD4(".nc.L1::no_allocate", p + i, m[i], m[i + 1], m[i + 2], m[i + 3]);
-			}
-		}
-	} else {
-		ld_mask<W>(base, idx, m);
-	}
-}
-
-__device__ __forceinline__ int ld_adj_stream(const int32_t *p) { // the 4 B/edge stream: read once, never again
-	int v;
-	asm volatile("ld.global.nc.L1::no_allocate.s32 %0, [%1];" : "=r"(v) : "l"(p));
-	return v;
-}
-
 __device__ __forceinline__ bool sat_bit(const uint32_t *bits, int64_t k) {
 	return (bits[k >> 5] >> (k & 31)) & 1u;
 }
@@ -172,9 +103,9 @@ __device__ __forceinline__ bool sat_bit(const uint32_t *bits, int64_t k) {
 // row's bit in the finished-rows bitmap.
 // (PATH: the discovery levels of the new bits are recorded here, by this one lane -- callers that have a whole
 // warp at hand pass PATH = false and record cooperatively, record_levels_warp.)  On return val = the new bits.
-template <int W, bool PATH, bool HAVE_SEEN = false>
+template <int W, bool PATH>
 __device__ __forceinline__ void pull_update_row(const PullArgs<W> &a, int row, u64 (&val)[W], bool finished,
-                                                int64_t satpos, PullTotals<W> &tot, u64 *seen_row = nullptr) {
+                                                int64_t satpos, PullTotals<W> &tot) {
 	if (finished) { // (both mask buffers hold zeros for it, or k_pull_finish is about to see to that)
 #pragma unroll
 		for (int i = 0; i < W; i++) {
@@ -183,14 +114,7 @@ __device__ __forceinline__ void pull_update_row(const PullArgs<W> &a, int row, u
 		return;
 	}
 	u64 sn[W];
-	if constexpr (HAVE_SEEN) {
-#pragma unroll
-		for (int i = 0; i < W; i++) {
-			sn[i] = seen_row[i];
-		}
-	} else {
-		ld_mask_rw<W>(a.seen, row, sn);
-	}
+	ld_mask_rw<W>(a.seen, row, sn);
 	bool any_new = false, now_sat = true;
 #pragma unroll
 	for (int i = 0; i < W; i++) {
@@ -268,7 +192,7 @@ __device__ __forceinline__ void pull_totals_flush(PullTotals<W> &tot, LevelStatu
 }
 
 // ---- one slice of 32 short rows: lane = row, column j = the rows' j-th in-neighbours ------------------------
-template <int W, int G, bool PATH, int HINT, bool EXIT = false>
+template <int W, int G, bool PATH>
 __device__ __forceinline__ void pull_short_slice(const PullArgs<W> &a, int64_t s, int lane, PullTotals<W> &tot) {
 	const int64_t satpos = a.short_base + s * 32 + lane;
 	bool fin = false;
@@ -289,72 +213,35 @@ __device__ __forceinline__ void pull_short_slice(const PullArgs<W> &a, int64_t s
 	for (int i = 0; i < W; i++) {
 		acc[i] = 0;
 	}
-	// EXIT: the lane's row can gain only the bits need = live & ~seen (a lane whose frontier is empty has no bit
-	// in any visit mask); once the gathered OR covers them, the rest of the row cannot change the result.
-	u64 sn[W];
-	bool full = false; // early exit reached: no more gathers for this lane's row
-	if constexpr (EXIT) {
-		if (!fin && row >= 0) {
-			ld_mask_rw<W>(a.seen, row, sn);
-		} else {
+	const int32_t *col = a.g.s_adj + begin + lane;
+	for (int j0 = 0; j0 < width; j0 += G) {
+		int u[G];
+#pragma unroll
+		for (int j = 0; j < G; j++) {
+			u[j] = (j0 + j < width) ? col[(j0 + j) * 32] : -1;
+		}
+		u64 mv[G][W];
+#pragma unroll
+		for (int j = 0; j < G; j++) {
 #pragma unroll
 			for (int i = 0; i < W; i++) {
-				sn[i] = ~0ull;
+				mv[j][i] = 0;
+			}
+			if (!fin && (unsigned)u[j] < (unsigned)a.gather_limit) { // (padding is -1)
+				tot.gathers++;
+				ld_mask<W>(a.visit, u[j], mv[j]);
 			}
 		}
-	}
-	{
-		const int32_t *col = a.g.s_adj + begin + lane;
-		for (int j0 = 0; j0 < width; j0 += G) {
-			if constexpr (EXIT) {
-				if (__all_sync(FULL_MASK, fin || full || row < 0)) {
-					break;
-				}
-			}
-			int u[G];
 #pragma unroll
-			for (int j = 0; j < G; j++) {
-				u[j] = (j0 + j < width) ? (HINT != 0 ? ld_adj_stream(col + (j0 + j) * 32) : col[(j0 + j) * 32]) : -1;
-			}
-			u64 mv[G][W];
+		for (int j = 0; j < G; j++) {
 #pragma unroll
-			for (int j = 0; j < G; j++) {
-#pragma unroll
-				for (int i = 0; i < W; i++) {
-					mv[j][i] = 0;
-				}
-				if (!fin && !(EXIT && full) && (unsigned)u[j] < (unsigned)a.gather_limit) { // (padding is -1)
-					tot.gathers++;
-					if constexpr (HINT != 0) {
-						ld_mask_hint<W, HINT>(a.visit, u[j], mv[j], u[j] < a.hub_limit);
-					} else {
-						ld_mask<W>(a.visit, u[j], mv[j]);
-					}
-				}
-			}
-#pragma unroll
-			for (int j = 0; j < G; j++) {
-#pragma unroll
-				for (int i = 0; i < W; i++) {
-					acc[i] |= mv[j][i];
-				}
-			}
-			if constexpr (EXIT) {
-				bool covered = true;
-#pragma unroll
-				for (int i = 0; i < W; i++) {
-					covered &= (a.live.w[i] & ~sn[i] & ~acc[i]) == 0;
-				}
-				full = covered;
+			for (int i = 0; i < W; i++) {
+				acc[i] |= mv[j][i];
 			}
 		}
 	}
 	if (row >= 0) {
-		if constexpr (EXIT) {
-			pull_update_row<W, false, true>(a, row, acc, fin, satpos, tot, sn); // acc becomes the row's new bits
-		} else {
-			pull_update_row<W, false>(a, row, acc, fin, satpos, tot);
-		}
+		pull_update_row<W, false>(a, row, acc, fin, satpos, tot); // acc becomes the row's new bits
 	}
 	if (PATH) { // the warp records the rows' discovery levels together, one row at a time (coalesced 2-byte stores)
 		bool mine = false;
@@ -384,79 +271,38 @@ __device__ __forceinline__ void pull_short_slice(const PullArgs<W> &a, int64_t s
 	}
 }
 
-// ---- bulk async copies (TMA engine, cp.async.bulk -> UBLKCP) of the neighbour-id stream into shared memory ------
-// A warp keeps two 1 KB stages: while it gathers for one chunk (256 neighbour ids), the copy engine brings its
-// next chunk in, so the only global loads the warp itself issues for the long rows are the mask gathers.
-#define PGQ_CHUNK_BYTES (PGQ_CHUNK * 4)
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) {
-	return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(uint64_t *bar) {
-	asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(bar)));
-}
-// one lane: announce the bytes, start the copy global -> shared; completion arrives on the barrier
-__device__ __forceinline__ void bulk_load(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
-	asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-	asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-	             "l"(src), "r"(bytes), "r"(smem_u32(bar))
-	             : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-	asm volatile("{\n"
-	             ".reg .pred p;\n"
-	             "WAIT_%=:\n"
-	             "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-	             "@p bra DONE_%=;\n"
-	             "bra WAIT_%=;\n"
-	             "DONE_%=:\n"
-	             "}" ::"r"(smem_u32(bar)),
-	             "r"(parity)
-	             : "memory");
-}
-
-struct AdjPipe {
-	int32_t *stage = nullptr; // two stages of PGQ_CHUNK ids; nullptr = no staging (plain LDG)
-	uint64_t *bar = nullptr;
-	uint32_t parity0 = 0, parity1 = 0;
-	int cur = 0;
-};
-
 // ---- one range of the long rows ---------------------------------------------------------------------------------
-template <int W, int G, bool PATH, bool BULK, int HINT, bool EXIT = false>
-__device__ __forceinline__ void pull_long_range(const PullArgs<W> &a, int64_t range, int64_t next_range, int lane,
-                                                PullTotals<W> &tot, AdjPipe &pipe) {
+template <int W, int G, bool PATH>
+__device__ __forceinline__ void pull_long_range(const PullArgs<W> &a, int64_t range, int lane, PullTotals<W> &tot) {
 	const int64_t head_words = a.g.nchunks * PGQ_STEPS;
 	const int64_t c0 = range * PGQ_RANGE_CHUNKS;
 	const int64_t base = c0 * PGQ_CHUNK;
-	if constexpr (!BULK) {
-		if (a.skip) {
-			// the rows that touch this range are the ranks kf .. kl (chunk_rank = rank of the row that covers a
-			// chunk's first position): if all their finished bits are set there is nothing to do here
-			const int64_t nc0 = c0 + PGQ_RANGE_CHUNKS;
-			const int kf = a.g.chunk_rank[c0];
-			const int kl = (nc0 >= a.g.nchunks) ? (int)a.g.n_rows - 1
-			                                    : a.g.chunk_rank[nc0] - (int)(a.g.head[nc0 * PGQ_STEPS] & 1u);
-			bool ok = true;
-			for (int w0 = kf >> 5; w0 <= (kl >> 5); w0 += 32) {
-				const int w = w0 + lane;
-				if (w <= (kl >> 5)) {
-					uint32_t need = 0xffffffffu;
-					if (w == (kf >> 5)) {
-						need &= 0xffffffffu << (kf & 31);
-					}
-					if (w == (kl >> 5)) {
-						need &= 0xffffffffu >> (31 - (kl & 31));
-					}
-					ok &= (a.satbits[w] & need) == need;
+	if (a.skip) {
+		// the rows that touch this range are the ranks kf .. kl (chunk_rank = rank of the row that covers a
+		// chunk's first position): if all their finished bits are set there is nothing to do here
+		const int64_t nc0 = c0 + PGQ_RANGE_CHUNKS;
+		const int kf = a.g.chunk_rank[c0];
+		const int kl = (nc0 >= a.g.nchunks) ? (int)a.g.n_rows - 1
+		                                    : a.g.chunk_rank[nc0] - (int)(a.g.head[nc0 * PGQ_STEPS] & 1u);
+		bool ok = true;
+		for (int w0 = kf >> 5; w0 <= (kl >> 5); w0 += 32) {
+			const int w = w0 + lane;
+			if (w <= (kl >> 5)) {
+				uint32_t need = 0xffffffffu;
+				if (w == (kf >> 5)) {
+					need &= 0xffffffffu << (kf & 31);
 				}
-			}
-			if (__all_sync(FULL_MASK, ok)) {
-				if (lane == 31) {
-					a.shared_row[range] = -1;
+				if (w == (kl >> 5)) {
+					need &= 0xffffffffu >> (31 - (kl & 31));
 				}
-				return;
+				ok &= (a.satbits[w] & need) == need;
 			}
+		}
+		if (__all_sync(FULL_MASK, ok)) {
+			if (lane == 31) {
+				a.shared_row[range] = -1;
+			}
+			return;
 		}
 	}
 	const int64_t hw_idx = c0 * PGQ_STEPS + lane;
@@ -473,30 +319,6 @@ __device__ __forceinline__ void pull_long_range(const PullArgs<W> &a, int64_t ra
 	if (a.skip && open_valid) {
 		open_sat = sat_bit(a.satbits, running);
 	}
-	// EXIT: lane i < W holds word i of need = live & ~seen[open row] from the row's first head-less group on;
-	// once the warp's gathered OR covers it, the rest of the row (inside this range) is not gathered any more.
-	bool open_full = false, need_valid = false;
-	u64 need_word = 0;
-	if constexpr (EXIT) {
-		// A range that starts deep inside a row (no head in its first chunk) is a continuation range of a hub row:
-		// the kernel runs those after all others, so the ranges in front of it have usually published their part
-		// of the row's OR in cand already -- what they found need not be found again, and if nothing is missing the
-		// whole open part is skipped.  (Stale or partial values of cand only make the test more conservative.)
-		if (open_valid && !open_sat && (headmask & 0xffu) == 0u) {
-			const int orow = a.g.row[running];
-			const int wsel = lane & (W - 1);
-			u64 lw = a.live.w[0];
-#pragma unroll
-			for (int i = 1; i < W; i++) {
-				lw = (wsel == i) ? a.live.w[i] : lw;
-			}
-			const u64 sw = __ldcg(a.seen + (int64_t)orow * W + wsel);
-			const u64 cw = __ldcg(a.cand + (int64_t)orow * W + wsel);
-			need_word = lw & ~sw & ~cw;
-			need_valid = true;
-			open_full = !__any_sync(FULL_MASK, need_word != 0);
-		}
-	}
 	int shared = -1; // (lane 31) rank of the row that ends here but began in an earlier range
 	u64 acc[W];
 #pragma unroll
@@ -510,60 +332,20 @@ __device__ __forceinline__ void pull_long_range(const PullArgs<W> &a, int64_t ra
 			break;
 		}
 		const uint32_t chunk_heads = (headmask >> (c * PGQ_STEPS)) & 0xffu;
-		const int32_t *staged = nullptr;
-		if constexpr (BULK) {
-			// the copy of THIS chunk was started one chunk ago; start the copy of the warp's next chunk, then wait
-			int64_t nbase = cbase + PGQ_CHUNK; // next chunk of this range ...
-			if (c + 1 == PGQ_RANGE_CHUNKS || nbase >= a.g.m) {
-				nbase = (next_range >= 0) ? next_range * PGQ_RANGE_CHUNKS * PGQ_CHUNK : -1; // ... or the first of the next one
-			}
-			__syncwarp(); // every lane is done reading the stage that is about to be overwritten
-			if (nbase >= 0 && lane == 0) {
-				asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-				bulk_load(pipe.stage + (pipe.cur ^ 1) * PGQ_CHUNK, a.g.adj + nbase, PGQ_CHUNK_BYTES, &pipe.bar[pipe.cur ^ 1]);
-			}
-			if (pipe.cur == 0) {
-				mbar_wait(&pipe.bar[0], pipe.parity0);
-				pipe.parity0 ^= 1u;
-			} else {
-				mbar_wait(&pipe.bar[1], pipe.parity1);
-				pipe.parity1 ^= 1u;
-			}
-			staged = pipe.stage + pipe.cur * PGQ_CHUNK;
-			pipe.cur ^= 1;
-		}
-		if (chunk_heads == 0u && (open_sat || (EXIT && open_full))) {
+		if (chunk_heads == 0u && open_sat) {
 			continue; // the whole chunk lies inside a finished row: its neighbour ids are not looked at
 		}
-		int u[PGQ_STEPS]; // the chunk's neighbour ids: 8 coalesced 128 B loads in flight, or 8 LDS from the stage
+		int u[PGQ_STEPS]; // the chunk's neighbour ids: 8 coalesced 128 B loads in flight
 #pragma unroll
 		for (int k = 0; k < PGQ_STEPS; k++) {
 			const int64_t e = cbase + 32 * k + lane;
-			if constexpr (BULK) {
-				u[k] = (e < a.g.m) ? staged[32 * k + lane] : -1;
-			} else {
-				u[k] = (e < a.g.m) ? (HINT != 0 ? ld_adj_stream(a.g.adj + e) : a.g.adj[e]) : -1;
-			}
+			u[k] = (e < a.g.m) ? a.g.adj[e] : -1;
 		}
 #pragma unroll
 		for (int k0 = 0; k0 < PGQ_STEPS; k0 += G) {
 			if (((chunk_heads >> k0) & ((1u << G) - 1u)) == 0u) {
 				// ---- fast path: all G steps continue the open row
-				if (!open_sat && !(EXIT && open_full)) {
-					if constexpr (EXIT) {
-						if (!need_valid) { // (in flight together with the gathers below)
-							const int orow = a.g.row[running];
-							const int wsel = lane & (W - 1);
-							u64 sw, lw = a.live.w[0];
-							asm volatile("ld.global.u64 %0, [%1];" : "=l"(sw) : "l"(a.seen + (int64_t)orow * W + wsel));
-#pragma unroll
-							for (int i = 1; i < W; i++) {
-								lw = (wsel == i) ? a.live.w[i] : lw;
-							}
-							need_word = lw & ~sw;
-							need_valid = true;
-						}
-					}
+				if (!open_sat) {
 					u64 mv[G][W];
 #pragma unroll
 					for (int j = 0; j < G; j++) {
@@ -573,11 +355,7 @@ __device__ __forceinline__ void pull_long_range(const PullArgs<W> &a, int64_t ra
 						}
 						if ((unsigned)u[k0 + j] < (unsigned)a.gather_limit) {
 							tot.gathers++;
-							if constexpr (HINT != 0) {
-								ld_mask_hint<W, HINT>(a.visit, u[k0 + j], mv[j], u[k0 + j] < a.hub_limit);
-							} else {
-								ld_mask<W>(a.visit, u[k0 + j], mv[j]);
-							}
+							ld_mask<W>(a.visit, u[k0 + j], mv[j]);
 						}
 					}
 #pragma unroll
@@ -586,15 +364,6 @@ __device__ __forceinline__ void pull_long_range(const PullArgs<W> &a, int64_t ra
 						for (int i = 0; i < W; i++) {
 							acc[i] |= mv[j][i];
 						}
-					}
-					if constexpr (EXIT) {
-						u64 mine = 0; // word (lane & (W-1)) of the warp's OR so far
-#pragma unroll
-						for (int i = 0; i < W; i++) {
-							const u64 f = warp_or(acc[i]);
-							mine = ((lane & (W - 1)) == i) ? f : mine;
-						}
-						open_full = !__any_sync(FULL_MASK, (need_word & ~mine) != 0);
 					}
 				}
 				continue;
@@ -618,7 +387,7 @@ __device__ __forceinline__ void pull_long_range(const PullArgs<W> &a, int64_t ra
 			}
 			u64 mv[G][W];
 			{
-				bool cur_sat = open_sat || (EXIT && open_full);
+				bool cur_sat = open_sat;
 #pragma unroll
 				for (int j = 0; j < G; j++) {
 					const uint32_t h = hs[j];
@@ -629,11 +398,7 @@ __device__ __forceinline__ void pull_long_range(const PullArgs<W> &a, int64_t ra
 					}
 					if (!mine_sat && (unsigned)u[k0 + j] < (unsigned)a.gather_limit) {
 						tot.gathers++;
-						if constexpr (HINT != 0) {
-							ld_mask_hint<W, HINT>(a.visit, u[k0 + j], mv[j], u[k0 + j] < a.hub_limit);
-						} else {
-							ld_mask<W>(a.visit, u[k0 + j], mv[j]);
-						}
+						ld_mask<W>(a.visit, u[k0 + j], mv[j]);
 					}
 					if (h != 0u) {
 						cur_sat = sat_new[j];
@@ -687,8 +452,6 @@ __device__ __forceinline__ void pull_long_range(const PullArgs<W> &a, int64_t ra
 				open_valid = true;
 				open_began = true;
 				open_sat = sat_new[j];
-				open_full = false;
-				need_valid = false;
 #pragma unroll
 				for (int i = 0; i < W; i++) {
 					acc[i] = (lane >= first) ? mv[j][i] : 0;
@@ -729,103 +492,23 @@ __device__ __forceinline__ void pull_long_range(const PullArgs<W> &a, int64_t ra
 	}
 }
 
-template <int W, int G, int MB, bool PATH, bool BULK, int HINT = 0, bool EXIT = false>
-__global__ void __launch_bounds__(256, MB) k_pull_fused(const PullArgs<W> a) {
-	extern __shared__ __align__(128) unsigned char pull_smem[]; // BULK: per warp two 1 KB stages, then the barriers
+// 256 threads per block, PGQ_PULL_CTAS blocks per SM: at most 80 registers per thread
+#define PGQ_PULL_CTAS 3
+template <int W, bool PATH>
+__global__ void __launch_bounds__(256, PGQ_PULL_CTAS) k_pull_fused(const PullArgs<W> a) {
+	// mask gathers in flight per lane: steps of a long-row range on the fast path, columns of a short-row slice
+	constexpr int G = (W >= 8) ? 1 : ((W >= 4) ? 2 : 4);
+	constexpr int GS = (W >= 8) ? 2 : 4;
 	const int lane = threadIdx.x & 31;
 	const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
 	const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
 	PullTotals<W> tot;
-	AdjPipe pipe;
-	if constexpr (BULK) {
-		const int wib = threadIdx.x >> 5;
-		pipe.stage = reinterpret_cast<int32_t *>(pull_smem) + wib * 2 * PGQ_CHUNK;
-		pipe.bar = reinterpret_cast<uint64_t *>(pull_smem + 8 * 2 * PGQ_CHUNK_BYTES) + wib * 2;
-		if (lane == 0) {
-			mbar_init(&pipe.bar[0]);
-			mbar_init(&pipe.bar[1]);
-			asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-			if (warp < a.nranges) { // the first chunk of the warp's first range
-				bulk_load(pipe.stage, a.g.adj + warp * PGQ_RANGE_CHUNKS * PGQ_CHUNK, PGQ_CHUNK_BYTES, &pipe.bar[0]);
-			}
-		}
-		__syncwarp();
-	}
-	const int64_t items = a.nranges + a.g.n_slices;
-	if constexpr (EXIT && !BULK) {
-		// pass 0: the ranges with a row head in their first chunk; pass 1: continuation ranges of hub rows (see
-		// pull_long_range); then the short rows
-		// (work is handed out by tickets: rows that exit early make the ranges very unequal)
-		const int64_t head_words = a.g.nchunks * PGQ_STEPS;
-		for (int pass = 0; pass < 2; pass++) {
-			for (;;) {
-				unsigned t = 0;
-				if (lane == 0) {
-					t = atomicAdd(&a.st->pull_ticket[pass], 1u);
-				}
-				const int64_t it = __shfl_sync(FULL_MASK, t, 0);
-				if (it >= a.nranges) {
-					break;
-				}
-				const int64_t hi = it * PGQ_RANGE_STEPS + lane;
-				const uint32_t w0 = (lane < PGQ_STEPS && hi < head_words) ? a.g.head[hi] : 0u;
-				const int cls = __any_sync(FULL_MASK, w0 != 0u) ? 0 : 1;
-				if (cls == pass) {
-					pull_long_range<W, G, PATH, BULK, HINT, EXIT>(a, it, -1, lane, tot, pipe);
-				}
-			}
-		}
-		for (;;) {
-			unsigned t = 0;
-			if (lane == 0) {
-				t = atomicAdd(&a.st->pull_ticket[2], 1u);
-			}
-			const int64_t it = __shfl_sync(FULL_MASK, t, 0);
-			if (it >= a.g.n_slices) {
-				break;
-			}
-			pull_short_slice<W, (W >= 8 ? 2 : 4), PATH, HINT, EXIT>(a, it, lane, tot);
-		}
-	} else {
-		for (int64_t it = warp; it < items; it += nwarps) {
-			if (it < a.nranges) {
-				const int64_t nxt = (it + nwarps < a.nranges) ? it + nwarps : -1;
-				pull_long_range<W, G, PATH, BULK, HINT, EXIT>(a, it, nxt, lane, tot, pipe);
-			} else {
-				pull_short_slice<W, (W >= 8 ? 2 : 4), PATH, HINT, EXIT>(a, it - a.nranges, lane, tot);
-			}
-		}
-	}
-	pull_totals_flush<W>(tot, a.st);
-}
-
-// The same level with the masks of the first `hub_limit` vertices of the internal numbering -- the most gathered
-// ones: on R-MAT-22 the first 7168 serve 32 % of all gathers -- staged in shared memory: one CTA of 24 warps per SM
-// copies them in (coalesced, 224 KB) and serves those gathers with LDS instead of an L1-missing sector request.
-#define PGQ_HUB_SMEM_BYTES 229376
-template <int W, int G, bool PATH>
-__global__ void __launch_bounds__(768, 1) k_pull_fused_hub(const PullArgs<W> a) {
-	extern __shared__ __align__(128) unsigned char pull_smem[];
-	{
-		const uint4 *from = reinterpret_cast<const uint4 *>(a.visit);
-		uint4 *to = reinterpret_cast<uint4 *>(pull_smem);
-		const int n16 = a.hub_limit * W / 2;
-		for (int i = threadIdx.x; i < n16; i += blockDim.x) {
-			to[i] = __ldg(from + i);
-		}
-	}
-	__syncthreads();
-	const int lane = threadIdx.x & 31;
-	const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-	const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-	PullTotals<W> tot;
-	AdjPipe pipe;
 	const int64_t items = a.nranges + a.g.n_slices;
 	for (int64_t it = warp; it < items; it += nwarps) {
 		if (it < a.nranges) {
-			pull_long_range<W, G, PATH, false, 3>(a, it, -1, lane, tot, pipe);
+			pull_long_range<W, G, PATH>(a, it, lane, tot);
 		} else {
-			pull_short_slice<W, (W >= 8 ? 2 : 4), PATH, 3>(a, it - a.nranges, lane, tot);
+			pull_short_slice<W, GS, PATH>(a, it - a.nranges, lane, tot);
 		}
 	}
 	pull_totals_flush<W>(tot, a.st);

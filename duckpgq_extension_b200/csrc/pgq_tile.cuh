@@ -17,29 +17,15 @@ struct ChunkWalker {
 	int64_t base; // first position of the chunk
 
 	__device__ __forceinline__ ChunkWalker(const DirGraph &g, int64_t chunk, int lane) {
-		uint32_t w;
-		int r0;
-		fetch(g, chunk, lane, w, r0);
-		init(chunk, w, r0);
-	}
-	// the two loads a chunk starts with, separable so that a kernel can issue them for its NEXT chunk
-	// while it still works on the current one
-	static __device__ __forceinline__ void fetch(const DirGraph &g, int64_t chunk, int lane, uint32_t &w, int &r0) {
-		w = 1u;
-		r0 = 0;
+		hw = 1u;
+		int r0 = 0;
 		if (chunk < g.nchunks) {
 			if (lane < PGQ_STEPS || (lane == PGQ_STEPS && chunk + 1 < g.nchunks)) {
-				w = g.head[chunk * PGQ_STEPS + lane];
+				hw = g.head[chunk * PGQ_STEPS + lane];
 			}
 			r0 = g.chunk_rank[chunk];
 		}
-	}
-	__device__ __forceinline__ ChunkWalker(int64_t chunk, uint32_t w, int r0) {
-		init(chunk, w, r0);
-	}
-	__device__ __forceinline__ void init(int64_t chunk, uint32_t w, int r0) {
 		base = chunk * PGQ_CHUNK;
-		hw = w;
 		uint32_t h0 = __shfl_sync(FULL_MASK, hw, 0);
 		running = r0 - (int)(h0 & 1u);
 	}

@@ -166,7 +166,7 @@ def make_pairs(g, k, seed):
     return ps[order], pd[order], sv[order]
 
 
-def check_trace(text, schedule, no_tail=False, legacy_pull=False):
+def check_trace(text, schedule, no_tail=False):
     """Every level line of the trace ran what the schedule asked for; returns the level-to-level transitions seen.
     A t level runs top-down only where k_tail is not eligible.  After a fused bottom-up level the frontier has no
     item list yet, and eligibility is judged on the bound fv + fe / 256 of its length."""
@@ -174,7 +174,7 @@ def check_trace(text, schedule, no_tail=False, legacy_pull=False):
     seen = set()
     prev = None
     for b, lv, kind, fv, fe, items in lines:
-        after_pull = prev is not None and prev[:2] == (b, lv - 1) and prev[2] == "pull" and not legacy_pull
+        after_pull = prev is not None and prev[:2] == (b, lv - 1) and prev[2] == "pull"
         if after_pull:
             items = fv + fe // 256
         want = schedule[(lv - 1) % len(schedule)]
@@ -253,15 +253,14 @@ def test_alpha_matches_oracle(graphs, monkeypatch, graph, alpha):
 
 
 VARIANT_SCHEDULES = ["bp", "pb", "tb", "bt", "bbp", "tbp", "bbbt", "ppbb"] + RANDOM[:4]
-VARIANTS = [{"PGQ_B200_PULL_SKIP": "0"}, {"PGQ_B200_PULL": "17"}, {"PGQ_B200_PULL": "5"}, {"PGQ_B200_NO_TAIL": "1"}]
+VARIANTS = [{"PGQ_B200_PULL_SKIP": "0"}, {"PGQ_B200_NO_TAIL": "1"}]
 
 
 @pytest.mark.parametrize("variant", VARIANTS, ids=lambda v: "-".join(f"{k[9:]}={x}" for k, x in v.items()))
 @pytest.mark.parametrize("schedule", VARIANT_SCHEDULES)
 @pytest.mark.parametrize("graph", ["indeg", "snb", "rmat12"])
 def test_variant_schedule_matches_oracle(graphs, monkeypatch, capfd, graph, schedule, variant):
-    """Without skipping finished rows, the in-row early exit (from the 2nd bottom-up level on, also after top-down
-    levels), the legacy pull + k_update_dense pair, and no k_tail."""
+    """Without skipping finished rows, and without k_tail."""
     g = graphs(graph)
     _set_env(monkeypatch, schedule, **variant)
     capfd.readouterr()
@@ -271,8 +270,7 @@ def test_variant_schedule_matches_oracle(graphs, monkeypatch, capfd, graph, sche
         run_lengths(g, ps, pd, sv, lanes, rb)
     ps, pd, sv = make_pairs(g, 64, seed=seed)
     run_paths(g, ps, pd, sv, 64, seed % 2 == 0)
-    check_trace(capfd.readouterr().err, schedule, no_tail="PGQ_B200_NO_TAIL" in variant,
-                legacy_pull=variant.get("PGQ_B200_PULL") == "5")
+    check_trace(capfd.readouterr().err, schedule, no_tail="PGQ_B200_NO_TAIL" in variant)
 
 
 @pytest.mark.parametrize("schedule", ["a", "t", "pt", "tb", "bt", "p"])

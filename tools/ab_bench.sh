@@ -1,7 +1,7 @@
 #!/usr/bin/env bash
 # Interleaved A/B runs of bench.py on ONE box (run-to-run noise between boxes is larger than most kernel effects):
 #   tools/ab_bench.sh <out-prefix> <rounds> "ENV_A" "ENV_B" ...
-# e.g. tools/ab_bench.sh /tmp/ab 2 "" "PGQ_B200_PULL=17" "PGQ_B200_FIXED_ALPHA=1"
+# e.g. tools/ab_bench.sh /tmp/ab 2 "" "PGQ_B200_PULL_SKIP=0"
 # writes <out-prefix>_<variant index>_<round>.json (the bench line) and prints pairs/s, ms per step and the
 # bottom-up level's average time per variant.
 set -euo pipefail

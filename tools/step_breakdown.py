@@ -28,11 +28,11 @@ if ROOT not in sys.path:
 from duckpgq_extension_b200 import datagen  # noqa: E402
 
 # kernels that expand a frontier; everything else on the device is the level loop's overhead
-EXPANSION = ("k_pull_fused", "k_expand_push", "k_expand_pull", "k_tail")
+EXPANSION = ("k_pull_fused", "k_expand_push", "k_tail")
 
 
 def short_name(name: str) -> str:
-    """'void k_pull_fused<4, 1, 3, false, false, 0>(PullArgs<4>)' -> 'k_pull_fused<4, 1, 3, false, false, 0>'"""
+    """'void k_pull_fused<4, false>(PullArgs<4>)' -> 'k_pull_fused<4, false>'"""
     name = re.sub(r"^void\s+", "", name)
     depth = 0
     for i, ch in enumerate(name):
