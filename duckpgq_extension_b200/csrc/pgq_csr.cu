@@ -451,7 +451,7 @@ int pgq_scan_exclusive_i32(const int32_t *in, int32_t *out, int64_t count, int32
 }
 
 // ------------------------------------------------------------------------------------------------
-// stable LSD radix sort of (int32 key, int32 value) pairs, 5 bits per pass
+// stable LSD radix sort of (int32 or uint64 key, int32 value) pairs, 5 bits per pass
 //   pass = per-tile digit histogram -> exclusive scan (digit-major, tile-minor) -> stable scatter.
 // Stability is what makes the device CSR equal the reference's: edges of one source keep their
 // arrival order (csr_creation.cpp:132-139 with one feeding thread).
@@ -462,7 +462,8 @@ int pgq_scan_exclusive_i32(const int32_t *in, int32_t *out, int64_t count, int32
 #define RS_ITEMS 8
 #define RS_TILE (RS_THREADS * RS_ITEMS)
 
-__global__ void __launch_bounds__(RS_THREADS) k_rs_hist(const int32_t *__restrict__ keys, int64_t count, int shift,
+template <typename K>
+__global__ void __launch_bounds__(RS_THREADS) k_rs_hist(const K *__restrict__ keys, int64_t count, int shift,
                                                         int32_t *__restrict__ hist, int nblocks) {
 	__shared__ int bins[RS_BINS];
 	if (threadIdx.x < RS_BINS) {
@@ -474,7 +475,7 @@ __global__ void __launch_bounds__(RS_THREADS) k_rs_hist(const int32_t *__restric
 	for (int j = 0; j < RS_ITEMS; j++) {
 		const int64_t i = base + j * RS_THREADS + threadIdx.x; // any order will do for counting
 		if (i < count) {
-			atomicAdd(&bins[(keys[i] >> shift) & (RS_BINS - 1)], 1);
+			atomicAdd(&bins[(int)((keys[i] >> shift) & (RS_BINS - 1))], 1);
 		}
 	}
 	__syncthreads();
@@ -483,15 +484,17 @@ __global__ void __launch_bounds__(RS_THREADS) k_rs_hist(const int32_t *__restric
 	}
 }
 
-__global__ void __launch_bounds__(RS_THREADS) k_rs_scatter(const int32_t *__restrict__ keys_in,
+template <typename K>
+__global__ void __launch_bounds__(RS_THREADS) k_rs_scatter(const K *__restrict__ keys_in,
                                                            const int32_t *__restrict__ vals_in,
-                                                           int32_t *__restrict__ keys_out, int32_t *__restrict__ vals_out,
+                                                           K *__restrict__ keys_out, int32_t *__restrict__ vals_out,
                                                            int64_t count, int shift, const int32_t *__restrict__ offs,
                                                            int nblocks) {
 	__shared__ int cnt[RS_BINS][RS_THREADS]; // per-thread digit counts, then prefixes over the threads
 	const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
 	const int64_t base = (int64_t)blockIdx.x * RS_TILE + (int64_t)t * RS_ITEMS; // a thread owns 8 consecutive pairs
-	int k[RS_ITEMS], v[RS_ITEMS], local[RS_ITEMS];
+	K k[RS_ITEMS];
+	int v[RS_ITEMS], local[RS_ITEMS];
 #pragma unroll
 	for (int d = 0; d < RS_BINS; d++) {
 		cnt[d][t] = 0;
@@ -501,7 +504,7 @@ __global__ void __launch_bounds__(RS_THREADS) k_rs_scatter(const int32_t *__rest
 		if (base + j < count) {
 			k[j] = keys_in[base + j];
 			v[j] = vals_in[base + j];
-			const int d = (k[j] >> shift) & (RS_BINS - 1);
+			const int d = (int)((k[j] >> shift) & (RS_BINS - 1));
 			local[j] = cnt[d][t]; // rank among this thread's earlier pairs with the same digit
 			cnt[d][t] = local[j] + 1;
 		}
@@ -528,7 +531,7 @@ __global__ void __launch_bounds__(RS_THREADS) k_rs_scatter(const int32_t *__rest
 #pragma unroll
 	for (int j = 0; j < RS_ITEMS; j++) {
 		if (base + j < count) {
-			const int d = (k[j] >> shift) & (RS_BINS - 1);
+			const int d = (int)((k[j] >> shift) & (RS_BINS - 1));
 			const int64_t pos = (int64_t)offs[(int64_t)d * nblocks + blockIdx.x] + cnt[d][t] + local[j];
 			keys_out[pos] = k[j];
 			vals_out[pos] = v[j];
@@ -538,19 +541,21 @@ __global__ void __launch_bounds__(RS_THREADS) k_rs_scatter(const int32_t *__rest
 
 // Sorts by the low `end_bit` bits of the keys.  (keys_a, vals_a) hold the input and are clobbered;
 // the result is in (*keys_res, *vals_res), which is either the a or the b pair.
-int radix_sort_pairs(Workspace *ws, int32_t *keys_a, int32_t *keys_b, int32_t *vals_a, int32_t *vals_b, int64_t count,
-                     int end_bit, cudaStream_t s, int32_t **keys_res, int32_t **vals_res) {
+template <typename K>
+static int radix_sort_pairs_impl(Workspace *ws, K *keys_a, K *keys_b, int32_t *vals_a, int32_t *vals_b, int64_t count,
+                                 int end_bit, cudaStream_t s, K **keys_res, int32_t **vals_res) {
 	const int nblocks = (int)((count + RS_TILE - 1) / RS_TILE);
 	const int64_t hist_elems = (int64_t)RS_BINS * nblocks;
 	int32_t *hist, *scan_tmp;
 	PGQ_TRY(pgq_ws_reserve(ws, 14, (size_t)(hist_elems + 1) * sizeof(int32_t), (void **)&hist));
 	PGQ_TRY(pgq_ws_reserve(ws, 15, pgq_scan_tmp_elems(hist_elems) * sizeof(int32_t), (void **)&scan_tmp));
-	int32_t *kin = keys_a, *kout = keys_b, *vin = vals_a, *vout = vals_b;
+	K *kin = keys_a, *kout = keys_b;
+	int32_t *vin = vals_a, *vout = vals_b;
 	for (int shift = 0; shift < end_bit; shift += RS_BITS) {
-		k_rs_hist<<<nblocks, RS_THREADS, 0, s>>>(kin, count, shift, hist, nblocks);
+		k_rs_hist<K><<<nblocks, RS_THREADS, 0, s>>>(kin, count, shift, hist, nblocks);
 		PGQ_CUDA(cudaGetLastError());
 		PGQ_TRY(pgq_scan_exclusive_i32(hist, hist, hist_elems, scan_tmp, s));
-		k_rs_scatter<<<nblocks, RS_THREADS, 0, s>>>(kin, vin, kout, vout, count, shift, hist, nblocks);
+		k_rs_scatter<K><<<nblocks, RS_THREADS, 0, s>>>(kin, vin, kout, vout, count, shift, hist, nblocks);
 		PGQ_CUDA(cudaGetLastError());
 		std::swap(kin, kout);
 		std::swap(vin, vout);
@@ -558,6 +563,16 @@ int radix_sort_pairs(Workspace *ws, int32_t *keys_a, int32_t *keys_b, int32_t *v
 	*keys_res = kin;
 	*vals_res = vin;
 	return PGQ_OK;
+}
+
+int radix_sort_pairs(Workspace *ws, int32_t *keys_a, int32_t *keys_b, int32_t *vals_a, int32_t *vals_b, int64_t count,
+                     int end_bit, cudaStream_t s, int32_t **keys_res, int32_t **vals_res) {
+	return radix_sort_pairs_impl(ws, keys_a, keys_b, vals_a, vals_b, count, end_bit, s, keys_res, vals_res);
+}
+
+int radix_sort_pairs(Workspace *ws, uint64_t *keys_a, uint64_t *keys_b, int32_t *vals_a, int32_t *vals_b, int64_t count,
+                     int end_bit, cudaStream_t s, uint64_t **keys_res, int32_t **vals_res) {
+	return radix_sort_pairs_impl(ws, keys_a, keys_b, vals_a, vals_b, count, end_bit, s, keys_res, vals_res);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1772,6 +1787,295 @@ extern "C" int pgq_csr_build_device(pgq_ctx *ctx, int64_t n, int64_t m, const in
 	free_staging(csr);
 	*out = csr;
 	return PGQ_OK;
+}
+
+// ---- CSR from vertex-key and edge-key columns ------------------------------------------------------
+// The reference's directed CSR CTE (compressed_sparse_row.cpp:132-143,234-251) joins e.src and e.dst to v.id
+// only to turn keys into vertex rowids: degree(a) = count(k.src) over v a LEFT JOIN e k ON k.src = a.id, and
+// the rows handed to create_csr_edge are (a.rowid, c.rowid, k.rowid) of e k JOIN v a ON a.id = k.src JOIN v c
+// ON c.id = k.dst.  With ms(k) / md(k) = the number of vertex rows whose key equals k.src / k.dst (0 for a NULL
+// key), S = sum ms is the sum of the degrees and C = sum ms * md the number of rows; csr_creation.cpp:121-125
+// throws when S != C.  Here the (key, rowid) pairs of v are sorted on the device, every edge finds its two
+// ranges of matching vertex rows by binary search, and an edge with ms >= 1 must have md == 1: S == C alone
+// would let a dangling dst (md = 0) balance a duplicated one (md = 2), and the reference then scatters out
+// of place (DESIGN.md section 7).  Edge k becomes ms(k) rows, one per matching source row, at positions
+// given by an exclusive scan over ms -- in edge rowid order, which is the order the stable build keeps
+// within a source row.  The rows then take the pgq_csr_build_device path (finalize_from_rows).
+
+// an int64 key as an unsigned radix-sort key of the same order
+__device__ __forceinline__ uint64_t key_bits(int64_t k) {
+	return (uint64_t)k ^ 0x8000000000000000ull;
+}
+
+// flag[i] = 1 for a vertex row with a non-NULL key, flag[n] = 0: its exclusive scan numbers the valid rows
+__global__ void k_key_valid(const uint8_t *__restrict__ valid, int64_t n, int32_t *__restrict__ flag) {
+	for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (int64_t)gridDim.x * blockDim.x) {
+		flag[i] = (i < n && (!valid || valid[i])) ? 1 : 0;
+	}
+}
+
+// The nv = pos[n] valid rows go to [0, nv) in rowid order, the NULL rows behind them with the largest sort key:
+// a stable sort keeps them behind every valid row (a valid INT64_MAX key included), so the searches below look
+// at [0, nv) only.
+__global__ void k_key_pairs(const int64_t *__restrict__ keys, const uint8_t *__restrict__ valid, int64_t n,
+                            const int32_t *__restrict__ pos, uint64_t *__restrict__ key_out,
+                            int32_t *__restrict__ row_out) {
+	const int64_t nv = pos[n];
+	for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+		const bool ok = !valid || valid[i];
+		const int64_t p = ok ? pos[i] : nv + (i - pos[i]);
+		key_out[p] = ok ? key_bits(keys[i]) : ~0ull;
+		row_out[p] = (int32_t)i;
+	}
+}
+
+// [lo, hi) = the entries of the sorted a[0, n) equal to x.  Most keys are unique, so the end of the range is
+// found by galloping from lo rather than by a second full binary search.
+__device__ __forceinline__ int key_range(const uint64_t *__restrict__ a, int n, uint64_t x, int *hi) {
+	int lo = 0, len = n;
+	while (len > 0) {
+		const int half = len >> 1;
+		if (a[lo + half] < x) {
+			lo += half + 1;
+			len -= half + 1;
+		} else {
+			len = half;
+		}
+	}
+	if (lo >= n || a[lo] != x) {
+		*hi = lo;
+		return lo;
+	}
+	int good = lo, step = 1; // a[good] == x
+	while (good + step < n && a[good + step] == x) {
+		good += step;
+		step <<= 1;
+	}
+	int bad = min(good + step, n); // a[bad] != x or bad == n
+	while (bad - good > 1) {
+		const int mid = good + ((bad - good) >> 1);
+		if (a[mid] == x) {
+			good = mid;
+		} else {
+			bad = mid;
+		}
+	}
+	*hi = bad;
+	return lo;
+}
+
+// Per edge k: ms[k], the first matching source position src_lo[k] and, when md == 1, the destination rowid.
+// status[0] += S, status[1] += C (each term capped at 2^31: only C < 2^31 is ever used), status[2] |= "some
+// edge with ms >= 1 has md != 1".  md is not looked up for an edge without a source: it adds nothing to C.
+__global__ void __launch_bounds__(256) k_key_edges(const uint64_t *__restrict__ sorted_key,
+                                                   const int32_t *__restrict__ sorted_row,
+                                                   const int32_t *__restrict__ nv_ptr,
+                                                   const int64_t *__restrict__ src_key, const int64_t *__restrict__ dst_key,
+                                                   const uint8_t *__restrict__ src_valid,
+                                                   const uint8_t *__restrict__ dst_valid, int64_t m,
+                                                   int32_t *__restrict__ ms_out, int32_t *__restrict__ src_lo,
+                                                   int32_t *__restrict__ dst_row, unsigned long long *status) {
+	const int nv = *nv_ptr;
+	unsigned long long s_sum = 0, c_sum = 0;
+	unsigned int bad = 0;
+	for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += (int64_t)gridDim.x * blockDim.x) {
+		int lo = 0, hi = 0, drow = -1;
+		if (!src_valid || src_valid[k]) {
+			lo = key_range(sorted_key, nv, key_bits(src_key[k]), &hi);
+		}
+		const int ms = hi - lo;
+		if (ms > 0) {
+			int dhi = 0, dlo = 0;
+			if (!dst_valid || dst_valid[k]) {
+				dlo = key_range(sorted_key, nv, key_bits(dst_key[k]), &dhi);
+			}
+			const unsigned long long md = (unsigned long long)(dhi - dlo);
+			c_sum += min((unsigned long long)ms * md, 1ull << 31);
+			bad |= md != 1;
+			if (md == 1) {
+				drow = sorted_row[dlo];
+			}
+		}
+		s_sum += (unsigned long long)ms;
+		ms_out[k] = ms;
+		src_lo[k] = lo;
+		dst_row[k] = drow;
+	}
+	for (int d = 16; d > 0; d >>= 1) {
+		s_sum += __shfl_down_sync(FULL_MASK, s_sum, d);
+		c_sum += __shfl_down_sync(FULL_MASK, c_sum, d);
+		bad |= __shfl_down_sync(FULL_MASK, bad, d);
+	}
+	if ((threadIdx.x & 31) == 0) {
+		if (s_sum) atomicAdd(&status[0], s_sum);
+		if (c_sum) atomicAdd(&status[1], c_sum);
+		if (bad) atomicOr(&status[2], 1ull);
+	}
+}
+
+// edge k -> rows off[k] .. off[k + 1] - 1: (each matching source rowid, its destination rowid, k)
+__global__ void k_key_expand(const int32_t *__restrict__ off, const int32_t *__restrict__ src_lo,
+                             const int32_t *__restrict__ dst_row, const int32_t *__restrict__ sorted_row, int64_t m, int32_t *__restrict__ out_src,
+                             int32_t *__restrict__ out_dst, int64_t *__restrict__ out_eid) {
+	for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += (int64_t)gridDim.x * blockDim.x) {
+		const int64_t p = off[k];
+		const int c = off[k + 1] - off[k];
+		const int lo = src_lo[k], d = dst_row[k];
+		for (int j = 0; j < c; j++) {
+			out_src[p + j] = sorted_row[lo + j];
+			out_dst[p + j] = d;
+			out_eid[p + j] = k;
+		}
+	}
+}
+
+// The key -> rowid join of the CSR CTE on device columns, then the common build.  Sets csr->m.
+static int build_from_keys(pgq_csr *csr, Workspace *ws, cudaStream_t s, const int64_t *vkey, const uint8_t *vvalid,
+                           const int64_t *skey, const int64_t *dkey, const uint8_t *svalid, const uint8_t *dvalid,
+                           int64_t m) {
+	const int64_t n = csr->n;
+	const unsigned grid_n = grid_for(n + 1, 256, (int64_t)csr->ctx->sm_count * 8);
+	const unsigned grid_m = grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16);
+	int32_t *pos, *scan_tmp, *row_a, *row_b, *sorted_row = nullptr, *ms, *src_lo, *dst_row;
+	uint64_t *key_a, *key_b, *sorted_key = nullptr;
+	unsigned long long *d_status;
+	const size_t vb = (size_t)std::max<int64_t>(n, 1);
+	const size_t eb = (size_t)(m + 1);
+	PGQ_TRY(pgq_ws_reserve(ws, 2, 256, (void **)&d_status));
+	PGQ_TRY(pgq_ws_reserve(ws, 16, (size_t)(n + 1) * sizeof(int32_t), (void **)&pos));
+	PGQ_TRY(pgq_ws_reserve(ws, 17, pgq_scan_tmp_elems(std::max<int64_t>(n, m) + 1) * sizeof(int32_t), (void **)&scan_tmp));
+	PGQ_TRY(pgq_ws_reserve(ws, 18, vb * sizeof(uint64_t), (void **)&key_a));
+	PGQ_TRY(pgq_ws_reserve(ws, 19, vb * sizeof(uint64_t), (void **)&key_b));
+	PGQ_TRY(pgq_ws_reserve(ws, 20, vb * sizeof(int32_t), (void **)&row_a));
+	PGQ_TRY(pgq_ws_reserve(ws, 21, vb * sizeof(int32_t), (void **)&row_b));
+	PGQ_TRY(pgq_ws_reserve(ws, 22, eb * sizeof(int32_t), (void **)&ms));
+	PGQ_TRY(pgq_ws_reserve(ws, 23, eb * sizeof(int32_t), (void **)&src_lo));
+	PGQ_TRY(pgq_ws_reserve(ws, 24, eb * sizeof(int32_t), (void **)&dst_row));
+	PGQ_CUDA(cudaMemsetAsync(d_status, 0, 3 * sizeof(unsigned long long), s));
+	k_key_valid<<<grid_n, 256, 0, s>>>(vvalid, n, pos);
+	PGQ_CUDA(cudaGetLastError());
+	PGQ_TRY(pgq_scan_exclusive_i32(pos, pos, n + 1, scan_tmp, s));
+	if (n > 0) {
+		k_key_pairs<<<grid_n, 256, 0, s>>>(vkey, vvalid, n, pos, key_a, row_a);
+		PGQ_CUDA(cudaGetLastError());
+		PGQ_TRY(radix_sort_pairs(ws, key_a, key_b, row_a, row_b, n, 64, s, &sorted_key, &sorted_row));
+	}
+	if (m > 0) {
+		PGQ_CUDA(cudaMemsetAsync(ms + m, 0, sizeof(int32_t), s));
+		k_key_edges<<<grid_m, 256, 0, s>>>(sorted_key, sorted_row, pos + n, skey, dkey, svalid, dvalid, m, ms, src_lo,
+		                                    dst_row, d_status);
+		PGQ_CUDA(cudaGetLastError());
+	}
+	unsigned long long st[3] = {0, 0, 0};
+	PGQ_CUDA(cudaMemcpyAsync(st, d_status, sizeof(st), cudaMemcpyDeviceToHost, s));
+	PGQ_CUDA(cudaStreamSynchronize(s));
+	if (st[2] || st[0] != st[1]) {
+		return pgq_fail(PGQ_ERR_CONSTRAINT, "%s", pgq_status_text(PGQ_ERR_CONSTRAINT));
+	}
+	const int64_t rows = (int64_t)st[0];
+	if (rows >= 0x7fffffffLL) {
+		return pgq_fail(PGQ_ERR_RANGE, "the edge join yields %lld rows: beyond the int32 device CSR", (long long)rows);
+	}
+	csr->m = csr->edge_size = csr->staged = rows;
+	const size_t cap = (size_t)std::max<int64_t>(rows, 1);
+	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_src, cap * sizeof(int32_t)));
+	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_dst, cap * sizeof(int32_t)));
+	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_eid, cap * sizeof(int64_t)));
+	if (rows > 0) {
+		PGQ_TRY(pgq_scan_exclusive_i32(ms, ms, m + 1, scan_tmp, s)); // ms -> first row of every edge, ms[m] = rows
+		k_key_expand<<<grid_m, 256, 0, s>>>(ms, src_lo, dst_row, sorted_row, m, csr->st_src, csr->st_dst, csr->st_eid);
+		PGQ_CUDA(cudaGetLastError());
+	}
+	return finalize_from_rows(csr, ws, s);
+}
+
+// Copies a host column (NULL = absent) into workspace slot `slot`.
+static int stage_column(Workspace *ws, int slot, const void *host, size_t bytes, cudaStream_t s, const void **dev) {
+	*dev = nullptr;
+	if (!host) {
+		return PGQ_OK;
+	}
+	void *d;
+	PGQ_TRY(pgq_ws_reserve(ws, slot, bytes, &d));
+	if (bytes > 0) {
+		PGQ_CUDA(cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, s));
+	}
+	*dev = d;
+	return PGQ_OK;
+}
+
+static int csr_build_keys(pgq_ctx *ctx, int64_t n, const int64_t *vkey, const uint8_t *vvalid, int64_t m,
+                          const int64_t *skey, const int64_t *dkey, const uint8_t *svalid, const uint8_t *dvalid,
+                          bool host, pgq_csr **out) {
+	if (!ctx || !out || (n > 0 && !vkey) || (m > 0 && (!skey || !dkey))) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "null argument");
+	}
+	*out = nullptr;
+	PGQ_TRY(check_sizes(n, m));
+	PGQ_CUDA(cudaSetDevice(ctx->device));
+	pgq_csr *csr = new (std::nothrow) pgq_csr();
+	if (!csr) {
+		return pgq_fail(PGQ_ERR_OOM, "host allocation failed");
+	}
+	csr->ctx = ctx;
+	csr->n = n;
+	csr->edge_init = true;
+	Workspace *ws = nullptr;
+	int st = pgq_ws_acquire(ctx, &ws);
+	if (st != PGQ_OK) {
+		delete csr;
+		return st;
+	}
+	cudaStream_t s = ws->stream;
+	do {
+		if (host) {
+			const size_t n8 = (size_t)n * sizeof(int64_t), m8 = (size_t)m * sizeof(int64_t);
+			if ((st = stage_column(ws, 25, vkey, n8, s, (const void **)&vkey)) != PGQ_OK) break;
+			if ((st = stage_column(ws, 26, vvalid, (size_t)n, s, (const void **)&vvalid)) != PGQ_OK) break;
+			if ((st = stage_column(ws, 27, skey, m8, s, (const void **)&skey)) != PGQ_OK) break;
+			if ((st = stage_column(ws, 28, dkey, m8, s, (const void **)&dkey)) != PGQ_OK) break;
+			if ((st = stage_column(ws, 29, svalid, (size_t)m, s, (const void **)&svalid)) != PGQ_OK) break;
+			if ((st = stage_column(ws, 30, dvalid, (size_t)m, s, (const void **)&dvalid)) != PGQ_OK) break;
+		} else {
+			// the columns may have been produced on any stream of the caller: wait for the whole device once
+			cudaError_t e = cudaDeviceSynchronize();
+			if (e != cudaSuccess) {
+				cudaGetLastError();
+				st = pgq_fail(PGQ_ERR_CUDA, "cudaDeviceSynchronize failed: %s", cudaGetErrorString(e));
+				break;
+			}
+		}
+		st = build_from_keys(csr, ws, s, vkey, vvalid, skey, dkey, svalid, dvalid, m);
+	} while (0);
+	if (st != PGQ_OK) {
+		cudaStreamSynchronize(s); // (queued copies from the caller's columns must not outlive the call)
+		cudaGetLastError();
+	}
+	pgq_ws_release(ctx, ws);
+	if (st != PGQ_OK) {
+		pgq_csr_free(csr);
+		return st;
+	}
+	free_staging(csr);
+	*out = csr;
+	return PGQ_OK;
+}
+
+extern "C" int pgq_csr_build_keys(pgq_ctx *ctx, int64_t n_vertices, const int64_t *vertex_keys,
+                                  const uint8_t *vertex_key_valid, int64_t n_edges, const int64_t *edge_src_keys,
+                                  const int64_t *edge_dst_keys, const uint8_t *edge_src_valid,
+                                  const uint8_t *edge_dst_valid, pgq_csr **out) {
+	return csr_build_keys(ctx, n_vertices, vertex_keys, vertex_key_valid, n_edges, edge_src_keys, edge_dst_keys,
+	                      edge_src_valid, edge_dst_valid, true, out);
+}
+
+extern "C" int pgq_csr_build_keys_device(pgq_ctx *ctx, int64_t n_vertices, const int64_t *d_vertex_keys,
+                                         const uint8_t *d_vertex_key_valid, int64_t n_edges,
+                                         const int64_t *d_edge_src_keys, const int64_t *d_edge_dst_keys,
+                                         const uint8_t *d_edge_src_valid, const uint8_t *d_edge_dst_valid,
+                                         pgq_csr **out) {
+	return csr_build_keys(ctx, n_vertices, d_vertex_keys, d_vertex_key_valid, n_edges, d_edge_src_keys,
+	                      d_edge_dst_keys, d_edge_src_valid, d_edge_dst_valid, false, out);
 }
 
 extern "C" int pgq_csr_upload(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *v, const int64_t *e,

@@ -184,9 +184,12 @@ int pgq_ws_reserve(Workspace *ws, int slot, size_t bytes, void **out);
 int pgq_ws_pinned(Workspace *ws, size_t bytes, void **out);
 int pgq_scan_exclusive_i32(const int32_t *in, int32_t *out, int64_t count, int32_t *block_tmp, cudaStream_t s);
 size_t pgq_scan_tmp_elems(int64_t count);
-// stable LSD radix sort of (int32 key, int32 value) pairs by the low end_bit bits; uses workspace slots 14 and 15
+// stable LSD radix sort of (int32 or uint64 key, int32 value) pairs by the low end_bit bits; uses workspace slots 14
+// and 15
 int radix_sort_pairs(Workspace *ws, int32_t *keys_a, int32_t *keys_b, int32_t *vals_a, int32_t *vals_b, int64_t count,
                      int end_bit, cudaStream_t s, int32_t **keys_res, int32_t **vals_res);
+int radix_sort_pairs(Workspace *ws, uint64_t *keys_a, uint64_t *keys_b, int32_t *vals_a, int32_t *vals_b, int64_t count,
+                     int end_bit, cudaStream_t s, uint64_t **keys_res, int32_t **vals_res);
 
 // ---- BFS drivers implemented in pgq_bfs.cu -----------------------------------------------------
 int pgq_bfs_lengths_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,

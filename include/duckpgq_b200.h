@@ -154,6 +154,29 @@ int pgq_csr_upload(pgq_ctx *ctx, int64_t n_vertices, int64_t n_edges, const int6
  * (cudaDeviceSynchronize) before it reads them. */
 int pgq_csr_build_device(pgq_ctx *ctx, int64_t n_vertices, int64_t n_edges, const int32_t *d_src_rowid,
                          const int32_t *d_dst_rowid, const int64_t *d_edge_rowid, pgq_csr **out);
+/* The whole directed CSR CTE (CreateDirectedCSRCTE, compressed_sparse_row.cpp:132-143,234-251) from the columns a
+ * user holds: the vertex table's BIGINT key column (its rowid = the position) and the edge table's BIGINT src / dst
+ * key columns (its rowid = the position).  A NULL key (validity byte 0) matches nothing.  With ms(k) / md(k) the
+ * number of vertex rows whose key equals edge k's src / dst, the CTE gives vertex row a the degree
+ * count(k.src) of v a LEFT JOIN e k ON k.src = a.id (S = sum ms in all) and hands create_csr_edge the
+ * C = sum ms * md rows (a.rowid, c.rowid, k.rowid) of e k JOIN v a ON a.id = k.src JOIN v c ON c.id = k.dst.
+ *   - S != C, or any edge with ms >= 1 and md != 1 -> PGQ_ERR_CONSTRAINT (the text of csr_creation.cpp:121-125;
+ *     the reference throws on S != C only and scatters out of place when a dangling dst balances a duplicated one);
+ *   - a duplicated source key is legal: the edge is in the adjacency of every matching source row;
+ *   - within a source row, edges are in ascending edge rowid order (the order pgq_csr_build gives the same rows);
+ *   - n_vertices, n_edges and C must be < 2^31 -> PGQ_ERR_RANGE.
+ * The key -> rowid join runs on the device; only a small status block comes back before the rows go through
+ * pgq_csr_build_device's pipeline. */
+int pgq_csr_build_keys(pgq_ctx *ctx, int64_t n_vertices, const int64_t *vertex_keys, const uint8_t *vertex_key_valid,
+                       int64_t n_edges, const int64_t *edge_src_keys, const int64_t *edge_dst_keys,
+                       const uint8_t *edge_src_valid, const uint8_t *edge_dst_valid, pgq_csr **out);
+/* pgq_csr_build_keys for columns that already live in HBM on the context's device.  The inputs are not modified.
+ * As for pgq_csr_build_device, they may still be in the making on any stream of the caller: the call waits for
+ * the device (cudaDeviceSynchronize) before it reads them. */
+int pgq_csr_build_keys_device(pgq_ctx *ctx, int64_t n_vertices, const int64_t *d_vertex_keys,
+                              const uint8_t *d_vertex_key_valid, int64_t n_edges, const int64_t *d_edge_src_keys,
+                              const int64_t *d_edge_dst_keys, const uint8_t *d_edge_src_valid,
+                              const uint8_t *d_edge_dst_valid, pgq_csr **out);
 /* get_csr_v / get_csr_e (src/core/functions/table/pgq_scan.cpp:84-111): copy the CSR back in the
  * reference's layout.  Any output pointer may be NULL. */
 int pgq_csr_download(pgq_csr *csr, int64_t *v_out /* n+2 */, int64_t *e_out /* m */, int64_t *edge_ids_out /* m */);
