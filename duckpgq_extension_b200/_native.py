@@ -100,6 +100,8 @@ SYMBOLS = {
     "pgq_csr_download_weights": (C.c_int, [_VP, _VP]),
     "pgq_iterativelength": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, C.POINTER(PgqOptions), _P64, _PU8,
                                       C.POINTER(PgqStats)]),
+    "pgq_iterativelength_bidirectional": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, C.POINTER(PgqOptions),
+                                                    _P64, _PU8, C.POINTER(PgqStats)]),
     "pgq_shortestpath": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, C.POINTER(PgqOptions), _P64, _P64, _PU8,
                                    C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
     "pgq_free": (None, [_VP]),

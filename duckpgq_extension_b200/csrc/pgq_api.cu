@@ -113,6 +113,59 @@ extern "C" int pgq_iterativelength(pgq_csr *csr, int64_t p, const int64_t *src, 
 	return PGQ_OK;
 }
 
+extern "C" int pgq_iterativelength_bidirectional(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
+                                                 const uint8_t *src_valid, const uint8_t *dst_valid,
+                                                 const pgq_options *opts, int64_t *out_len, uint8_t *out_valid,
+                                                 pgq_stats *stats) {
+	PGQ_TRY(check_call(csr, p, src, dst));
+	if (p > 0 && (!out_len || !out_valid)) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "null output");
+	}
+	PGQ_CUDA(cudaSetDevice(csr->ctx->device));
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	Workspace *ws = g.ws;
+	cudaStream_t s = ws->stream;
+	const size_t b8 = (size_t)p * sizeof(int64_t);
+	int64_t *d_src = nullptr, *d_dst = nullptr, *d_len = nullptr;
+	uint8_t *d_v = nullptr, *d_ov = nullptr;
+	int64_t h2d = 0;
+	std::vector<uint8_t> valid; // a row searches only when both of its ids are valid
+	if (p > 0) {
+		PGQ_TRY(pgq_ws_reserve(ws, 6, b8, (void **)&d_src));
+		PGQ_TRY(pgq_ws_reserve(ws, 7, b8, (void **)&d_dst));
+		PGQ_TRY(pgq_ws_reserve(ws, 9, b8, (void **)&d_len));
+		PGQ_TRY(pgq_ws_reserve(ws, 10, (size_t)p, (void **)&d_ov));
+		PGQ_CUDA(cudaMemcpyAsync(d_src, src, b8, cudaMemcpyHostToDevice, s));
+		PGQ_CUDA(cudaMemcpyAsync(d_dst, dst, b8, cudaMemcpyHostToDevice, s));
+		h2d = 2 * (int64_t)b8;
+		if (src_valid || dst_valid) {
+			valid.resize((size_t)p);
+			for (int64_t i = 0; i < p; i++) {
+				valid[(size_t)i] = (!src_valid || src_valid[i]) && (!dst_valid || dst_valid[i]) ? 1 : 0;
+			}
+			PGQ_TRY(pgq_ws_reserve(ws, 8, (size_t)p, (void **)&d_v));
+			PGQ_CUDA(cudaMemcpyAsync(d_v, valid.data(), (size_t)p, cudaMemcpyHostToDevice, s));
+			h2d += p;
+		}
+	}
+	pgq_stats st;
+	memset(&st, 0, sizeof(st));
+	PGQ_TRY(pgq_bfs_bidirectional_device(csr, ws, p, d_src, d_dst, d_v, opts, d_len, d_ov, s, &st));
+	if (p > 0) {
+		PGQ_CUDA(cudaMemcpyAsync(out_len, d_len, b8, cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaMemcpyAsync(out_valid, d_ov, (size_t)p, cudaMemcpyDeviceToHost, s));
+	}
+	PGQ_CUDA(cudaStreamSynchronize(s));
+	g.settled = true;
+	st.h2d_bytes += h2d;
+	st.d2h_bytes += p > 0 ? (int64_t)b8 + p : 0;
+	if (stats) {
+		*stats = st;
+	}
+	return PGQ_OK;
+}
+
 extern "C" int pgq_shortestpath(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
                                 const uint8_t *src_valid, const pgq_options *opts, int64_t *out_offsets,
                                 int64_t *out_lengths, uint8_t *out_valid, int64_t **out_elems, int64_t *out_total,

@@ -79,7 +79,7 @@ struct PullGraph {
 	int64_t n_short = 0, n_slices = 0, s_total = 0;
 };
 
-#define PGQ_WS_SLOTS 32
+#define PGQ_WS_SLOTS 40
 // Scratch of one path-function call (mask arrays etc.), pooled per context and grown on demand.
 struct Workspace {
 	pgq_ctx *ctx = nullptr; // the context whose pool it belongs to
@@ -199,3 +199,7 @@ int pgq_bfs_paths_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *
                          const uint8_t *d_src_valid, const pgq_options *opts, int64_t *d_out_offsets,
                          int64_t *d_out_lengths, uint8_t *d_out_valid, int64_t **d_out_elems, int64_t *out_total,
                          cudaStream_t stream, pgq_stats *stats);
+// d_valid: rows whose source AND destination are valid (nullable = all)
+int pgq_bfs_bidirectional_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,
+                                 const uint8_t *d_valid, const pgq_options *opts, int64_t *d_out_len,
+                                 uint8_t *d_out_valid, cudaStream_t stream, pgq_stats *stats);

@@ -68,7 +68,8 @@ namespace duckdb {
 static std::mutex g_ctx_lock;
 static pgq_ctx *g_ctx = nullptr;
 static std::atomic<int64_t> g_calls_lengths {0}, g_calls_paths {0}, g_calls_cheapest {0}, g_pairs {0}, g_uploads {0},
-    g_device_builds {0}, g_chunks {0}, g_materialized {0}, g_calls_lcc {0}, g_calls_pagerank {0}, g_calls_wcc {0};
+    g_device_builds {0}, g_chunks {0}, g_materialized {0}, g_calls_lcc {0}, g_calls_pagerank {0}, g_calls_wcc {0},
+    g_calls_bidirectional {0}, g_calls_w_type {0};
 
 [[noreturn]] static void ThrowStatus(int status) {
 	string msg = pgq_last_error();
@@ -675,6 +676,81 @@ static void IterativeLengthB200Function(DataChunk &args, ExpressionState &state,
 	duckpgq_state->csr_to_delete.insert(info.csr_id); // iterativelength.cpp:142
 }
 
+// ---- iterativelengthbidirectional ----------------------------------------------------------------------
+// iterativelength_bidirectional.cpp:43-153 on the device (pgq_iterativelength_bidirectional: the reference's 512-lane
+// batches of the chunk's rows, one CSR, no fan-out -- a row's answer depends on the rows of its batch).  The reference
+// reads its key columns through UnifiedVectorFormat::data, a byte pointer (l.61-62,104-110): row r searches from the
+// BYTE at offset sel(r) of the column, and so does this callback.  Deviations in undefined territory (DESIGN §7): a
+// NULL destination gives NULL, an id outside [0, v_size) fails, a missing CSR raises the texts of iterativelength.
+static void IterativeLengthBidirectionalB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
+	auto &info = func_expr.BindInfo()->Cast<IterativeLengthFunctionData>();
+	auto duckpgq_state = GetDuckPGQState(info.context);
+	if (static_cast<idx_t>(info.csr_id) + 1 > duckpgq_state->csr_list.size()) {
+		throw ConstraintException("Invalid ID");
+	}
+	auto csr_entry = duckpgq_state->csr_list.find(info.csr_id);
+	if (csr_entry == duckpgq_state->csr_list.end() || !csr_entry->second->initialized_v) {
+		throw ConstraintException("Need to initialize CSR before doing shortest path");
+	}
+	int64_t v_size = args.data[1].GetValue(0).GetValue<int64_t>();
+	idx_t count = args.size();
+	auto device_csr = GetB200State(info.context)->ForPathFunction(info.csr_id, *csr_entry->second, v_size);
+	UnifiedVectorFormat vsrc, vdst;
+	args.data[2].ToUnifiedFormat(vsrc);
+	args.data[3].ToUnifiedFormat(vdst);
+	vector<int64_t> src(count), dst(count), out_len(count);
+	vector<uint8_t> src_valid(count), dst_valid(count), out_valid(count);
+	for (idx_t i = 0; i < count; i++) {
+		auto sp = vsrc.sel->get_index(i), dp = vdst.sel->get_index(i);
+		src_valid[i] = vsrc.validity.RowIsValid(sp) ? 1 : 0;
+		dst_valid[i] = vdst.validity.RowIsValid(dp) ? 1 : 0;
+		src[i] = vsrc.data[sp]; // (one byte, as the reference reads it)
+		dst[i] = vdst.data[dp];
+	}
+	pgq_options opts = OptionsFromEnv();
+	opts.lanes = 512;
+	opts.flags = 0;
+	int st = pgq_iterativelength_bidirectional(device_csr, static_cast<int64_t>(count), src.data(), dst.data(),
+	                                           src_valid.data(), dst_valid.data(), &opts, out_len.data(),
+	                                           out_valid.data(), nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_bidirectional++;
+	g_pairs += static_cast<int64_t>(count);
+	result.SetVectorType(VectorType::FLAT_VECTOR);
+	auto result_data = FlatVector::GetDataMutable<int64_t>(result);
+	ValidityMask &result_validity = FlatVector::ValidityMutable(result);
+	for (idx_t i = 0; i < count; i++) {
+		result_data[i] = out_len[i]; // -1 under NULL, l.102-103,147
+		if (!out_valid[i]) {
+			result_validity.SetInvalid(i);
+		}
+	}
+	duckpgq_state->csr_to_delete.insert(info.csr_id); // l.152
+}
+
+// ---- csr_get_w_type ------------------------------------------------------------------------------------
+// csr_get_w_type.cpp:16-36 from the device build's weight type (0 unweighted -- also while no edge has arrived, as
+// initialized_w == false --, 1 BIGINT, 2 DOUBLE): no host copy of the CSR.  A CSR without a usable device build is
+// answered by the reference from the materialised host arrays.
+static void CsrGetWTypeB200(const scalar_function_t &reference, DataChunk &args, ExpressionState &state,
+                            Vector &result) {
+	auto &info = state.expr.Cast<BoundFunctionExpression>().BindInfo()->Cast<CSRFunctionData>();
+	auto duckpgq_state = GetDuckPGQState(info.context);
+	duckpgq_state->GetCSR(info.id); // "CSR not found with ID %d", duckpgq_state.cpp:180-186
+	auto entry = GetB200State(info.context)->Find(info.id);
+	int wt = 0;
+	if (!entry || !entry->error.empty() || pgq_csr_weight_type(entry->csr, &wt) != PGQ_OK) {
+		HostConsumerB200(reference, args, state, result);
+		return;
+	}
+	g_calls_w_type++;
+	result.SetVectorType(VectorType::CONSTANT_VECTOR);
+	ConstantVector::GetData<int32_t>(result)[0] = static_cast<int32_t>(wt);
+}
+
 // ---- shortestpath ---------------------------------------------------------------------------------------
 static void ShortestPathB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
 	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
@@ -890,7 +966,9 @@ static void B200StatsFunction(DataChunk &args, ExpressionState &state, Vector &r
 	              ",host_csr_materialisations=" + std::to_string(g_materialized.load()) +
 	              ",local_clustering_coefficient_calls=" + std::to_string(g_calls_lcc.load()) +
 	              ",pagerank_calls=" + std::to_string(g_calls_pagerank.load()) +
-	              ",weakly_connected_component_calls=" + std::to_string(g_calls_wcc.load());
+	              ",weakly_connected_component_calls=" + std::to_string(g_calls_wcc.load()) +
+	              ",iterativelengthbidirectional_calls=" + std::to_string(g_calls_bidirectional.load()) +
+	              ",csr_get_w_type_calls=" + std::to_string(g_calls_w_type.load());
 	result.SetVectorType(VectorType::CONSTANT_VECTOR);
 	ConstantVector::GetData<string_t>(result)[0] = StringVector::AddString(result, text);
 }
@@ -954,10 +1032,9 @@ static void LoadInternal(ExtensionLoader &loader) {
 	WrapScalar(loader, "create_csr_vertex", CreateCsrVertexB200);
 	WrapScalar(loader, "create_csr_edge", CreateCsrEdgeB200);
 	WrapScalar(loader, "delete_csr", DeleteCsrB200);
-	// reference functions that read the host CSR
-	for (auto name : {"reachability", "csr_get_w_type", "iterativelength_bidirectional"}) {
-		WrapScalar(loader, name, HostConsumerB200);
-	}
+	// the reference function that reads the host CSR
+	WrapScalar(loader, "reachability", HostConsumerB200);
+	WrapScalar(loader, "csr_get_w_type", CsrGetWTypeB200);
 	// the other consumers of the CSR: on the device
 	WrapScalar(loader, "local_clustering_coefficient", LocalClusteringCoefficientB200);
 	WrapScalar(loader, "pagerank", PageRankB200);
@@ -981,6 +1058,11 @@ static void LoadInternal(ExtensionLoader &loader) {
 	loader.RegisterFunction(ScalarFunction(
 	    "iterativelength2", {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
 	    LogicalType::BIGINT, IterativeLengthB200Function, IterativeLengthFunctionData::IterativeLengthBind));
+	// iterativelengthbidirectional: signature and bind of iterativelength_bidirectional.cpp:158-163
+	loader.RegisterFunction(ScalarFunction(
+	    "iterativelengthbidirectional",
+	    {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT}, LogicalType::BIGINT,
+	    IterativeLengthBidirectionalB200Function, IterativeLengthFunctionData::IterativeLengthBind));
 	loader.RegisterFunction(ScalarFunction(
 	    "cheapest_path_length", {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
 	    LogicalType::ANY, CheapestPathLengthB200Function, CheapestPathLengthFunctionData::CheapestPathLengthBind));

@@ -335,6 +335,22 @@ class DeviceCSR:
                                              _pu8(ov), C.byref(st)))
         return out[:p], ov[:p], st.as_dict()
 
+    def iterativelengthbidirectional(self, src, dst, src_valid=None, dst_valid=None,
+                                     options: Optional[Options] = None):
+        """-> (lengths int64 [-1 where NULL], valid uint8, stats dict): the reference's 512-lane batches, each lane
+        searching from both ends along out-edges (include/duckpgq_b200.h, pgq_iterativelength_bidirectional)"""
+        src, dst = _i64(src), _i64(dst)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        dv = None if dst_valid is None else np.ascontiguousarray(dst_valid, dtype=np.uint8)
+        out = np.full(max(p, 1), -1, dtype=np.int64)
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        st = _native.PgqStats()
+        opts = (options or Options()).c()
+        _check(self._lib.pgq_iterativelength_bidirectional(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv),
+                                                           C.byref(opts), _p64(out), _pu8(ov), C.byref(st)))
+        return out[:p], ov[:p], st.as_dict()
+
     def iterativelength_device(self, d_src: int, d_dst: int, p: int, d_out_len: int, d_out_valid: int,
                                d_src_valid: int = 0, stream: int = 0, options: Optional[Options] = None) -> dict:
         """Device-pointer form (raw addresses, e.g. torch.Tensor.data_ptr()); work runs on `stream`."""
@@ -504,6 +520,19 @@ def iterativelength(state: DuckPGQState, csr_id: int, v_size: int, src, dst, src
         raise InvalidInputException(PGQ_ERR_INVALID_ARG, f"v_size {v_size} does not match the CSR ({csr.n} vertices)")
     out, valid, _ = csr.iterativelength(src, dst, src_valid, options)
     state.csr_to_delete.add(csr_id)  # iterativelength.cpp:142
+    return out, valid
+
+
+def iterativelengthbidirectional(state: DuckPGQState, csr_id: int, v_size: int, src, dst, src_valid=None,
+                                 dst_valid=None, options: Optional[Options] = None):
+    """iterativelengthbidirectional(INT, BIGINT, BIGINT, BIGINT) -> BIGINT.  Returns (lengths, valid): the meeting
+    iteration + 1, 0 for src == dst, or NULL (valid 0, value -1) per row.  A missing or uninitialised CSR raises the
+    texts of iterativelength (the reference only asserts)."""
+    csr = _lookup_for_path(state, csr_id, lengths=True)
+    if int(v_size) != csr.n:
+        raise InvalidInputException(PGQ_ERR_INVALID_ARG, f"v_size {v_size} does not match the CSR ({csr.n} vertices)")
+    out, valid, _ = csr.iterativelengthbidirectional(src, dst, src_valid, dst_valid, options)
+    state.csr_to_delete.add(csr_id)  # iterativelength_bidirectional.cpp:152
     return out, valid
 
 

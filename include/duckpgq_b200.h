@@ -205,6 +205,23 @@ int pgq_shortestpath(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const in
                      uint8_t *out_valid, int64_t **out_elems, int64_t *out_total, pgq_stats *stats);
 void pgq_free(void *p);
 
+/* pgq_iterativelength_bidirectional <- IterativeLengthBidirectionalFunction iterativelength_bidirectional.cpp:43-153
+ *   Rows in input order; every row with a valid source, a valid destination and src != dst takes a lane, 512 lanes
+ *   per batch, no de-duplication and no degree shortcut.  Each lane searches from src (side 0) and from dst (side 1),
+ *   BOTH along out-edges; iteration i = 0, 1, ... runs one BFS level of side i & 1.  out_len[i] = i + 1 for the first
+ *   iteration after which the two sides' seen sets share a vertex, out_valid[i] = 1.  A batch ends when every lane
+ *   has met, or at the first iteration that adds no bit for any lane of the batch: its lanes not met yet are NULL
+ *   (out_len -1, out_valid 0).  Met lanes keep expanding, so a row's answer depends on the rows of its batch.
+ *   On a graph holding both directions of every edge the result equals pgq_iterativelength's.
+ *   src == dst -> 0 without a lane; a NULL source or a NULL destination (src_valid / dst_valid, nullable) -> NULL
+ *   without a lane.  Ids outside [0, n) -> PGQ_ERR_RANGE.
+ *   opts (nullable): lanes 0 or 512 (else PGQ_ERR_INVALID_ARG), direction and alpha as for pgq_iterativelength;
+ *   flags != 0 or shard_count > 1 -> PGQ_ERR_UNSUPPORTED.  stats: batches, levels (= iterations, both sides) and
+ *   edges_traversed (out-edges of the expanded frontiers of both sides) are the reference's. */
+int pgq_iterativelength_bidirectional(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const int64_t *dst,
+                                      const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
+                                      int64_t *out_len, uint8_t *out_valid, pgq_stats *stats);
+
 /* pgq_cheapest_path_length <- CheapestPathLengthFunction cheapest_path_length.cpp:138-160 (batched
  * Bellman-Ford, TemplatedBatchBellmanFord l.52-105) over a CSR built with pgq_csr_add_edges_weighted.
  *   out_cost[i] = cost of the cheapest path src[i] -> dst[i] as a raw 8-byte value of the CSR's weight type
