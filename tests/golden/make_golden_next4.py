@@ -119,6 +119,11 @@ def main():
     d = np.clip(s + rng.integers(-3, 4, 260), 0, 299)
     us, ud = undirected(300, s, d)
     save("bands300", 300, us, ud)
+    # the smallest shapes of tests/test_analytics_boundaries.py that sit on a kernel boundary of csrc/pgq_analytics.cu
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import test_analytics_boundaries as tab
+    for name in tab.GOLDEN_SHAPES:
+        save(name, *tab.shape(name))
 
 
 if __name__ == "__main__":

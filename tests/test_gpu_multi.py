@@ -47,7 +47,6 @@ def test_multi_device_iterativelength(gpu_ctx, ndev):
     searches = [s["searches"] for s in sts]
     assert sum(searches) == one["searches"] and max(searches) - min(searches) <= 1  # lanes dealt evenly
     out, valid, _ = multi.iterativelength(ps[:3], pd[:3])  # fewer searches than devices
-    assert np.array_equal(out, exp[:3]) or True
     e3, v3, _ = orc.iterativelength(n, v, e, ps[:3], pd[:3], None, 512)
     assert np.array_equal(out, e3) and np.array_equal(valid, v3)
     multi.free()
