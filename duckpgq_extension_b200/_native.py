@@ -102,6 +102,8 @@ SYMBOLS = {
                                       C.POINTER(PgqStats)]),
     "pgq_iterativelength_bidirectional": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, C.POINTER(PgqOptions),
                                                     _P64, _PU8, C.POINTER(PgqStats)]),
+    "pgq_reachability": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, C.POINTER(PgqOptions), _PU8, _PU8,
+                                   C.POINTER(PgqStats)]),
     "pgq_shortestpath": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, C.POINTER(PgqOptions), _P64, _P64, _PU8,
                                    C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
     "pgq_free": (None, [_VP]),

@@ -166,6 +166,80 @@ extern "C" int pgq_iterativelength_bidirectional(pgq_csr *csr, int64_t p, const 
 	return PGQ_OK;
 }
 
+extern "C" int pgq_reachability(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
+                                const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts, uint8_t *out,
+                                uint8_t *out_valid, pgq_stats *stats) {
+	PGQ_TRY(check_call(csr, p, src, dst));
+	if (p > 0 && (!out || !out_valid)) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "null output");
+	}
+	const bool ref = opts && (opts->flags & PGQ_OPT_REFERENCE_BATCHING);
+	// answered rows: both ids valid.  The searches: by default those rows; with the reference's batches every row with
+	// a valid source, a NULL destination replaced by the source (the row keeps its lane and is answered NULL)
+	std::vector<uint8_t> valid((size_t)p);
+	std::vector<int64_t> search_dst;
+	for (int64_t i = 0; i < p; i++) {
+		const bool sv = !src_valid || src_valid[i], dv = !dst_valid || dst_valid[i];
+		if ((sv && (src[i] < 0 || src[i] >= csr->n)) || (dv && (dst[i] < 0 || dst[i] >= csr->n))) {
+			return pgq_fail(PGQ_ERR_RANGE, "source or destination rowid outside [0,%lld)", (long long)csr->n);
+		}
+		valid[(size_t)i] = sv && dv;
+	}
+	const uint8_t *h_sv = ref ? src_valid : (src_valid || dst_valid ? valid.data() : nullptr);
+	const int64_t *h_dst = dst;
+	if (ref && dst_valid) {
+		search_dst.assign(dst, dst + p);
+		for (int64_t i = 0; i < p; i++) {
+			if (!dst_valid[i]) {
+				search_dst[(size_t)i] = src[i];
+			}
+		}
+		h_dst = search_dst.data();
+	}
+	if (p == 0) {
+		if (stats) {
+			memset(stats, 0, sizeof(*stats));
+		}
+		return PGQ_OK;
+	}
+	PGQ_CUDA(cudaSetDevice(csr->ctx->device));
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	Workspace *ws = g.ws;
+	cudaStream_t s = ws->stream;
+	int64_t *d_src, *d_dst, *d_len;
+	uint8_t *d_sv = nullptr, *d_ov;
+	const size_t b8 = (size_t)p * sizeof(int64_t);
+	PGQ_TRY(pgq_ws_reserve(ws, 6, b8, (void **)&d_src));
+	PGQ_TRY(pgq_ws_reserve(ws, 7, b8, (void **)&d_dst));
+	PGQ_TRY(pgq_ws_reserve(ws, 9, b8, (void **)&d_len));
+	PGQ_TRY(pgq_ws_reserve(ws, 10, (size_t)p, (void **)&d_ov));
+	PGQ_CUDA(cudaMemcpyAsync(d_src, src, b8, cudaMemcpyHostToDevice, s));
+	PGQ_CUDA(cudaMemcpyAsync(d_dst, h_dst, b8, cudaMemcpyHostToDevice, s));
+	int64_t h2d = 2 * (int64_t)b8;
+	if (h_sv) {
+		PGQ_TRY(pgq_ws_reserve(ws, 8, (size_t)p, (void **)&d_sv));
+		PGQ_CUDA(cudaMemcpyAsync(d_sv, h_sv, (size_t)p, cudaMemcpyHostToDevice, s));
+		h2d += p;
+	}
+	pgq_stats st;
+	memset(&st, 0, sizeof(st));
+	PGQ_TRY(pgq_bfs_reachability_device(csr, ws, p, d_src, d_dst, d_sv, src, h_sv, opts, d_len, d_ov, s, &st));
+	PGQ_CUDA(cudaMemcpyAsync(out, d_ov, (size_t)p, cudaMemcpyDeviceToHost, s));
+	PGQ_CUDA(cudaStreamSynchronize(s));
+	g.settled = true;
+	for (int64_t i = 0; i < p; i++) {
+		out[i] &= valid[(size_t)i];
+		out_valid[i] = valid[(size_t)i];
+	}
+	st.h2d_bytes += h2d;
+	st.d2h_bytes += p;
+	if (stats) {
+		*stats = st;
+	}
+	return PGQ_OK;
+}
+
 extern "C" int pgq_shortestpath(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
                                 const uint8_t *src_valid, const pgq_options *opts, int64_t *out_offsets,
                                 int64_t *out_lengths, uint8_t *out_valid, int64_t **out_elems, int64_t *out_total,

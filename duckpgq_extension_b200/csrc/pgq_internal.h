@@ -199,6 +199,11 @@ int pgq_bfs_paths_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *
                          const uint8_t *d_src_valid, const pgq_options *opts, int64_t *d_out_offsets,
                          int64_t *d_out_lengths, uint8_t *d_out_valid, int64_t **d_out_elems, int64_t *out_total,
                          cudaStream_t stream, pgq_stats *stats);
+// h_src / h_src_valid: host copies of d_src / d_src_valid (PGQ_OPT_REFERENCE_BATCHING cuts the batches on the host)
+int pgq_bfs_reachability_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,
+                                const uint8_t *d_src_valid, const int64_t *h_src, const uint8_t *h_src_valid,
+                                const pgq_options *opts, int64_t *d_out_len, uint8_t *d_out_valid, cudaStream_t stream,
+                                pgq_stats *stats);
 // d_valid: rows whose source AND destination are valid (nullable = all)
 int pgq_bfs_bidirectional_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,
                                  const uint8_t *d_valid, const pgq_options *opts, int64_t *d_out_len,

@@ -6,6 +6,8 @@
 //
 //   create_csr_vertex / create_csr_edge (3 overloads) / delete_csr   csr_creation.cpp:86-238, csr_deletion.cpp:10-29
 //   iterativelength / iterativelength2 / shortestpath                iterativelength.cpp:148-152, shortest_path.cpp:212-217
+//   iterativelengthbidirectional / reachability                      iterativelength_bidirectional.cpp:158-163,
+//                                                                    reachability.cpp:259-264
 //   cheapest_path_length                                             cheapest_path_length.cpp:162-166
 //   local_clustering_coefficient / pagerank / weakly_connected_component (the reference's binds, device callbacks)
 //                                                                    local_clustering_coefficient.cpp:14-83,
@@ -20,8 +22,8 @@
 // forwarded to the device build (pgq_csr_add_*; asynchronous pinned staging, no upload at query time).
 // What happens to the HOST arrays is a mode (PGQ_B200_HOST_CSR):
 //   skip   (default) the reference's scatter into the int64 host arrays is not run at all; the functions
-//          of the reference that read the host CSR (reachability, csr_get_w_type, iterativelength_bidirectional,
-//          get_csr_v / _e / _w / _ptr) are
+//          of the reference that read the host CSR (get_csr_v / _e / _w / _ptr, and csr_get_w_type for a CSR
+//          without a usable device build) are
 //          wrapped: the wrapper first materialises the host arrays from the device copy (pgq_csr_download,
 //          the reference's own layout), then calls the captured reference callback;
 //   mirror the captured reference callback runs for every chunk as well (host and device CSR side by side).
@@ -69,7 +71,7 @@ static std::mutex g_ctx_lock;
 static pgq_ctx *g_ctx = nullptr;
 static std::atomic<int64_t> g_calls_lengths {0}, g_calls_paths {0}, g_calls_cheapest {0}, g_pairs {0}, g_uploads {0},
     g_device_builds {0}, g_chunks {0}, g_materialized {0}, g_calls_lcc {0}, g_calls_pagerank {0}, g_calls_wcc {0},
-    g_calls_bidirectional {0}, g_calls_w_type {0};
+    g_calls_bidirectional {0}, g_calls_w_type {0}, g_calls_reachability {0};
 
 [[noreturn]] static void ThrowStatus(int status) {
 	string msg = pgq_last_error();
@@ -731,6 +733,53 @@ static void IterativeLengthBidirectionalB200Function(DataChunk &args, Expression
 	duckpgq_state->csr_to_delete.insert(info.csr_id); // l.152
 }
 
+// ---- reachability ------------------------------------------------------------------------------------------------
+// reachability.cpp:165-254 on the device (pgq_reachability: the rows of iterativelength by default, the reference's
+// 512-lane batches with PGQ_B200_FLAGS=1).  Like the reference it reads both key columns through
+// UnifiedVectorFormat::data, a byte pointer (l.177,181,26,242): row r searches from the BYTE at offset sel(r).  input_size
+// is the v_size of the CSR; is_variant only picks the reference's traversal and is ignored.  Deviations in undefined
+// territory (DESIGN §7): a NULL source or destination gives NULL, an id outside [0, input_size) fails, and NULL sources do
+// not restart a batch.
+static void ReachabilityB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
+	auto &info = func_expr.BindInfo()->Cast<IterativeLengthFunctionData>();
+	auto duckpgq_state = GetDuckPGQState(info.context);
+	CSR *csr = duckpgq_state->GetCSR(info.csr_id); // "CSR not found with ID %d", l.192
+	int64_t input_size = args.data[2].GetValue(0).GetValue<int64_t>();
+	idx_t count = args.size();
+	auto device_csr = GetB200State(info.context)->ForPathFunction(info.csr_id, *csr, input_size);
+	UnifiedVectorFormat vsrc, vdst;
+	args.data[3].ToUnifiedFormat(vsrc);
+	args.data[4].ToUnifiedFormat(vdst);
+	vector<int64_t> src(count), dst(count);
+	vector<uint8_t> src_valid(count), dst_valid(count), out(count), out_valid(count);
+	for (idx_t i = 0; i < count; i++) {
+		auto sp = vsrc.sel->get_index(i), dp = vdst.sel->get_index(i);
+		src_valid[i] = vsrc.validity.RowIsValid(sp) ? 1 : 0;
+		dst_valid[i] = vdst.validity.RowIsValid(dp) ? 1 : 0;
+		src[i] = vsrc.data[sp]; // (one byte, as the reference reads it)
+		dst[i] = vdst.data[dp];
+	}
+	pgq_options opts = OptionsFromEnv();
+	int st = pgq_reachability(device_csr, static_cast<int64_t>(count), src.data(), dst.data(), src_valid.data(),
+	                          dst_valid.data(), &opts, out.data(), out_valid.data(), nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_reachability++;
+	g_pairs += static_cast<int64_t>(count);
+	result.SetVectorType(VectorType::FLAT_VECTOR);
+	auto result_data = FlatVector::GetDataMutable<bool>(result);
+	ValidityMask &result_validity = FlatVector::ValidityMutable(result);
+	for (idx_t i = 0; i < count; i++) {
+		result_data[i] = out[i] != 0;
+		if (!out_valid[i]) {
+			result_validity.SetInvalid(i);
+		}
+	}
+	duckpgq_state->csr_to_delete.insert(info.csr_id); // l.253
+}
+
 // ---- csr_get_w_type ------------------------------------------------------------------------------------
 // csr_get_w_type.cpp:16-36 from the device build's weight type (0 unweighted -- also while no edge has arrived, as
 // initialized_w == false --, 1 BIGINT, 2 DOUBLE): no host copy of the CSR.  A CSR without a usable device build is
@@ -968,7 +1017,8 @@ static void B200StatsFunction(DataChunk &args, ExpressionState &state, Vector &r
 	              ",pagerank_calls=" + std::to_string(g_calls_pagerank.load()) +
 	              ",weakly_connected_component_calls=" + std::to_string(g_calls_wcc.load()) +
 	              ",iterativelengthbidirectional_calls=" + std::to_string(g_calls_bidirectional.load()) +
-	              ",csr_get_w_type_calls=" + std::to_string(g_calls_w_type.load());
+	              ",csr_get_w_type_calls=" + std::to_string(g_calls_w_type.load()) +
+	              ",reachability_calls=" + std::to_string(g_calls_reachability.load());
 	result.SetVectorType(VectorType::CONSTANT_VECTOR);
 	ConstantVector::GetData<string_t>(result)[0] = StringVector::AddString(result, text);
 }
@@ -1032,8 +1082,6 @@ static void LoadInternal(ExtensionLoader &loader) {
 	WrapScalar(loader, "create_csr_vertex", CreateCsrVertexB200);
 	WrapScalar(loader, "create_csr_edge", CreateCsrEdgeB200);
 	WrapScalar(loader, "delete_csr", DeleteCsrB200);
-	// the reference function that reads the host CSR
-	WrapScalar(loader, "reachability", HostConsumerB200);
 	WrapScalar(loader, "csr_get_w_type", CsrGetWTypeB200);
 	// the other consumers of the CSR: on the device
 	WrapScalar(loader, "local_clustering_coefficient", LocalClusteringCoefficientB200);
@@ -1063,6 +1111,11 @@ static void LoadInternal(ExtensionLoader &loader) {
 	    "iterativelengthbidirectional",
 	    {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT}, LogicalType::BIGINT,
 	    IterativeLengthBidirectionalB200Function, IterativeLengthFunctionData::IterativeLengthBind));
+	// reachability: signature and bind of reachability.cpp:259-264
+	loader.RegisterFunction(ScalarFunction(
+	    "reachability",
+	    {LogicalType::INTEGER, LogicalType::BOOLEAN, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
+	    LogicalType::BOOLEAN, ReachabilityB200Function, IterativeLengthFunctionData::IterativeLengthBind));
 	loader.RegisterFunction(ScalarFunction(
 	    "cheapest_path_length", {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
 	    LogicalType::ANY, CheapestPathLengthB200Function, CheapestPathLengthFunctionData::CheapestPathLengthBind));

@@ -351,6 +351,21 @@ class DeviceCSR:
                                                            C.byref(opts), _p64(out), _pu8(ov), C.byref(st)))
         return out[:p], ov[:p], st.as_dict()
 
+    def reachability(self, src, dst, src_valid=None, dst_valid=None, options: Optional[Options] = None):
+        """-> (reachable uint8 [0 where NULL], valid uint8, stats dict): the rows of pgq_iterativelength, or with
+        reference_batching the reference's 512-lane batches (include/duckpgq_b200.h, pgq_reachability)"""
+        src, dst = _i64(src), _i64(dst)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        dv = None if dst_valid is None else np.ascontiguousarray(dst_valid, dtype=np.uint8)
+        out = np.zeros(max(p, 1), dtype=np.uint8)
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        st = _native.PgqStats()
+        opts = (options or Options()).c()
+        _check(self._lib.pgq_reachability(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv), C.byref(opts),
+                                          _pu8(out), _pu8(ov), C.byref(st)))
+        return out[:p], ov[:p], st.as_dict()
+
     def iterativelength_device(self, d_src: int, d_dst: int, p: int, d_out_len: int, d_out_valid: int,
                                d_src_valid: int = 0, stream: int = 0, options: Optional[Options] = None) -> dict:
         """Device-pointer form (raw addresses, e.g. torch.Tensor.data_ptr()); work runs on `stream`."""
@@ -534,6 +549,22 @@ def iterativelengthbidirectional(state: DuckPGQState, csr_id: int, v_size: int, 
     out, valid, _ = csr.iterativelengthbidirectional(src, dst, src_valid, dst_valid, options)
     state.csr_to_delete.add(csr_id)  # iterativelength_bidirectional.cpp:152
     return out, valid
+
+
+def reachability(state: DuckPGQState, csr_id: int, is_variant: bool, input_size: int, src, dst, src_valid=None,
+                 dst_valid=None, options: Optional[Options] = None):
+    """reachability(INTEGER, BOOLEAN, BIGINT, BIGINT, BIGINT) -> BOOLEAN (reachability.cpp:165-264).  Returns
+    (reachable, valid): True / False per row, NULL (valid 0) for a NULL source or destination.  is_variant picks the
+    reference's traversal, which does not change the answers: it is ignored.  A missing CSR raises GetCSR's text."""
+    del is_variant
+    csr = state.get_csr(csr_id)  # "CSR not found with ID %d", duckpgq_state.cpp:180-186
+    if int(input_size) != csr.n:
+        raise InvalidInputException(PGQ_ERR_INVALID_ARG,
+                                    f"input_size {input_size} does not match the CSR ({csr.n} vertices)")
+    csr.finalize()
+    out, valid, _ = csr.reachability(src, dst, src_valid, dst_valid, options)
+    state.csr_to_delete.add(csr_id)  # l.253
+    return out.astype(bool), valid
 
 
 def shortestpath(state: DuckPGQState, csr_id: int, v_size: int, src, dst, src_valid=None,

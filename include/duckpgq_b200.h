@@ -222,6 +222,24 @@ int pgq_iterativelength_bidirectional(pgq_csr *csr, int64_t n_pairs, const int64
                                       const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
                                       int64_t *out_len, uint8_t *out_valid, pgq_stats *stats);
 
+/* pgq_reachability <- ReachabilityFunction reachability.cpp:165-254
+ *   out[i] = 1 when dst[i] is reachable from src[i] along out-edges (src == dst included), else 0; out_valid[i] = 1.
+ *   A NULL source or a NULL destination (src_valid / dst_valid, nullable) gives NULL (out 0, out_valid 0).  Any
+ *   non-NULL id outside [0, n) -> PGQ_ERR_RANGE.
+ *   By default the rows run exactly as pgq_iterativelength runs them, a NULL destination counting as a NULL source
+ *   (de-duplication, degree shortcut, early stop once every row is answered; PGQ_OPT_NO_DEDUP / _NO_PRUNE apply), and
+ *   stats equal pgq_iterativelength's.
+ *   PGQ_OPT_REFERENCE_BATCHING: the reference's batches.  Rows in input order; a row whose source is new to the batch
+ *   opens the next lane, a row whose source is not shares its lane (src == dst rows and rows with a NULL destination
+ *   too); a NULL source takes no lane; a batch ends behind the row that opened lane 512.  Every source is seen from the
+ *   start and a batch runs until a level adds no bit.  batches, levels and edges_traversed are the reference's for
+ *   rows without NULL sources; with them, the reference restarts its next batch early (DESIGN.md section 7), this
+ *   call does not.  lanes must be 0 or 512 (else PGQ_ERR_INVALID_ARG).
+ *   opts (nullable): direction and alpha as for pgq_iterativelength; shard_count > 1 -> PGQ_ERR_UNSUPPORTED. */
+int pgq_reachability(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const int64_t *dst, const uint8_t *src_valid,
+                     const uint8_t *dst_valid, const pgq_options *opts, uint8_t *out, uint8_t *out_valid,
+                     pgq_stats *stats);
+
 /* pgq_cheapest_path_length <- CheapestPathLengthFunction cheapest_path_length.cpp:138-160 (batched
  * Bellman-Ford, TemplatedBatchBellmanFord l.52-105) over a CSR built with pgq_csr_add_edges_weighted.
  *   out_cost[i] = cost of the cheapest path src[i] -> dst[i] as a raw 8-byte value of the CSR's weight type
