@@ -1929,37 +1929,53 @@ __global__ void k_key_expand(const int32_t *__restrict__ off, const int32_t *__r
 	}
 }
 
-// The key -> rowid join of the CSR CTE on device columns, then the common build.  Sets csr->m.
-static int build_from_keys(pgq_csr *csr, Workspace *ws, cudaStream_t s, const int64_t *vkey, const uint8_t *vvalid,
-                           const int64_t *skey, const int64_t *dkey, const uint8_t *svalid, const uint8_t *dvalid,
-                           int64_t m) {
+// The vertex table's (key, rowid) pairs sorted by key: the nv = (*pos)[n] non-NULL ones first (slots 16-21; the scan
+// scratch in slot 17 has room for max(n, m) + 1 elements).
+static int sort_vertex_keys(pgq_csr *csr, Workspace *ws, cudaStream_t s, const int64_t *vkey, const uint8_t *vvalid,
+                            int64_t m, int32_t **pos_out, int32_t **scan_tmp_out, uint64_t **sorted_key,
+                            int32_t **sorted_row) {
 	const int64_t n = csr->n;
 	const unsigned grid_n = grid_for(n + 1, 256, (int64_t)csr->ctx->sm_count * 8);
-	const unsigned grid_m = grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16);
-	int32_t *pos, *scan_tmp, *row_a, *row_b, *sorted_row = nullptr, *ms, *src_lo, *dst_row;
-	uint64_t *key_a, *key_b, *sorted_key = nullptr;
-	unsigned long long *d_status;
+	int32_t *pos, *scan_tmp, *row_a, *row_b;
+	uint64_t *key_a, *key_b;
 	const size_t vb = (size_t)std::max<int64_t>(n, 1);
-	const size_t eb = (size_t)(m + 1);
-	PGQ_TRY(pgq_ws_reserve(ws, 2, 256, (void **)&d_status));
 	PGQ_TRY(pgq_ws_reserve(ws, 16, (size_t)(n + 1) * sizeof(int32_t), (void **)&pos));
 	PGQ_TRY(pgq_ws_reserve(ws, 17, pgq_scan_tmp_elems(std::max<int64_t>(n, m) + 1) * sizeof(int32_t), (void **)&scan_tmp));
 	PGQ_TRY(pgq_ws_reserve(ws, 18, vb * sizeof(uint64_t), (void **)&key_a));
 	PGQ_TRY(pgq_ws_reserve(ws, 19, vb * sizeof(uint64_t), (void **)&key_b));
 	PGQ_TRY(pgq_ws_reserve(ws, 20, vb * sizeof(int32_t), (void **)&row_a));
 	PGQ_TRY(pgq_ws_reserve(ws, 21, vb * sizeof(int32_t), (void **)&row_b));
-	PGQ_TRY(pgq_ws_reserve(ws, 22, eb * sizeof(int32_t), (void **)&ms));
-	PGQ_TRY(pgq_ws_reserve(ws, 23, eb * sizeof(int32_t), (void **)&src_lo));
-	PGQ_TRY(pgq_ws_reserve(ws, 24, eb * sizeof(int32_t), (void **)&dst_row));
-	PGQ_CUDA(cudaMemsetAsync(d_status, 0, 3 * sizeof(unsigned long long), s));
+	*sorted_key = nullptr;
+	*sorted_row = nullptr;
 	k_key_valid<<<grid_n, 256, 0, s>>>(vvalid, n, pos);
 	PGQ_CUDA(cudaGetLastError());
 	PGQ_TRY(pgq_scan_exclusive_i32(pos, pos, n + 1, scan_tmp, s));
 	if (n > 0) {
 		k_key_pairs<<<grid_n, 256, 0, s>>>(vkey, vvalid, n, pos, key_a, row_a);
 		PGQ_CUDA(cudaGetLastError());
-		PGQ_TRY(radix_sort_pairs(ws, key_a, key_b, row_a, row_b, n, 64, s, &sorted_key, &sorted_row));
+		PGQ_TRY(radix_sort_pairs(ws, key_a, key_b, row_a, row_b, n, 64, s, sorted_key, sorted_row));
 	}
+	*pos_out = pos;
+	*scan_tmp_out = scan_tmp;
+	return PGQ_OK;
+}
+
+// The key -> rowid join of the CSR CTE on device columns, then the common build.  Sets csr->m.
+static int build_from_keys(pgq_csr *csr, Workspace *ws, cudaStream_t s, const int64_t *vkey, const uint8_t *vvalid,
+                           const int64_t *skey, const int64_t *dkey, const uint8_t *svalid, const uint8_t *dvalid,
+                           int64_t m) {
+	const int64_t n = csr->n;
+	const unsigned grid_m = grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16);
+	int32_t *pos, *scan_tmp, *sorted_row, *ms, *src_lo, *dst_row;
+	uint64_t *sorted_key;
+	unsigned long long *d_status;
+	const size_t eb = (size_t)(m + 1);
+	PGQ_TRY(pgq_ws_reserve(ws, 2, 256, (void **)&d_status));
+	PGQ_TRY(pgq_ws_reserve(ws, 22, eb * sizeof(int32_t), (void **)&ms));
+	PGQ_TRY(pgq_ws_reserve(ws, 23, eb * sizeof(int32_t), (void **)&src_lo));
+	PGQ_TRY(pgq_ws_reserve(ws, 24, eb * sizeof(int32_t), (void **)&dst_row));
+	PGQ_CUDA(cudaMemsetAsync(d_status, 0, 3 * sizeof(unsigned long long), s));
+	PGQ_TRY(sort_vertex_keys(csr, ws, s, vkey, vvalid, m, &pos, &scan_tmp, &sorted_key, &sorted_row));
 	if (m > 0) {
 		PGQ_CUDA(cudaMemsetAsync(ms + m, 0, sizeof(int32_t), s));
 		k_key_edges<<<grid_m, 256, 0, s>>>(sorted_key, sorted_row, pos + n, skey, dkey, svalid, dvalid, m, ms, src_lo,
@@ -1989,6 +2005,351 @@ static int build_from_keys(pgq_csr *csr, Workspace *ws, cudaStream_t s, const in
 	return finalize_from_rows(csr, ws, s);
 }
 
+// ---- the undirected CSR from vertex-key and edge-key columns ---------------------------------------
+// CreateUndirectedCSRCTE (compressed_sparse_row.cpp:125-130,145-172,192-223).  edges_cte holds (a, c, k) for every
+// vertex row a whose key is e.src[k] and c whose key is e.dst[k]; create_csr_edge gets one row (p, q, any_value(k))
+// per distinct pair of edges_cte UNION ALL its reverse, R in all.  The degree of row a is the number of distinct
+// "other end" values over the edges incident to a's key in either direction, a NULL or unmatched other end included
+// (a UNION BY NAME of the two join branches grouped by rowid); S = their sum, and the reference throws when S != R.
+//
+// Here edge k expands into its ms * md forward rows and as many reverse ones, in edge rowid order, and one stable
+// radix sort of the keys (p, q) -- 2 * bits(n) + 1 bits -- with k as the value groups the duplicates with the
+// smallest k first.  The lowest key bit is 0 when q is the first row (in key order) of its key, so every distinct
+// neighbour key is counted once per row: M(p).  The ends no vertex row holds are counted per key of the other end:
+// a NULL end by a flag (null_mult), the unmatched values by a small sort of those half edges.  With D(x) the number
+// of such distinct ends of key x, degree(p) = M(p) + D(key p), and R(p) = degree(p) must hold for every row
+// (S == R alone lets a dangling end balance a duplicated key, and the reference then scatters out of place).
+
+// Per edge k: its matching source / destination rows are sorted positions [slo, slo + ms) / [dlo, dlo + md), and it
+// expands into rows[k] = 2 ms md rows.  An edge with just one matched end gives that end's key an end that no row
+// holds: null_mult[lo] = the number of rows with the key (the same for every such edge) for a NULL one, else it
+// counts as a half edge.  status[0] += sum rows (each term capped at 2^31), status[1] += half edges.
+__global__ void __launch_bounds__(256) k_ukey_edges(const uint64_t *__restrict__ sorted_key,
+                                                    const int32_t *__restrict__ nv_ptr,
+                                                    const int64_t *__restrict__ src_key, const int64_t *__restrict__ dst_key,
+                                                    const uint8_t *__restrict__ src_valid,
+                                                    const uint8_t *__restrict__ dst_valid, int64_t m,
+                                                    int32_t *__restrict__ rows, int32_t *__restrict__ slo_out,
+                                                    int32_t *__restrict__ dlo_out, int32_t *__restrict__ ms_out,
+                                                    int32_t *__restrict__ md_out, int32_t *__restrict__ null_mult,
+                                                    unsigned long long *status) {
+	const int nv = *nv_ptr;
+	unsigned long long t_sum = 0, h_sum = 0;
+	for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += (int64_t)gridDim.x * blockDim.x) {
+		const bool sv = !src_valid || src_valid[k], dv = !dst_valid || dst_valid[k];
+		int slo = 0, shi = 0, dlo = 0, dhi = 0;
+		if (sv) {
+			slo = key_range(sorted_key, nv, key_bits(src_key[k]), &shi);
+		}
+		if (dv) {
+			dlo = key_range(sorted_key, nv, key_bits(dst_key[k]), &dhi);
+		}
+		const int ms = shi - slo, md = dhi - dlo;
+		const unsigned long long r = 2ull * (unsigned long long)ms * (unsigned long long)md;
+		t_sum += min(r, 1ull << 31);
+		rows[k] = (int32_t)min(r, 0x7fffffffull);
+		if ((ms > 0) != (md > 0)) {
+			if (ms > 0 ? dv : sv) {
+				h_sum++;
+			} else {
+				null_mult[ms > 0 ? slo : dlo] = ms > 0 ? ms : md;
+			}
+		}
+		slo_out[k] = slo;
+		dlo_out[k] = dlo;
+		ms_out[k] = ms;
+		md_out[k] = md;
+	}
+	for (int d = 16; d > 0; d >>= 1) {
+		t_sum += __shfl_down_sync(FULL_MASK, t_sum, d);
+		h_sum += __shfl_down_sync(FULL_MASK, h_sum, d);
+	}
+	if ((threadIdx.x & 31) == 0) {
+		if (t_sum) atomicAdd(&status[0], t_sum);
+		if (h_sum) atomicAdd(&status[1], h_sum);
+	}
+}
+
+// the half edges with a non-NULL unmatched end: (position of the matched key, its row count, the other end's value);
+// the order of the list does not matter (it is sorted next), status[4] hands out the places
+__global__ void k_ukey_half(const int64_t *__restrict__ src_key, const int64_t *__restrict__ dst_key,
+                            const uint8_t *__restrict__ src_valid, const uint8_t *__restrict__ dst_valid, int64_t m,
+                            const int32_t *__restrict__ slo, const int32_t *__restrict__ dlo,
+                            const int32_t *__restrict__ ms, const int32_t *__restrict__ md, int32_t *__restrict__ h_lo,
+                            int32_t *__restrict__ h_mult, uint64_t *__restrict__ h_val, int32_t *__restrict__ h_idx,
+                            unsigned long long *status) {
+	for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += (int64_t)gridDim.x * blockDim.x) {
+		const int s = ms[k], d = md[k];
+		if ((s > 0) == (d > 0)) {
+			continue;
+		}
+		if (s > 0 ? (dst_valid && !dst_valid[k]) : (src_valid && !src_valid[k])) {
+			continue; // a NULL end: null_mult
+		}
+		const int i = (int)atomicAdd(&status[4], 1ull);
+		h_lo[i] = s > 0 ? slo[k] : dlo[k];
+		h_mult[i] = s > 0 ? s : d;
+		h_val[i] = key_bits(s > 0 ? dst_key[k] : src_key[k]);
+		h_idx[i] = i;
+	}
+}
+
+// after the sort by value: key = the half edge's key position, value = its place in value order
+__global__ void k_ukey_half_keys(const int32_t *__restrict__ idx, const int32_t *__restrict__ h_lo, int64_t h,
+                                 int32_t *__restrict__ key_out, int32_t *__restrict__ val_out) {
+	for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < h; i += (int64_t)gridDim.x * blockDim.x) {
+		key_out[i] = h_lo[idx[i]];
+		val_out[i] = (int32_t)i;
+	}
+}
+
+// the half edges sorted by (key position, value): each distinct pair is one end of that key, which every row of the
+// key has (status[2] += the key's row count)
+__global__ void __launch_bounds__(256) k_ukey_half_unique(const int32_t *__restrict__ lo_sorted,
+                                                          const int32_t *__restrict__ at,
+                                                          const uint64_t *__restrict__ val_sorted,
+                                                          const int32_t *__restrict__ idx,
+                                                          const int32_t *__restrict__ h_mult, int64_t h,
+                                                          int32_t *__restrict__ dcnt, unsigned long long *status) {
+	unsigned long long s_sum = 0;
+	for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < h; i += (int64_t)gridDim.x * blockDim.x) {
+		const int j = at[i];
+		if (i == 0 || lo_sorted[i] != lo_sorted[i - 1] || val_sorted[j] != val_sorted[at[i - 1]]) {
+			atomicAdd(&dcnt[lo_sorted[i]], 1);
+			s_sum += (unsigned long long)h_mult[idx[j]];
+		}
+	}
+	for (int d = 16; d > 0; d >>= 1) {
+		s_sum += __shfl_down_sync(FULL_MASK, s_sum, d);
+	}
+	if ((threadIdx.x & 31) == 0 && s_sum) {
+		atomicAdd(&status[2], s_sum);
+	}
+}
+
+// edge k -> rows off[k] .. off[k + 1] - 1: key (p << (b + 1)) | (q << 1) | (q is not the first row of its key), value k
+__global__ void k_ukey_expand(const int32_t *__restrict__ off, const int32_t *__restrict__ slo,
+                              const int32_t *__restrict__ dlo, const int32_t *__restrict__ ms,
+                              const int32_t *__restrict__ md, const int32_t *__restrict__ sorted_row, int64_t m, int b,
+                              uint64_t *__restrict__ key_out, int32_t *__restrict__ val_out) {
+	for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += (int64_t)gridDim.x * blockDim.x) {
+		int64_t p = off[k];
+		const int s = ms[k], d = md[k], s0 = slo[k], d0 = dlo[k];
+		for (int i = 0; i < s; i++) {
+			const uint64_t a = (uint64_t)sorted_row[s0 + i];
+			for (int j = 0; j < d; j++) {
+				const uint64_t c = (uint64_t)sorted_row[d0 + j];
+				key_out[p] = (a << (b + 1)) | (c << 1) | (j != 0);
+				val_out[p] = (int32_t)k;
+				key_out[p + 1] = (c << (b + 1)) | (a << 1) | (i != 0);
+				val_out[p + 1] = (int32_t)k;
+				p += 2;
+			}
+		}
+	}
+}
+
+// flag[i] = 1 for the first of each run of equal keys (flag[t] = 0); per row p, r_row[p] = R(p) and m_row[p] = M(p);
+// status[3] += sum M
+__global__ void __launch_bounds__(256) k_ukey_unique(const uint64_t *__restrict__ keys, int64_t t, int b,
+                                                     int32_t *__restrict__ flag, int32_t *__restrict__ r_row,
+                                                     int32_t *__restrict__ m_row, unsigned long long *status) {
+	unsigned long long m_sum = 0;
+	for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= t; i += (int64_t)gridDim.x * blockDim.x) {
+		int u = 0;
+		if (i < t) {
+			const uint64_t key = keys[i];
+			u = i == 0 || key != keys[i - 1];
+			if (u) {
+				const int p = (int)(key >> (b + 1));
+				atomicAdd(&r_row[p], 1);
+				if (!(key & 1)) {
+					atomicAdd(&m_row[p], 1);
+					m_sum++;
+				}
+			}
+		}
+		flag[i] = u;
+	}
+	for (int d = 16; d > 0; d >>= 1) {
+		m_sum += __shfl_down_sync(FULL_MASK, m_sum, d);
+	}
+	if ((threadIdx.x & 31) == 0 && m_sum) {
+		atomicAdd(&status[3], m_sum);
+	}
+}
+
+// the first of every run -> row pos[i] of the create_csr_edge input: (p, q, smallest k)
+__global__ void k_ukey_compact(const uint64_t *__restrict__ keys, const int32_t *__restrict__ vals,
+                               const int32_t *__restrict__ pos, int64_t t, int b, int32_t *__restrict__ out_src,
+                               int32_t *__restrict__ out_dst, int64_t *__restrict__ out_eid) {
+	const uint64_t qmask = ((uint64_t)1 << b) - 1;
+	for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < t; i += (int64_t)gridDim.x * blockDim.x) {
+		const int o = pos[i];
+		if (pos[i + 1] != o) {
+			const uint64_t key = keys[i];
+			out_src[o] = (int32_t)(key >> (b + 1));
+			out_dst[o] = (int32_t)((key >> 1) & qmask);
+			out_eid[o] = vals[i];
+		}
+	}
+}
+
+// Per key (at the sorted position of its first row): D = distinct unmatched values + a NULL end, status[2] += the
+// key's row count for a NULL end, status[5] = 1 when R(p) != M(p) + D for its rows (all rows of a key have the
+// same neighbours, so its first row stands for all).
+__global__ void __launch_bounds__(256) k_ukey_check(const uint64_t *__restrict__ sorted_key,
+                                                    const int32_t *__restrict__ sorted_row,
+                                                    const int32_t *__restrict__ nv_ptr,
+                                                    const int32_t *__restrict__ r_row, const int32_t *__restrict__ m_row,
+                                                    const int32_t *__restrict__ dcnt,
+                                                    const int32_t *__restrict__ null_mult, unsigned long long *status) {
+	const int nv = *nv_ptr;
+	unsigned long long s_sum = 0;
+	unsigned int bad = 0;
+	for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += gridDim.x * blockDim.x) {
+		if (i == 0 || sorted_key[i] != sorted_key[i - 1]) {
+			const int r = sorted_row[i], nm = null_mult[i];
+			bad |= r_row[r] - m_row[r] != dcnt[i] + (nm > 0);
+			s_sum += (unsigned long long)nm;
+		}
+	}
+	for (int d = 16; d > 0; d >>= 1) {
+		s_sum += __shfl_down_sync(FULL_MASK, s_sum, d);
+		bad |= __shfl_down_sync(FULL_MASK, bad, d);
+	}
+	if ((threadIdx.x & 31) == 0) {
+		if (s_sum) atomicAdd(&status[2], s_sum);
+		if (bad) atomicOr(&status[5], 1ull);
+	}
+}
+
+// The undirected CSR CTE on device columns, then the common build.  Sets csr->m.  Workspace slots: 2 the status
+// block, 16-21 the vertex sort, 22-24 and 46-47 per edge, 48-52 the row sort (and before it the half-edge sort),
+// 53-58 per vertex and per half edge.
+static int build_from_keys_undirected(pgq_csr *csr, Workspace *ws, cudaStream_t s, const int64_t *vkey,
+                                      const uint8_t *vvalid, const int64_t *skey, const int64_t *dkey,
+                                      const uint8_t *svalid, const uint8_t *dvalid, int64_t m) {
+	const int64_t n = csr->n;
+	const int64_t sms = csr->ctx->sm_count;
+	const unsigned grid_m = grid_for(m, 256, sms * 16);
+	int32_t *pos, *scan_tmp, *sorted_row, *rows, *slo, *dlo, *ms, *md, *r_row, *m_row, *dcnt, *null_mult;
+	uint64_t *sorted_key;
+	unsigned long long *d_status;
+	const size_t vb = (size_t)std::max<int64_t>(n, 1) * sizeof(int32_t);
+	const size_t eb = (size_t)(m + 1) * sizeof(int32_t);
+	PGQ_TRY(pgq_ws_reserve(ws, 2, 256, (void **)&d_status));
+	PGQ_TRY(pgq_ws_reserve(ws, 22, eb, (void **)&rows));
+	PGQ_TRY(pgq_ws_reserve(ws, 23, eb, (void **)&slo));
+	PGQ_TRY(pgq_ws_reserve(ws, 24, eb, (void **)&dlo));
+	PGQ_TRY(pgq_ws_reserve(ws, 46, eb, (void **)&ms));
+	PGQ_TRY(pgq_ws_reserve(ws, 47, eb, (void **)&md));
+	PGQ_TRY(pgq_ws_reserve(ws, 53, vb, (void **)&r_row));
+	PGQ_TRY(pgq_ws_reserve(ws, 54, vb, (void **)&m_row));
+	PGQ_TRY(pgq_ws_reserve(ws, 55, vb, (void **)&dcnt));
+	PGQ_TRY(pgq_ws_reserve(ws, 56, vb, (void **)&null_mult));
+	PGQ_CUDA(cudaMemsetAsync(d_status, 0, 6 * sizeof(unsigned long long), s));
+	PGQ_CUDA(cudaMemsetAsync(r_row, 0, vb, s));
+	PGQ_CUDA(cudaMemsetAsync(m_row, 0, vb, s));
+	PGQ_CUDA(cudaMemsetAsync(dcnt, 0, vb, s));
+	PGQ_CUDA(cudaMemsetAsync(null_mult, 0, vb, s));
+	PGQ_TRY(sort_vertex_keys(csr, ws, s, vkey, vvalid, m, &pos, &scan_tmp, &sorted_key, &sorted_row));
+	if (m > 0) {
+		PGQ_CUDA(cudaMemsetAsync(rows + m, 0, sizeof(int32_t), s));
+		k_ukey_edges<<<grid_m, 256, 0, s>>>(sorted_key, pos + n, skey, dkey, svalid, dvalid, m, rows, slo, dlo, ms, md,
+		                                    null_mult, d_status);
+		PGQ_CUDA(cudaGetLastError());
+	}
+	unsigned long long st[6] = {0, 0, 0, 0, 0, 0};
+	PGQ_CUDA(cudaMemcpyAsync(st, d_status, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+	PGQ_CUDA(cudaStreamSynchronize(s));
+	const int64_t t = (int64_t)st[0], h = (int64_t)st[1];
+	if (t >= 0x7fffffffLL) {
+		return pgq_fail(PGQ_ERR_RANGE, "the undirected edge join yields %lld rows before de-duplication: beyond the int32 "
+		                "device CSR", (long long)t);
+	}
+	int b = 1;
+	while (b < 31 && ((int64_t)1 << b) < n) {
+		b++;
+	}
+	// the half edges: distinct (key, unmatched value) pairs by a sort on the value, then a stable one on the key
+	if (h > 0) {
+		int32_t *h_lo, *h_mult, *idx_a, *idx_b, *idx, *lo_a, *lo_b, *at_a, *at_b, *lo_sorted, *at;
+		uint64_t *val_a, *val_b, *val_sorted;
+		const size_t hb = (size_t)h * sizeof(int32_t);
+		PGQ_TRY(pgq_ws_reserve(ws, 57, hb, (void **)&h_lo));
+		PGQ_TRY(pgq_ws_reserve(ws, 58, hb, (void **)&h_mult));
+		PGQ_TRY(pgq_ws_reserve(ws, 48, (size_t)h * sizeof(uint64_t), (void **)&val_a));
+		PGQ_TRY(pgq_ws_reserve(ws, 49, (size_t)h * sizeof(uint64_t), (void **)&val_b));
+		PGQ_TRY(pgq_ws_reserve(ws, 50, hb, (void **)&idx_a));
+		PGQ_TRY(pgq_ws_reserve(ws, 51, hb, (void **)&idx_b));
+		PGQ_TRY(pgq_ws_reserve(ws, 52, 4 * hb, (void **)&lo_a));
+		lo_b = lo_a + h;
+		at_a = lo_b + h;
+		at_b = at_a + h;
+		k_ukey_half<<<grid_m, 256, 0, s>>>(skey, dkey, svalid, dvalid, m, slo, dlo, ms, md, h_lo, h_mult, val_a, idx_a,
+		                                   d_status);
+		PGQ_CUDA(cudaGetLastError());
+		PGQ_TRY(radix_sort_pairs(ws, val_a, val_b, idx_a, idx_b, h, 64, s, &val_sorted, &idx));
+		const unsigned grid_h = grid_for(h, 256, sms * 8);
+		k_ukey_half_keys<<<grid_h, 256, 0, s>>>(idx, h_lo, h, lo_a, at_a);
+		PGQ_CUDA(cudaGetLastError());
+		PGQ_TRY(radix_sort_pairs(ws, lo_a, lo_b, at_a, at_b, h, b, s, &lo_sorted, &at));
+		k_ukey_half_unique<<<grid_h, 256, 0, s>>>(lo_sorted, at, val_sorted, idx, h_mult, h, dcnt, d_status);
+		PGQ_CUDA(cudaGetLastError());
+	}
+	// the rows: expand, sort by (p, q) with the edge rowid as value, keep the first of each run
+	int32_t *flag = nullptr;
+	if (t > 0) {
+		uint64_t *key_a, *key_b, *key_sorted;
+		int32_t *val_a, *val_b, *val_sorted;
+		const size_t tb = (size_t)t * sizeof(int32_t);
+		PGQ_TRY(pgq_ws_reserve(ws, 48, (size_t)t * sizeof(uint64_t), (void **)&key_a));
+		PGQ_TRY(pgq_ws_reserve(ws, 49, (size_t)t * sizeof(uint64_t), (void **)&key_b));
+		PGQ_TRY(pgq_ws_reserve(ws, 50, tb, (void **)&val_a));
+		PGQ_TRY(pgq_ws_reserve(ws, 51, tb, (void **)&val_b));
+		PGQ_TRY(pgq_ws_reserve(ws, 52, tb + sizeof(int32_t), (void **)&flag));
+		PGQ_TRY(pgq_ws_reserve(ws, 17, pgq_scan_tmp_elems(std::max<int64_t>(m, t) + 1) * sizeof(int32_t),
+		                       (void **)&scan_tmp));
+		PGQ_TRY(pgq_scan_exclusive_i32(rows, rows, m + 1, scan_tmp, s)); // rows -> first row of every edge
+		k_ukey_expand<<<grid_m, 256, 0, s>>>(rows, slo, dlo, ms, md, sorted_row, m, b, key_a, val_a);
+		PGQ_CUDA(cudaGetLastError());
+		PGQ_TRY(radix_sort_pairs(ws, key_a, key_b, val_a, val_b, t, 2 * b + 1, s, &key_sorted, &val_sorted));
+		const unsigned grid_t = grid_for(t + 1, 256, sms * 16);
+		k_ukey_unique<<<grid_t, 256, 0, s>>>(key_sorted, t, b, flag, r_row, m_row, d_status);
+		PGQ_CUDA(cudaGetLastError());
+		PGQ_TRY(pgq_scan_exclusive_i32(flag, flag, t + 1, scan_tmp, s));
+		int32_t r = 0;
+		PGQ_CUDA(cudaMemcpyAsync(&r, flag + t, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaStreamSynchronize(s));
+		const size_t cap = (size_t)std::max<int32_t>(r, 1);
+		PGQ_TRY(dev_alloc(csr, (void **)&csr->st_src, cap * sizeof(int32_t)));
+		PGQ_TRY(dev_alloc(csr, (void **)&csr->st_dst, cap * sizeof(int32_t)));
+		PGQ_TRY(dev_alloc(csr, (void **)&csr->st_eid, cap * sizeof(int64_t)));
+		k_ukey_compact<<<grid_for(t, 256, sms * 16), 256, 0, s>>>(key_sorted, val_sorted, flag, t, b, csr->st_src,
+		                                                          csr->st_dst, csr->st_eid);
+		PGQ_CUDA(cudaGetLastError());
+		csr->m = csr->edge_size = csr->staged = r;
+	} else {
+		PGQ_TRY(dev_alloc(csr, (void **)&csr->st_src, sizeof(int32_t)));
+		PGQ_TRY(dev_alloc(csr, (void **)&csr->st_dst, sizeof(int32_t)));
+		PGQ_TRY(dev_alloc(csr, (void **)&csr->st_eid, sizeof(int64_t)));
+		csr->m = csr->edge_size = csr->staged = 0;
+	}
+	if (n > 0) {
+		k_ukey_check<<<grid_for(n, 256, sms * 8), 256, 0, s>>>(sorted_key, sorted_row, pos + n, r_row, m_row, dcnt,
+		                                                       null_mult, d_status);
+		PGQ_CUDA(cudaGetLastError());
+	}
+	PGQ_CUDA(cudaMemcpyAsync(st, d_status, sizeof(st), cudaMemcpyDeviceToHost, s));
+	PGQ_CUDA(cudaStreamSynchronize(s));
+	const unsigned long long degree_sum = st[2] + st[3];
+	if (st[5] || degree_sum != (unsigned long long)csr->m) {
+		return pgq_fail(PGQ_ERR_CONSTRAINT, "%s", pgq_status_text(PGQ_ERR_CONSTRAINT));
+	}
+	return finalize_from_rows(csr, ws, s);
+}
+
 // Copies a host column (NULL = absent) into workspace slot `slot`.
 static int stage_column(Workspace *ws, int slot, const void *host, size_t bytes, cudaStream_t s, const void **dev) {
 	*dev = nullptr;
@@ -2006,7 +2367,7 @@ static int stage_column(Workspace *ws, int slot, const void *host, size_t bytes,
 
 static int csr_build_keys(pgq_ctx *ctx, int64_t n, const int64_t *vkey, const uint8_t *vvalid, int64_t m,
                           const int64_t *skey, const int64_t *dkey, const uint8_t *svalid, const uint8_t *dvalid,
-                          bool host, pgq_csr **out) {
+                          bool host, bool undirected, pgq_csr **out) {
 	if (!ctx || !out || (n > 0 && !vkey) || (m > 0 && (!skey || !dkey))) {
 		return pgq_fail(PGQ_ERR_INVALID_ARG, "null argument");
 	}
@@ -2029,13 +2390,15 @@ static int csr_build_keys(pgq_ctx *ctx, int64_t n, const int64_t *vkey, const ui
 	cudaStream_t s = ws->stream;
 	do {
 		if (host) {
+			// (slots 40-45: the searches' lane-mask arrays, slots 28-30, must not be written -- a workspace remembers
+			// which of their rows hold zeros, Workspace::clean_from)
 			const size_t n8 = (size_t)n * sizeof(int64_t), m8 = (size_t)m * sizeof(int64_t);
-			if ((st = stage_column(ws, 25, vkey, n8, s, (const void **)&vkey)) != PGQ_OK) break;
-			if ((st = stage_column(ws, 26, vvalid, (size_t)n, s, (const void **)&vvalid)) != PGQ_OK) break;
-			if ((st = stage_column(ws, 27, skey, m8, s, (const void **)&skey)) != PGQ_OK) break;
-			if ((st = stage_column(ws, 28, dkey, m8, s, (const void **)&dkey)) != PGQ_OK) break;
-			if ((st = stage_column(ws, 29, svalid, (size_t)m, s, (const void **)&svalid)) != PGQ_OK) break;
-			if ((st = stage_column(ws, 30, dvalid, (size_t)m, s, (const void **)&dvalid)) != PGQ_OK) break;
+			if ((st = stage_column(ws, 40, vkey, n8, s, (const void **)&vkey)) != PGQ_OK) break;
+			if ((st = stage_column(ws, 41, vvalid, (size_t)n, s, (const void **)&vvalid)) != PGQ_OK) break;
+			if ((st = stage_column(ws, 42, skey, m8, s, (const void **)&skey)) != PGQ_OK) break;
+			if ((st = stage_column(ws, 43, dkey, m8, s, (const void **)&dkey)) != PGQ_OK) break;
+			if ((st = stage_column(ws, 44, svalid, (size_t)m, s, (const void **)&svalid)) != PGQ_OK) break;
+			if ((st = stage_column(ws, 45, dvalid, (size_t)m, s, (const void **)&dvalid)) != PGQ_OK) break;
 		} else {
 			// the columns may have been produced on any stream of the caller: wait for the whole device once
 			cudaError_t e = cudaDeviceSynchronize();
@@ -2045,7 +2408,8 @@ static int csr_build_keys(pgq_ctx *ctx, int64_t n, const int64_t *vkey, const ui
 				break;
 			}
 		}
-		st = build_from_keys(csr, ws, s, vkey, vvalid, skey, dkey, svalid, dvalid, m);
+		st = undirected ? build_from_keys_undirected(csr, ws, s, vkey, vvalid, skey, dkey, svalid, dvalid, m)
+		                : build_from_keys(csr, ws, s, vkey, vvalid, skey, dkey, svalid, dvalid, m);
 	} while (0);
 	if (st != PGQ_OK) {
 		cudaStreamSynchronize(s); // (queued copies from the caller's columns must not outlive the call)
@@ -2066,7 +2430,7 @@ extern "C" int pgq_csr_build_keys(pgq_ctx *ctx, int64_t n_vertices, const int64_
                                   const int64_t *edge_dst_keys, const uint8_t *edge_src_valid,
                                   const uint8_t *edge_dst_valid, pgq_csr **out) {
 	return csr_build_keys(ctx, n_vertices, vertex_keys, vertex_key_valid, n_edges, edge_src_keys, edge_dst_keys,
-	                      edge_src_valid, edge_dst_valid, true, out);
+	                      edge_src_valid, edge_dst_valid, true, false, out);
 }
 
 extern "C" int pgq_csr_build_keys_device(pgq_ctx *ctx, int64_t n_vertices, const int64_t *d_vertex_keys,
@@ -2075,7 +2439,25 @@ extern "C" int pgq_csr_build_keys_device(pgq_ctx *ctx, int64_t n_vertices, const
                                          const uint8_t *d_edge_src_valid, const uint8_t *d_edge_dst_valid,
                                          pgq_csr **out) {
 	return csr_build_keys(ctx, n_vertices, d_vertex_keys, d_vertex_key_valid, n_edges, d_edge_src_keys,
-	                      d_edge_dst_keys, d_edge_src_valid, d_edge_dst_valid, false, out);
+	                      d_edge_dst_keys, d_edge_src_valid, d_edge_dst_valid, false, false, out);
+}
+
+extern "C" int pgq_csr_build_keys_undirected(pgq_ctx *ctx, int64_t n_vertices, const int64_t *vertex_keys,
+                                             const uint8_t *vertex_key_valid, int64_t n_edges,
+                                             const int64_t *edge_src_keys, const int64_t *edge_dst_keys,
+                                             const uint8_t *edge_src_valid, const uint8_t *edge_dst_valid,
+                                             pgq_csr **out) {
+	return csr_build_keys(ctx, n_vertices, vertex_keys, vertex_key_valid, n_edges, edge_src_keys, edge_dst_keys,
+	                      edge_src_valid, edge_dst_valid, true, true, out);
+}
+
+extern "C" int pgq_csr_build_keys_undirected_device(pgq_ctx *ctx, int64_t n_vertices, const int64_t *d_vertex_keys,
+                                                    const uint8_t *d_vertex_key_valid, int64_t n_edges,
+                                                    const int64_t *d_edge_src_keys, const int64_t *d_edge_dst_keys,
+                                                    const uint8_t *d_edge_src_valid, const uint8_t *d_edge_dst_valid,
+                                                    pgq_csr **out) {
+	return csr_build_keys(ctx, n_vertices, d_vertex_keys, d_vertex_key_valid, n_edges, d_edge_src_keys,
+	                      d_edge_dst_keys, d_edge_src_valid, d_edge_dst_valid, false, true, out);
 }
 
 extern "C" int pgq_csr_upload(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *v, const int64_t *e,

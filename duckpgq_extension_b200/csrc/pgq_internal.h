@@ -79,7 +79,7 @@ struct PullGraph {
 	int64_t n_short = 0, n_slices = 0, s_total = 0;
 };
 
-#define PGQ_WS_SLOTS 40
+#define PGQ_WS_SLOTS 60
 // Scratch of one path-function call (mask arrays etc.), pooled per context and grown on demand.
 struct Workspace {
 	pgq_ctx *ctx = nullptr; // the context whose pool it belongs to

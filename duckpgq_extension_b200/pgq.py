@@ -163,11 +163,16 @@ class DeviceCSR:
 
     @classmethod
     def build_from_keys(cls, ctx: Context, vertex_keys, edge_src, edge_dst, vertex_valid=None, src_valid=None,
-                        dst_valid=None) -> "DeviceCSR":
+                        dst_valid=None, undirected: bool = False) -> "DeviceCSR":
         """The directed CSR CTE (compressed_sparse_row.cpp:132-143,234-251) from key columns: vertex row i has key
         vertex_keys[i], edge k joins src key edge_src[k] to dst key edge_dst[k]; the *_valid arrays (1 = valid,
         0 = NULL) are optional.  Raises ConstraintException (csr_creation.cpp:121-125) when an edge with a
-        matching source has no or several matching destination rows."""
+        matching source has no or several matching destination rows.
+
+        undirected=True builds the undirected CSR CTE instead (compressed_sparse_row.cpp:125-130,145-172,192-223):
+        one row per distinct pair of the joined edges and their reverses, its edge id the smallest edge rowid of the
+        pair, neighbours in ascending rowid order; ConstraintException when a row's pair count differs from its
+        number of distinct other-end keys (NULL and unmatched ones included)."""
         vk, sk, dk = _i64(vertex_keys), _i64(edge_src), _i64(edge_dst)
         if sk.shape != dk.shape:
             raise ValueError("edge_src and edge_dst differ in length")
@@ -178,20 +183,20 @@ class DeviceCSR:
                 raise ValueError("a validity array differs in length from its key column")
         n = vk.shape[0]
         h = C.c_void_p()
-        _check(ctx._lib.pgq_csr_build_keys(ctx._h, n, _p64(vk), _pu8(vv), sk.shape[0], _p64(sk), _p64(dk), _pu8(sv),
-                                           _pu8(dv), C.byref(h)))
+        fn = ctx._lib.pgq_csr_build_keys_undirected if undirected else ctx._lib.pgq_csr_build_keys
+        _check(fn(ctx._h, n, _p64(vk), _pu8(vv), sk.shape[0], _p64(sk), _p64(dk), _pu8(sv), _pu8(dv), C.byref(h)))
         return cls(ctx, h, n)
 
     @classmethod
     def build_from_keys_device(cls, ctx: Context, n: int, m: int, d_vertex_keys: int, d_edge_src: int,
                                d_edge_dst: int, d_vertex_valid: int = 0, d_src_valid: int = 0,
-                               d_dst_valid: int = 0) -> "DeviceCSR":
+                               d_dst_valid: int = 0, undirected: bool = False) -> "DeviceCSR":
         """build_from_keys for columns already in HBM: raw device addresses of the int64 key columns (n vertex
         keys, m edge src / dst keys) and of the optional uint8 validity columns (0 = all valid)."""
         h = C.c_void_p()
-        _check(ctx._lib.pgq_csr_build_keys_device(ctx._h, n, d_vertex_keys or None, d_vertex_valid or None, m,
-                                                  d_edge_src or None, d_edge_dst or None, d_src_valid or None,
-                                                  d_dst_valid or None, C.byref(h)))
+        fn = ctx._lib.pgq_csr_build_keys_undirected_device if undirected else ctx._lib.pgq_csr_build_keys_device
+        _check(fn(ctx._h, n, d_vertex_keys or None, d_vertex_valid or None, m, d_edge_src or None, d_edge_dst or None,
+                  d_src_valid or None, d_dst_valid or None, C.byref(h)))
         return cls(ctx, h, n)
 
     @classmethod

@@ -177,6 +177,35 @@ int pgq_csr_build_keys_device(pgq_ctx *ctx, int64_t n_vertices, const int64_t *d
                               const uint8_t *d_vertex_key_valid, int64_t n_edges, const int64_t *d_edge_src_keys,
                               const int64_t *d_edge_dst_keys, const uint8_t *d_edge_src_valid,
                               const uint8_t *d_edge_dst_valid, pgq_csr **out);
+/* The undirected CSR CTE (CreateUndirectedCSRCTE, compressed_sparse_row.cpp:125-130,145-172,192-223; emitted for
+ * every undirected MATCH and for the weakly_connected_component / local_clustering_coefficient table functions) from
+ * the same columns as pgq_csr_build_keys.  A NULL key (validity byte 0) matches nothing.
+ *   - edges_cte = every (a, c, k) with vertex row a holding key e.src[k] and row c holding e.dst[k]; the CSR rows are
+ *     the distinct pairs (p, q) of edges_cte and its reverse (c, a, k), R in all: parallel edges collapse, a -> b and
+ *     b -> a give one row each way, a self-loop stays once;
+ *   - the degree of row a = the number of distinct "other end" values over the edges incident to a's key in either
+ *     direction (the UNION BY NAME of the two join branches grouped by rowid), a NULL or unmatched other end
+ *     included; S = their sum;
+ *   - S != R -> PGQ_ERR_CONSTRAINT (the text of csr_creation.cpp:121-125), and so is S == R with some row whose R(p)
+ *     differs from its degree (the reference scatters out of place there).  A dangling end balanced by a duplicated
+ *     key can give R(p) == degree(p) for every row: that CSR is well-formed and is built;
+ *   - two choices the reference leaves open (any_value, hash order) are defined: a pair's edge id is the SMALLEST edge
+ *     rowid of its group (both directions), and within a row the neighbours are in ascending rowid order;
+ *   - an edge table that joins to no pair gives the reference no CSR at all (create_csr_edge never runs); here, as for
+ *     pgq_csr_build_keys, it gives the edgeless CSR of n_vertices rows when S == 0 and PGQ_ERR_CONSTRAINT otherwise;
+ *   - n_vertices, n_edges and the 2 * sum ms * md rows before de-duplication must be < 2^31 -> PGQ_ERR_RANGE, checked
+ *     before they are allocated. */
+int pgq_csr_build_keys_undirected(pgq_ctx *ctx, int64_t n_vertices, const int64_t *vertex_keys,
+                                  const uint8_t *vertex_key_valid, int64_t n_edges, const int64_t *edge_src_keys,
+                                  const int64_t *edge_dst_keys, const uint8_t *edge_src_valid,
+                                  const uint8_t *edge_dst_valid, pgq_csr **out);
+/* pgq_csr_build_keys_undirected for columns that already live in HBM on the context's device, with the contract of
+ * pgq_csr_build_keys_device (inputs not modified; the call waits for the device before it reads them). */
+int pgq_csr_build_keys_undirected_device(pgq_ctx *ctx, int64_t n_vertices, const int64_t *d_vertex_keys,
+                                         const uint8_t *d_vertex_key_valid, int64_t n_edges,
+                                         const int64_t *d_edge_src_keys, const int64_t *d_edge_dst_keys,
+                                         const uint8_t *d_edge_src_valid, const uint8_t *d_edge_dst_valid,
+                                         pgq_csr **out);
 /* get_csr_v / get_csr_e (src/core/functions/table/pgq_scan.cpp:84-111): copy the CSR back in the
  * reference's layout.  Any output pointer may be NULL. */
 int pgq_csr_download(pgq_csr *csr, int64_t *v_out /* n+2 */, int64_t *e_out /* m */, int64_t *edge_ids_out /* m */);

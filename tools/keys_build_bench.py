@@ -16,6 +16,17 @@ runs after one warm-up run of the device phases (the host route, whose searchsor
     host_build_call_ms     pgq_csr_build on the mapped rowids (host clock)
 The CSRs of the three routes are downloaded once and compared.  Prints one JSON object (and writes
 DIR/keys_build_bench.json with --out), with the GPU's name and power limit.
+
+    python tools/keys_build_bench.py --undirected [--scale 22] [--reps 5] [--out DIR]
+
+times the directed and the undirected build (pgq_csr_build_keys_undirected) on the same columns instead:
+    {dir,undir}_host_call_ms    from host columns (host clock)
+    {dir,undir}_device_call_ms  from the columns in HBM (CUDA events around the call)
+    {dir,undir}_rows_call_ms    pgq_csr_build_device on the rows the key build hands on (the directed edge rows; the
+                                distinct pairs of both directions), already in HBM: the difference to the device call
+                                is the join (and the de-duplication) on the device
+The oracle's restatements run once each, for scale (oracle_{dir,undir}_ms); all CSRs are compared with them.
+Writes DIR/keys_build_bench_undirected_<scale>.json with --out.
 """
 from __future__ import annotations
 
@@ -67,7 +78,10 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--host-reps", type=int, default=1, help="timed runs of the host route (minutes each at scale 22)")
     ap.add_argument("--out", default=None)
+    ap.add_argument("--undirected", action="store_true", help="time the directed and the undirected key builds")
     args = ap.parse_args()
+    if args.undirected:
+        return main_undirected(args)
 
     import torch
     if not torch.cuda.is_available():
@@ -139,6 +153,75 @@ def main():
     if args.out:
         os.makedirs(args.out, exist_ok=True)
         with open(os.path.join(args.out, "keys_build_bench.json"), "w") as f:
+            f.write(line + "\n")
+
+
+def main_undirected(args):
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("no CUDA device: this measurement needs the GPU")
+    from oracle import pgq_oracle_keys as orck
+    from oracle import pgq_oracle_keys_undirected as orcu
+    info = gpu_info()
+    n, src, dst = datagen.rmat_edges(args.scale)
+    m = len(src)
+    vkey = np.random.default_rng(args.scale).permutation(n).astype(np.int64)
+    skey, dkey = vkey[src], vkey[dst]
+    ctx = pgq.default_context(0)
+    # the rows each build hands to the common pipeline: the edges as they are; the distinct pairs of both directions
+    pairs = np.unique(np.concatenate([src.astype(np.int64) * n + dst, dst.astype(np.int64) * n + src]))
+    rows = {"dir": (torch.from_numpy(src.astype(np.int32)).cuda(), torch.from_numpy(dst.astype(np.int32)).cuda()),
+            "undir": (torch.from_numpy((pairs // n).astype(np.int32)).cuda(),
+                      torch.from_numpy((pairs % n).astype(np.int32)).cuda())}
+    cols = [torch.from_numpy(c).cuda() for c in (vkey, skey, dkey)]
+
+    def ev():
+        e = torch.cuda.Event(enable_timing=True)
+        e.record()
+        return e
+
+    phases = {f"{d}_{k}": [] for d in ("dir", "undir") for k in ("host_call_ms", "device_call_ms", "rows_call_ms")}
+    got = {}
+    for rep in range(args.reps + 1):
+        t = {}
+        for d, und in (("dir", False), ("undir", True)):
+            t0 = time.perf_counter()
+            a = pgq.DeviceCSR.build_from_keys(ctx, vkey, skey, dkey, undirected=und)
+            t[f"{d}_host_call_ms"] = (time.perf_counter() - t0) * 1e3
+            torch.cuda.synchronize()
+            e0 = ev()
+            b = pgq.DeviceCSR.build_from_keys_device(ctx, n, m, *(c.data_ptr() for c in cols), undirected=und)
+            e1 = ev()
+            r = pgq.DeviceCSR.build_device(ctx, n, rows[d][0].shape[0], rows[d][0].data_ptr(), rows[d][1].data_ptr())
+            e2 = ev()
+            torch.cuda.synchronize()
+            t[f"{d}_device_call_ms"] = e0.elapsed_time(e1)
+            t[f"{d}_rows_call_ms"] = e1.elapsed_time(e2)
+            if rep == 0:
+                got[d] = (a.download(), b.download())
+            for csr in (a, b, r):
+                csr.free()
+        if rep >= 1:
+            for k, x in t.items():
+                phases[k].append(x)
+        print(f"rep {rep}: " + ", ".join(f"{k} {x:.1f}" for k, x in t.items()), file=sys.stderr, flush=True)
+    results = {}
+    for d, fn in (("dir", orck.csr_build_keys), ("undir", orcu.csr_build_keys_undirected)):
+        t0 = time.perf_counter()
+        ref = fn(vkey, skey, dkey)
+        results[f"oracle_{d}_ms"] = round((time.perf_counter() - t0) * 1e3, 1)
+        results[f"{d}_equals_oracle"] = all(all(np.array_equal(x, y) for x, y in zip(g, ref)) for g in got[d])
+    med = {k: round(float(np.median(v)), 2) for k, v in phases.items()}
+    join = {d: round(med[f"{d}_device_call_ms"] - med[f"{d}_rows_call_ms"], 2) for d in ("dir", "undir")}
+    out = {"scale": args.scale, "n": n, "m": m, "undirected_rows": int(pairs.shape[0]), "reps": args.reps, **info,
+           **results, "median_ms": med, "join_ms": join,
+           "join_share": {d: round(join[d] / med[f"{d}_device_call_ms"], 3) for d in join},
+           "all_ms": {k: [round(x, 2) for x in v] for k, v in phases.items()}}
+    line = json.dumps(out)
+    print(line)
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+        with open(os.path.join(args.out, f"keys_build_bench_undirected_{args.scale}.json"), "w") as f:
             f.write(line + "\n")
 
 
