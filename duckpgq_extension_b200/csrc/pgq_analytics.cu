@@ -41,8 +41,8 @@ __global__ void k_an_odeg(const int32_t *__restrict__ off, const int32_t *__rest
 static int ref_offsets(pgq_csr *csr, Workspace *ws, cudaStream_t s, int32_t **ref_off, int64_t *launches) {
 	const int64_t n = csr->n;
 	int32_t *ro, *scan_tmp;
-	PGQ_TRY(pgq_ws_reserve(ws, 16, (size_t)(n + 3) * sizeof(int32_t), (void **)&ro));
-	PGQ_TRY(pgq_ws_reserve(ws, 17, pgq_scan_tmp_elems(n + 3) * sizeof(int32_t), (void **)&scan_tmp));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_AN_REF_OFF, (size_t)(n + 3) * sizeof(int32_t), (void **)&ro));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_AN_SCAN, pgq_scan_tmp_elems(n + 3) * sizeof(int32_t), (void **)&scan_tmp));
 	k_an_odeg<<<an_grid(n + 3, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->out.off, csr->perm, n, ro);
 	PGQ_CUDA(cudaGetLastError());
 	PGQ_TRY(pgq_scan_exclusive_i32(ro, ro, n + 3, scan_tmp, s));
@@ -284,88 +284,82 @@ extern "C" int pgq_local_clustering_coefficient(pgq_csr *csr, int64_t p, const i
 		return PGQ_OK;
 	}
 	PGQ_CUDA(cudaSetDevice(csr->ctx->device));
-	Workspace *ws;
-	PGQ_TRY(pgq_ws_acquire(csr->ctx, &ws));
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
-	int rc = PGQ_OK;
-	do {
-		int64_t *d_src;
-		uint8_t *d_sv = nullptr, *d_ov;
-		float *d_out;
-		int32_t *big_rows;
-		int *big_count, *h_big;
-		u64 *big_cnt;
-		uint32_t *bitmap;
-		const size_t b8 = (size_t)p * sizeof(int64_t);
-		if ((rc = pgq_ws_reserve(ws, 16, b8, (void **)&d_src)) != PGQ_OK) break;
-		if ((rc = pgq_ws_reserve(ws, 17, (size_t)p * sizeof(float), (void **)&d_out)) != PGQ_OK) break;
-		if ((rc = pgq_ws_reserve(ws, 18, (size_t)p, (void **)&d_ov)) != PGQ_OK) break;
-		if ((rc = pgq_ws_reserve(ws, 19, (size_t)p * sizeof(int32_t) + 64, (void **)&big_rows)) != PGQ_OK) break;
-		if ((rc = pgq_ws_reserve(ws, 20, (size_t)p * sizeof(u64), (void **)&big_cnt)) != PGQ_OK) break;
-		if ((rc = pgq_ws_pinned(ws, 256, (void **)&h_big)) != PGQ_OK) break;
-		big_count = big_rows + p;
-		cudaEventRecord(ws->ev_begin, s);
-		cudaMemcpyAsync(d_src, src, b8, cudaMemcpyHostToDevice, s);
-		st.h2d_bytes = (int64_t)b8;
-		if (src_valid) {
-			if ((rc = pgq_ws_reserve(ws, 21, (size_t)p, (void **)&d_sv)) != PGQ_OK) break;
-			cudaMemcpyAsync(d_sv, src_valid, (size_t)p, cudaMemcpyHostToDevice, s);
-			st.h2d_bytes += p;
+	int64_t *d_src;
+	uint8_t *d_sv, *d_ov;
+	float *d_out;
+	int32_t *big_rows;
+	int *big_count, *h_big;
+	u64 *big_cnt;
+	uint32_t *bitmap;
+	const size_t b8 = (size_t)p * sizeof(int64_t);
+	PGQ_TRY(pgq_ws_reserve(ws, WS_LCC_OUT, (size_t)p * sizeof(float), (void **)&d_out));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_LCC_OUT_VALID, (size_t)p, (void **)&d_ov));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_LCC_BIG_ROWS, (size_t)p * sizeof(int32_t) + 64, (void **)&big_rows));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_LCC_BIG_CNT, (size_t)p * sizeof(u64), (void **)&big_cnt));
+	PGQ_TRY(pgq_ws_pinned(ws, 256, (void **)&h_big));
+	big_count = big_rows + p;
+	cudaEventRecord(ws->ev_begin, s);
+	PGQ_TRY(stage_column(ws, WS_LCC_SRC, src, b8, (const void **)&d_src));
+	PGQ_TRY(stage_column(ws, WS_LCC_SRC_VALID, src_valid, (size_t)p, (const void **)&d_sv));
+	st.h2d_bytes = (int64_t)b8 + (src_valid ? p : 0);
+	cudaMemsetAsync(big_count, 0, sizeof(int), s);
+	k_lcc_rows<<<(unsigned)std::min<int64_t>(p, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(
+	    p, d_src, d_sv, csr->perm, csr->out.off, csr->out.adj, d_out, d_ov, big_rows, big_count);
+	st.kernel_launches++;
+	cudaError_t e = cudaMemcpyAsync(h_big, big_count, sizeof(int), cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) {
+		e = cudaStreamSynchronize(s);
+	}
+	if (e != cudaSuccess) {
+		return pgq_fail(PGQ_ERR_CUDA, "local_clustering_coefficient failed: %s", cudaGetErrorString(e));
+	}
+	const int nbig = *h_big;
+	if (nbig > 0) {
+		// one bitmap per row of a group, as many rows as 256 MB of bitmaps hold (at most 65535, the grid's y limit);
+		// zeroed once, and after a group only the words it marked are cleared again
+		const int64_t words = csr->n / 32 + 1;
+		const int group = (int)std::max<int64_t>(
+		    1, std::min<int64_t>({(int64_t)nbig, ((int64_t)256 << 20) / (words * 4), (int64_t)65535}));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_LCC_BITMAP, (size_t)(group * words) * sizeof(uint32_t), (void **)&bitmap));
+		cudaMemsetAsync(bitmap, 0, (size_t)(group * words) * sizeof(uint32_t), s);
+		cudaMemsetAsync(big_cnt, 0, (size_t)nbig * sizeof(u64), s);
+		const unsigned gx_mark = (unsigned)std::max(1, csr->ctx->sm_count * 4 / group);
+		const unsigned gx_count = (unsigned)std::max(4, csr->ctx->sm_count * 8 / group);
+		for (int i0 = 0; i0 < nbig; i0 += group) {
+			const unsigned gy = (unsigned)std::min(group, nbig - i0);
+			k_lcc_big_mark<<<dim3(gx_mark, gy), 256, 0, s>>>(i0, big_rows, d_src, csr->perm, csr->out.off, csr->out.adj,
+			                                                 bitmap, words, true);
+			k_lcc_big_count<<<dim3(gx_count, gy), 256, 0, s>>>(i0, big_rows, d_src, csr->perm, csr->out.off,
+			                                                   csr->out.adj, bitmap, words, big_cnt);
+			k_lcc_big_mark<<<dim3(gx_mark, gy), 256, 0, s>>>(i0, big_rows, d_src, csr->perm, csr->out.off, csr->out.adj,
+			                                                 bitmap, words, false);
+			st.kernel_launches += 3;
 		}
-		cudaMemsetAsync(big_count, 0, sizeof(int), s);
-		k_lcc_rows<<<(unsigned)std::min<int64_t>(p, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(
-		    p, d_src, d_sv, csr->perm, csr->out.off, csr->out.adj, d_out, d_ov, big_rows, big_count);
+		k_lcc_big_finish<<<an_grid(nbig, 128, 1024), 128, 0, s>>>(nbig, big_rows, d_src, csr->perm, csr->out.off, big_cnt,
+		                                                          d_out);
 		st.kernel_launches++;
-		if (cudaMemcpyAsync(h_big, big_count, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-		    cudaStreamSynchronize(s) != cudaSuccess) {
-			break; // (reported below)
-		}
-		const int nbig = *h_big;
-		if (nbig > 0) {
-			// one bitmap per row of a group, as many rows as 256 MB of bitmaps hold (at most 65535, the grid's y limit);
-			// zeroed once, and after a group only the words it marked are cleared again
-			const int64_t words = csr->n / 32 + 1;
-			const int group = (int)std::max<int64_t>(
-			    1, std::min<int64_t>({(int64_t)nbig, ((int64_t)256 << 20) / (words * 4), (int64_t)65535}));
-			if ((rc = pgq_ws_reserve(ws, 22, (size_t)(group * words) * sizeof(uint32_t), (void **)&bitmap)) != PGQ_OK) break;
-			cudaMemsetAsync(bitmap, 0, (size_t)(group * words) * sizeof(uint32_t), s);
-			cudaMemsetAsync(big_cnt, 0, (size_t)nbig * sizeof(u64), s);
-			const unsigned gx_mark = (unsigned)std::max(1, csr->ctx->sm_count * 4 / group);
-			const unsigned gx_count = (unsigned)std::max(4, csr->ctx->sm_count * 8 / group);
-			for (int i0 = 0; i0 < nbig; i0 += group) {
-				const unsigned gy = (unsigned)std::min(group, nbig - i0);
-				k_lcc_big_mark<<<dim3(gx_mark, gy), 256, 0, s>>>(i0, big_rows, d_src, csr->perm, csr->out.off, csr->out.adj,
-				                                                 bitmap, words, true);
-				k_lcc_big_count<<<dim3(gx_count, gy), 256, 0, s>>>(i0, big_rows, d_src, csr->perm, csr->out.off,
-				                                                   csr->out.adj, bitmap, words, big_cnt);
-				k_lcc_big_mark<<<dim3(gx_mark, gy), 256, 0, s>>>(i0, big_rows, d_src, csr->perm, csr->out.off, csr->out.adj,
-				                                                 bitmap, words, false);
-				st.kernel_launches += 3;
-			}
-			k_lcc_big_finish<<<an_grid(nbig, 128, 1024), 128, 0, s>>>(nbig, big_rows, d_src, csr->perm, csr->out.off, big_cnt,
-			                                                          d_out);
-			st.kernel_launches++;
-		}
-		cudaMemcpyAsync(out, d_out, (size_t)p * sizeof(float), cudaMemcpyDeviceToHost, s);
-		cudaMemcpyAsync(out_valid, d_ov, (size_t)p, cudaMemcpyDeviceToHost, s);
-		cudaEventRecord(ws->ev_end, s);
-		st.d2h_bytes = (int64_t)p * (int64_t)(sizeof(float) + 1);
-	} while (0);
-	cudaError_t e = cudaStreamSynchronize(s); // (also on the error paths: nothing may outlive the call)
-	if (rc == PGQ_OK && (e != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess)) {
-		rc = pgq_fail(PGQ_ERR_CUDA, "local_clustering_coefficient failed: %s", cudaGetErrorString(e));
 	}
-	if (rc == PGQ_OK) {
-		float ms = 0.0f;
-		cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end);
-		st.total_ms = ms;
+	cudaMemcpyAsync(out, d_out, (size_t)p * sizeof(float), cudaMemcpyDeviceToHost, s);
+	cudaMemcpyAsync(out_valid, d_ov, (size_t)p, cudaMemcpyDeviceToHost, s);
+	cudaEventRecord(ws->ev_end, s);
+	st.d2h_bytes = (int64_t)p * (int64_t)(sizeof(float) + 1);
+	e = cudaStreamSynchronize(s);
+	if (e != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess) {
+		return pgq_fail(PGQ_ERR_CUDA, "local_clustering_coefficient failed: %s", cudaGetErrorString(e));
 	}
+	g.settled = true;
+	float ms = 0.0f;
+	cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end);
+	st.total_ms = ms;
 	cudaGetLastError();
-	pgq_ws_release(csr->ctx, ws);
-	if (rc == PGQ_OK && stats) {
+	if (stats) {
 		*stats = st;
 	}
-	return rc;
+	return PGQ_OK;
 }
 
 // =================================================================================================================
@@ -525,13 +519,13 @@ static int pagerank_compute(pgq_csr *csr, Workspace *ws, pgq_stats *st) {
 	// the in-CSC in original ids, in-lists by ascending source: the edges in reference order, stably sorted by target
 	int32_t *key_a, *key_b, *val_a, *val_b, *key_res, *in_src, *in_off, *scan_tmp, *dflag;
 	const size_t mb = (size_t)std::max<int64_t>(m, 1) * sizeof(int32_t);
-	PGQ_TRY(pgq_ws_reserve(ws, 18, mb, (void **)&key_a));
-	PGQ_TRY(pgq_ws_reserve(ws, 19, mb, (void **)&key_b));
-	PGQ_TRY(pgq_ws_reserve(ws, 20, mb, (void **)&val_a));
-	PGQ_TRY(pgq_ws_reserve(ws, 21, mb, (void **)&val_b));
-	PGQ_TRY(pgq_ws_reserve(ws, 22, (size_t)(vsize + 1) * sizeof(int32_t), (void **)&in_off));
-	PGQ_TRY(pgq_ws_reserve(ws, 23, pgq_scan_tmp_elems(vsize + 1) * sizeof(int32_t), (void **)&scan_tmp));
-	PGQ_TRY(pgq_ws_reserve(ws, 24, (size_t)(vsize + 1) * sizeof(int32_t), (void **)&dflag));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_PR_KEY_A, mb, (void **)&key_a));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_PR_KEY_B, mb, (void **)&key_b));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_PR_VAL_A, mb, (void **)&val_a));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_PR_VAL_B, mb, (void **)&val_b));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_PR_IN_OFF, (size_t)(vsize + 1) * sizeof(int32_t), (void **)&in_off));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_PR_SCAN, pgq_scan_tmp_elems(vsize + 1) * sizeof(int32_t), (void **)&scan_tmp));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_PR_DFLAG, (size_t)(vsize + 1) * sizeof(int32_t), (void **)&dflag));
 	PGQ_CUDA(cudaMemsetAsync(in_off, 0, (size_t)(vsize + 1) * sizeof(int32_t), s));
 	in_src = val_a;
 	if (m > 0) {
@@ -547,11 +541,11 @@ static int pagerank_compute(pgq_csr *csr, Workspace *ws, pgq_stats *st) {
 	double *rank, *temp, *contrib, *dangling, *d_total;
 	u64 *max_bits, *h_max;
 	const size_t vb = (size_t)vsize * sizeof(double);
-	PGQ_TRY(pgq_ws_reserve(ws, 25, vb, (void **)&rank));
-	PGQ_TRY(pgq_ws_reserve(ws, 26, vb, (void **)&temp));
-	PGQ_TRY(pgq_ws_reserve(ws, 27, vb, (void **)&contrib));
-	PGQ_TRY(pgq_ws_reserve(ws, 12, vb, (void **)&dangling));
-	PGQ_TRY(pgq_ws_reserve(ws, 13, 256, (void **)&d_total));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_PR_RANK, vb, (void **)&rank));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_PR_TEMP, vb, (void **)&temp));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_PR_CONTRIB, vb, (void **)&contrib));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_PR_DANGLING, vb, (void **)&dangling));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_PR_TOTAL, 256, (void **)&d_total));
 	PGQ_TRY(pgq_ws_pinned(ws, 256, (void **)&h_max));
 	max_bits = (u64 *)(d_total + 1);
 	k_pr_init<<<an_grid(vsize + 1, 256, big_grid), 256, 0, s>>>(vsize, ref_off, rank, contrib, dflag);
@@ -773,17 +767,17 @@ static int wcc_compute(pgq_csr *csr, Workspace *ws, pgq_stats *st) {
 		int32_t *e[6], *comp, *hook, *mk, *ma, *mb, *key_b, *idx_a, *idx_b, *key_res, *idx_res;
 		const size_t mb_bytes = (size_t)m * sizeof(int32_t), nb = (size_t)(n + 1) * sizeof(int32_t);
 		for (int i = 0; i < 6; i++) {
-			PGQ_TRY(pgq_ws_reserve(ws, 18 + i, mb_bytes, (void **)&e[i]));
+			PGQ_TRY(pgq_ws_reserve(ws, (WsSlot)(WS_WCC_EDGES + i), mb_bytes, (void **)&e[i]));
 		}
 		u64 *best;
 		int *flags, *h_flags;
-		PGQ_TRY(pgq_ws_reserve(ws, 24, nb, (void **)&comp));
-		PGQ_TRY(pgq_ws_reserve(ws, 25, nb, (void **)&hook));
-		PGQ_TRY(pgq_ws_reserve(ws, 26, (size_t)n * sizeof(u64), (void **)&best));
-		PGQ_TRY(pgq_ws_reserve(ws, 27, nb, (void **)&mk));
-		PGQ_TRY(pgq_ws_reserve(ws, 11, nb, (void **)&ma));
-		PGQ_TRY(pgq_ws_reserve(ws, 12, nb, (void **)&mb));
-		PGQ_TRY(pgq_ws_reserve(ws, 13, 256, (void **)&flags)); // [0] merges, [1] jump changed, [2] edges kept
+		PGQ_TRY(pgq_ws_reserve(ws, WS_WCC_COMP, nb, (void **)&comp));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_WCC_HOOK, nb, (void **)&hook));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_WCC_BEST, (size_t)n * sizeof(u64), (void **)&best));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_WCC_MERGE_POS, nb, (void **)&mk));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_WCC_MERGE_A, nb, (void **)&ma));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_WCC_MERGE_B, nb, (void **)&mb));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_WCC_FLAGS, 256, (void **)&flags)); // [0] merges, [1] jump changed, [2] edges kept
 		PGQ_TRY(pgq_ws_pinned(ws, 256, (void **)&h_flags));
 		k_wcc_edges<<<an_grid(n * 32, 256, big_grid), 256, 0, s>>>(csr->out.off, csr->out.adj, csr->inv, n, ref_off, e[0],
 		                                                            e[1], e[2]);
@@ -823,9 +817,9 @@ static int wcc_compute(pgq_csr *csr, Workspace *ws, pgq_stats *st) {
 		n_merge = h_flags[0];
 		if (n_merge > 0) {
 			// the merge positions in ascending order (a stable radix sort of (position, index))
-			PGQ_TRY(pgq_ws_reserve(ws, 18, (size_t)n_merge * sizeof(int32_t), (void **)&key_b));
-			PGQ_TRY(pgq_ws_reserve(ws, 19, (size_t)n_merge * sizeof(int32_t), (void **)&idx_a));
-			PGQ_TRY(pgq_ws_reserve(ws, 20, (size_t)n_merge * sizeof(int32_t), (void **)&idx_b));
+			PGQ_TRY(pgq_ws_reserve(ws, WS_WCC_SORT_KEY, (size_t)n_merge * sizeof(int32_t), (void **)&key_b));
+			PGQ_TRY(pgq_ws_reserve(ws, WS_WCC_SORT_IDX_A, (size_t)n_merge * sizeof(int32_t), (void **)&idx_a));
+			PGQ_TRY(pgq_ws_reserve(ws, WS_WCC_SORT_IDX_B, (size_t)n_merge * sizeof(int32_t), (void **)&idx_b));
 			k_wcc_init<<<an_grid(n_merge, 256, big_grid), 256, 0, s>>>(n_merge, idx_a);
 			PGQ_CUDA(cudaGetLastError());
 			PGQ_TRY(radix_sort_pairs(ws, mk, key_b, idx_a, idx_b, n_merge, bits_for(m), s, &key_res, &idx_res));
@@ -874,23 +868,22 @@ static int ensure_cached(pgq_csr *csr, bool pgq_csr::*done, pgq_stats *st, F com
 		return PGQ_OK;
 	}
 	PGQ_CUDA(cudaSetDevice(csr->ctx->device));
-	Workspace *ws;
-	PGQ_TRY(pgq_ws_acquire(csr->ctx, &ws));
+	WsGuard wg(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &wg.ws));
+	Workspace *ws = wg.ws;
 	cudaEventRecord(ws->ev_begin, ws->stream);
-	int rc = compute(csr, ws, st);
+	PGQ_TRY(compute(csr, ws, st));
 	cudaEventRecord(ws->ev_end, ws->stream);
 	cudaError_t e = cudaStreamSynchronize(ws->stream);
-	if (rc == PGQ_OK && (e != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess)) {
-		rc = pgq_fail(PGQ_ERR_CUDA, "analytics computation failed: %s", cudaGetErrorString(e));
+	if (e != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess) {
+		return pgq_fail(PGQ_ERR_CUDA, "analytics computation failed: %s", cudaGetErrorString(e));
 	}
-	if (rc == PGQ_OK) {
-		float ms = 0.0f;
-		cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end);
-		st->total_ms = ms;
-	}
+	wg.settled = true;
+	float ms = 0.0f;
+	cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end);
+	st->total_ms = ms;
 	cudaGetLastError();
-	pgq_ws_release(csr->ctx, ws);
-	return rc;
+	return PGQ_OK;
 }
 
 static int check_cached_call(pgq_csr *csr, int64_t p, const int64_t *src, const void *out, const uint8_t *out_valid) {

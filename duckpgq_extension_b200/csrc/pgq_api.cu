@@ -23,30 +23,6 @@ static int check_call(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t
 	return PGQ_OK;
 }
 
-struct WsGuard {
-	pgq_ctx *ctx;
-	Workspace *ws = nullptr;
-	cudaStream_t used = nullptr; // a caller-provided stream the work was enqueued on, if any
-	bool has_used = false;
-	bool settled = false; // the call has synchronised the workspace stream itself
-	explicit WsGuard(pgq_ctx *c) : ctx(c) {
-	}
-	~WsGuard() {
-		if (ws) {
-			if (!settled) {
-				// error path: copies from / to the caller's buffers may still be queued on the workspace
-				// stream; they must not outlive the call (nor leak into the workspace's next user)
-				cudaStreamSynchronize(ws->stream);
-				if (has_used) {
-					cudaStreamSynchronize(used); // kernels queued on the caller's stream still touch the workspace
-				}
-				cudaGetLastError();
-			}
-			pgq_ws_release(ctx, ws);
-		}
-	}
-};
-
 extern "C" int pgq_iterativelength_device(pgq_csr *csr, int64_t p, const int64_t *d_src, const int64_t *d_dst,
                                           const uint8_t *d_src_valid, const pgq_options *opts, int64_t *d_out_len,
                                           uint8_t *d_out_valid, void *stream, pgq_stats *stats) {
@@ -84,20 +60,14 @@ extern "C" int pgq_iterativelength(pgq_csr *csr, int64_t p, const int64_t *src, 
 	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
 	int64_t *d_src, *d_dst, *d_len;
-	uint8_t *d_sv = nullptr, *d_ov;
+	uint8_t *d_sv, *d_ov;
 	const size_t b8 = (size_t)p * sizeof(int64_t);
-	PGQ_TRY(pgq_ws_reserve(ws, 6, b8, (void **)&d_src));
-	PGQ_TRY(pgq_ws_reserve(ws, 7, b8, (void **)&d_dst));
-	PGQ_TRY(pgq_ws_reserve(ws, 9, b8, (void **)&d_len));
-	PGQ_TRY(pgq_ws_reserve(ws, 10, (size_t)p, (void **)&d_ov));
-	PGQ_CUDA(cudaMemcpyAsync(d_src, src, b8, cudaMemcpyHostToDevice, s));
-	PGQ_CUDA(cudaMemcpyAsync(d_dst, dst, b8, cudaMemcpyHostToDevice, s));
-	int64_t h2d = 2 * (int64_t)b8;
-	if (src_valid) {
-		PGQ_TRY(pgq_ws_reserve(ws, 8, (size_t)p, (void **)&d_sv));
-		PGQ_CUDA(cudaMemcpyAsync(d_sv, src_valid, (size_t)p, cudaMemcpyHostToDevice, s));
-		h2d += p;
-	}
+	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
+	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d_dst));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LEN, b8, (void **)&d_len));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_ov));
+	PGQ_TRY(stage_column(ws, WS_IN_VALID, src_valid, (size_t)p, (const void **)&d_sv));
+	const int64_t h2d = 2 * (int64_t)b8 + (src_valid ? p : 0);
 	pgq_stats st;
 	memset(&st, 0, sizeof(st));
 	PGQ_TRY(pgq_bfs_lengths_device(csr, ws, p, d_src, d_dst, d_sv, opts, d_len, d_ov, s, &st));
@@ -132,20 +102,17 @@ extern "C" int pgq_iterativelength_bidirectional(pgq_csr *csr, int64_t p, const 
 	int64_t h2d = 0;
 	std::vector<uint8_t> valid; // a row searches only when both of its ids are valid
 	if (p > 0) {
-		PGQ_TRY(pgq_ws_reserve(ws, 6, b8, (void **)&d_src));
-		PGQ_TRY(pgq_ws_reserve(ws, 7, b8, (void **)&d_dst));
-		PGQ_TRY(pgq_ws_reserve(ws, 9, b8, (void **)&d_len));
-		PGQ_TRY(pgq_ws_reserve(ws, 10, (size_t)p, (void **)&d_ov));
-		PGQ_CUDA(cudaMemcpyAsync(d_src, src, b8, cudaMemcpyHostToDevice, s));
-		PGQ_CUDA(cudaMemcpyAsync(d_dst, dst, b8, cudaMemcpyHostToDevice, s));
+		PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
+		PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d_dst));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LEN, b8, (void **)&d_len));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_ov));
 		h2d = 2 * (int64_t)b8;
 		if (src_valid || dst_valid) {
 			valid.resize((size_t)p);
 			for (int64_t i = 0; i < p; i++) {
 				valid[(size_t)i] = (!src_valid || src_valid[i]) && (!dst_valid || dst_valid[i]) ? 1 : 0;
 			}
-			PGQ_TRY(pgq_ws_reserve(ws, 8, (size_t)p, (void **)&d_v));
-			PGQ_CUDA(cudaMemcpyAsync(d_v, valid.data(), (size_t)p, cudaMemcpyHostToDevice, s));
+			PGQ_TRY(stage_column(ws, WS_IN_VALID, valid.data(), (size_t)p, (const void **)&d_v));
 			h2d += p;
 		}
 	}
@@ -208,20 +175,14 @@ extern "C" int pgq_reachability(pgq_csr *csr, int64_t p, const int64_t *src, con
 	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
 	int64_t *d_src, *d_dst, *d_len;
-	uint8_t *d_sv = nullptr, *d_ov;
+	uint8_t *d_sv, *d_ov;
 	const size_t b8 = (size_t)p * sizeof(int64_t);
-	PGQ_TRY(pgq_ws_reserve(ws, 6, b8, (void **)&d_src));
-	PGQ_TRY(pgq_ws_reserve(ws, 7, b8, (void **)&d_dst));
-	PGQ_TRY(pgq_ws_reserve(ws, 9, b8, (void **)&d_len));
-	PGQ_TRY(pgq_ws_reserve(ws, 10, (size_t)p, (void **)&d_ov));
-	PGQ_CUDA(cudaMemcpyAsync(d_src, src, b8, cudaMemcpyHostToDevice, s));
-	PGQ_CUDA(cudaMemcpyAsync(d_dst, h_dst, b8, cudaMemcpyHostToDevice, s));
-	int64_t h2d = 2 * (int64_t)b8;
-	if (h_sv) {
-		PGQ_TRY(pgq_ws_reserve(ws, 8, (size_t)p, (void **)&d_sv));
-		PGQ_CUDA(cudaMemcpyAsync(d_sv, h_sv, (size_t)p, cudaMemcpyHostToDevice, s));
-		h2d += p;
-	}
+	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
+	PGQ_TRY(stage_column(ws, WS_IN_DST, h_dst, b8, (const void **)&d_dst));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LEN, b8, (void **)&d_len));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_ov));
+	PGQ_TRY(stage_column(ws, WS_IN_VALID, h_sv, (size_t)p, (const void **)&d_sv));
+	const int64_t h2d = 2 * (int64_t)b8 + (h_sv ? p : 0);
 	pgq_stats st;
 	memset(&st, 0, sizeof(st));
 	PGQ_TRY(pgq_bfs_reachability_device(csr, ws, p, d_src, d_dst, d_sv, src, h_sv, opts, d_len, d_ov, s, &st));
@@ -262,21 +223,15 @@ extern "C" int pgq_shortestpath(pgq_csr *csr, int64_t p, const int64_t *src, con
 	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
 	int64_t *d_src, *d_dst, *d_off, *d_lens;
-	uint8_t *d_sv = nullptr, *d_ov;
+	uint8_t *d_sv, *d_ov;
 	const size_t b8 = (size_t)p * sizeof(int64_t);
-	PGQ_TRY(pgq_ws_reserve(ws, 6, b8, (void **)&d_src));
-	PGQ_TRY(pgq_ws_reserve(ws, 7, b8, (void **)&d_dst));
-	PGQ_TRY(pgq_ws_reserve(ws, 11, b8, (void **)&d_off));
-	PGQ_TRY(pgq_ws_reserve(ws, 12, b8, (void **)&d_lens));
-	PGQ_TRY(pgq_ws_reserve(ws, 10, (size_t)p, (void **)&d_ov));
-	PGQ_CUDA(cudaMemcpyAsync(d_src, src, b8, cudaMemcpyHostToDevice, s));
-	PGQ_CUDA(cudaMemcpyAsync(d_dst, dst, b8, cudaMemcpyHostToDevice, s));
-	int64_t h2d = 2 * (int64_t)b8;
-	if (src_valid) {
-		PGQ_TRY(pgq_ws_reserve(ws, 8, (size_t)p, (void **)&d_sv));
-		PGQ_CUDA(cudaMemcpyAsync(d_sv, src_valid, (size_t)p, cudaMemcpyHostToDevice, s));
-		h2d += p;
-	}
+	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
+	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d_dst));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_OFFSETS, b8, (void **)&d_off));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LENGTHS, b8, (void **)&d_lens));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_ov));
+	PGQ_TRY(stage_column(ws, WS_IN_VALID, src_valid, (size_t)p, (const void **)&d_sv));
+	const int64_t h2d = 2 * (int64_t)b8 + (src_valid ? p : 0);
 	pgq_stats st;
 	memset(&st, 0, sizeof(st));
 	int64_t *d_elems = nullptr;

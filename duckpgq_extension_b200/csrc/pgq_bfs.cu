@@ -22,6 +22,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <string>
 #include <thread>
 #include <unordered_set>
@@ -1530,44 +1531,6 @@ static int pick_lanes(const pgq_options *opts, int64_t n, int64_t searches, bool
 	return lanes;
 }
 
-// workspace slots
-enum {
-	// (slots 0..2 are scratch of the CSR build and of cheapest_path_length: the mask arrays have slots of their
-	// own because a workspace remembers which of their rows are known to be zero, Workspace::clean_from)
-	WS_SEEN = 28,
-	WS_VISIT_A = 29,
-	WS_VISIT_B = 30,
-	WS_ROW_LANE = 3,
-	WS_STATUS = 4,
-	WS_LEVEL = 5,
-	// 6..12 are used by pgq_api.cu for the staged inputs / outputs
-	WS_ITEMS_A = 13,
-	WS_ITEMS_B = 14,
-	WS_TLIST = 15,
-	WS_TBITS = 16,
-	WS_WALK = 17,
-	WS_ELEMS = 18,
-	WS_SLOT_OFF = 19,
-	WS_PSRC = 20,
-	WS_PDST = 21,
-	WS_SATBITS = 22,
-	WS_SHARED_ROWS = 23,
-	WS_LANE_SRC = 24,
-	WS_ASSIGN_TMP = 25,
-	WS_BATCH_ROWS = 26,
-	WS_PATH_TOTAL = 27,
-	// iterativelengthbidirectional: the destination side's mask set and item lists, its lane -> seed vertex map, and
-	// the meet test's accumulator (slots no other consumer uses: a call of it leaves the search slots 28-30 dirty
-	// outside the known-zero rows, and says so through Workspace::clean_from)
-	WS_SEEN_D = 32,
-	WS_VISIT_A_D = 33,
-	WS_VISIT_B_D = 34,
-	WS_LANE_DST = 35,
-	WS_ITEMS_A_D = 36,
-	WS_ITEMS_B_D = 37,
-	WS_MEET = 38,
-};
-
 // Everything the batches of one call share (read-only once k_assign has run)
 struct CallCtx {
 	int64_t p = 0;
@@ -2213,14 +2176,14 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 	// second workspace is only taken if the context's workspace budget allows it.
 	int n_streams = getenv("PGQ_B200_BATCH_STREAMS") ? atoi(getenv("PGQ_B200_BATCH_STREAMS")) : 2;
 	n_streams = std::max(1, std::min<int>(n_streams, (int)batches.size()));
-	std::vector<Workspace *> extra_ws;
+	std::deque<WsGuard> extra_ws;
 	if (!PATH) {
 		for (int t = 1; t < n_streams; t++) {
-			Workspace *w2 = nullptr;
-			if (pgq_ws_try_acquire(csr->ctx, &w2) != PGQ_OK) {
+			extra_ws.emplace_back(csr->ctx);
+			if (pgq_ws_try_acquire(csr->ctx, &extra_ws.back().ws) != PGQ_OK) {
+				extra_ws.pop_back();
 				break;
 			}
-			extra_ws.push_back(w2);
 		}
 	}
 	n_streams = PATH ? 1 : 1 + (int)extra_ws.size();
@@ -2236,9 +2199,6 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 		}
 		if (ce != cudaSuccess) {
 			cudaGetLastError();
-			for (auto w2 : extra_ws) {
-				pgq_ws_release(csr->ctx, w2);
-			}
 			return pgq_fail(PGQ_ERR_CUDA, "event setup failed: %s", cudaGetErrorString(ce));
 		}
 		std::vector<Run> runs((size_t)n_streams);
@@ -2246,7 +2206,7 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 		std::vector<std::string> errs((size_t)n_streams);
 		std::vector<std::thread> threads;
 		for (int t = 1; t < n_streams; t++) { // worker t takes batches t, t + n_streams, ...
-			Workspace *w2 = extra_ws[(size_t)t - 1];
+			Workspace *w2 = extra_ws[(size_t)t - 1].ws;
 			Run &rr = runs[(size_t)t];
 			rr.csr = csr;
 			rr.ws = w2;
@@ -2285,6 +2245,9 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 		for (auto &th : threads) {
 			th.join();
 		}
+		for (WsGuard &g : extra_ws) {
+			g.settled = true; // (its worker has waited for its stream)
+		}
 		for (int t = 1; t < n_streams; t++) {
 			Run &rw = runs[(size_t)t];
 			// fold the worker's counters and expansion times into the call's
@@ -2310,11 +2273,11 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 			r.st.pull_levels += rw.st.pull_levels;
 			r.st.kernel_launches += rw.st.kernel_launches;
 			r.st.d2h_bytes += rw.st.d2h_bytes;
-			pgq_ws_release(csr->ctx, rw.ws);
 			if (rc == PGQ_OK && rcs[(size_t)t] != PGQ_OK) {
 				rc = pgq_fail(rcs[(size_t)t], "%s", errs[(size_t)t].c_str());
 			}
 		}
+		extra_ws.clear(); // (back to the pool)
 	}
 	if (rc != PGQ_OK) {
 		return rc;
@@ -2446,7 +2409,7 @@ static int run_bidir_batch(Run &r, const CallCtx &cc, const LaneMap &lm_dst, Lev
 	const size_t mask_bytes = (size_t)std::max<int64_t>(n, 1) * W * sizeof(u64);
 	const size_t items_cap = (size_t)n + (size_t)(m / PGQ_ITEM_EDGES) + 64;
 	const size_t tbits_bytes = ((size_t)n / 32 + 1) * sizeof(uint32_t);
-	static const int slots[2][5] = {{WS_SEEN, WS_VISIT_A, WS_VISIT_B, WS_ITEMS_A, WS_ITEMS_B},
+	static const WsSlot slots[2][5] = {{WS_SEEN, WS_VISIT_A, WS_VISIT_B, WS_ITEMS_A, WS_ITEMS_B},
 	                                {WS_SEEN_D, WS_VISIT_A_D, WS_VISIT_B_D, WS_ITEMS_A_D, WS_ITEMS_B_D}};
 	BfsSide<W> side[2];
 	for (int k = 0; k < 2; k++) {

@@ -166,9 +166,9 @@ static int run_bf(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, 
 	int *flags, *h_flags;
 	const size_t dist_elems = (size_t)std::max<int64_t>(n, 1) * L;
 	const size_t dirty_bytes = ((size_t)n / 32 + 1) * sizeof(uint32_t);
-	PGQ_TRY(pgq_ws_reserve(ws, 0, dist_elems * sizeof(u64), (void **)&dist));
-	PGQ_TRY(pgq_ws_reserve(ws, 1, dirty_bytes, (void **)&dirty));
-	PGQ_TRY(pgq_ws_reserve(ws, 2, 256, (void **)&flags)); // [0] changed, [1] range error
+	PGQ_TRY(pgq_ws_reserve(ws, WS_BF_DIST, dist_elems * sizeof(u64), (void **)&dist));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_BF_DIRTY, dirty_bytes, (void **)&dirty));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_BF_FLAGS, 256, (void **)&flags)); // [0] changed, [1] range error
 	PGQ_TRY(pgq_ws_pinned(ws, 256, (void **)&h_flags));
 	PGQ_CUDA(cudaMemsetAsync(flags, 0, 2 * sizeof(int), s));
 	const int sms = csr->ctx->sm_count;
@@ -233,46 +233,32 @@ extern "C" int pgq_cheapest_path_length(pgq_csr *csr, int64_t p, const int64_t *
 		return PGQ_OK;
 	}
 	PGQ_CUDA(cudaSetDevice(csr->ctx->device));
-	Workspace *ws;
-	PGQ_TRY(pgq_ws_acquire(csr->ctx, &ws));
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
-	int rc = PGQ_OK;
-	do {
-		int64_t *d_src, *d_dst, *d_out;
-		uint8_t *d_sv = nullptr, *d_dv = nullptr, *d_ov;
-		const size_t b8 = (size_t)p * sizeof(int64_t);
-		if ((rc = pgq_ws_reserve(ws, 6, b8, (void **)&d_src)) != PGQ_OK) break;
-		if ((rc = pgq_ws_reserve(ws, 7, b8, (void **)&d_dst)) != PGQ_OK) break;
-		if ((rc = pgq_ws_reserve(ws, 9, b8, (void **)&d_out)) != PGQ_OK) break;
-		if ((rc = pgq_ws_reserve(ws, 10, (size_t)p, (void **)&d_ov)) != PGQ_OK) break;
-		cudaMemcpyAsync(d_src, src, b8, cudaMemcpyHostToDevice, s);
-		cudaMemcpyAsync(d_dst, dst, b8, cudaMemcpyHostToDevice, s);
-		st.h2d_bytes = 2 * (int64_t)b8;
-		if (src_valid) {
-			if ((rc = pgq_ws_reserve(ws, 8, (size_t)p, (void **)&d_sv)) != PGQ_OK) break;
-			cudaMemcpyAsync(d_sv, src_valid, (size_t)p, cudaMemcpyHostToDevice, s);
-			st.h2d_bytes += p;
-		}
-		if (dst_valid) {
-			if ((rc = pgq_ws_reserve(ws, 11, (size_t)p, (void **)&d_dv)) != PGQ_OK) break;
-			cudaMemcpyAsync(d_dv, dst_valid, (size_t)p, cudaMemcpyHostToDevice, s);
-			st.h2d_bytes += p;
-		}
-		rc = (csr->weight_type == 2) ? run_bf<true>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_out, d_ov, &st)
-		                             : run_bf<false>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_out, d_ov, &st);
-		if (rc != PGQ_OK) break;
-		cudaMemcpyAsync(out_cost, d_out, b8, cudaMemcpyDeviceToHost, s);
-		cudaMemcpyAsync(out_valid, d_ov, (size_t)p, cudaMemcpyDeviceToHost, s);
-		st.d2h_bytes = (int64_t)b8 + p;
-	} while (0);
-	cudaError_t e = cudaStreamSynchronize(s); // (also on the error paths: nothing may outlive the call)
-	if (rc == PGQ_OK && (e != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess)) {
-		rc = pgq_fail(PGQ_ERR_CUDA, "cheapest_path_length failed: %s", cudaGetErrorString(e));
+	int64_t *d_src, *d_dst, *d_out;
+	uint8_t *d_sv, *d_dv, *d_ov;
+	const size_t b8 = (size_t)p * sizeof(int64_t);
+	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
+	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d_dst));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LEN, b8, (void **)&d_out));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_ov));
+	PGQ_TRY(stage_column(ws, WS_IN_VALID, src_valid, (size_t)p, (const void **)&d_sv));
+	PGQ_TRY(stage_column(ws, WS_IN_DST_VALID, dst_valid, (size_t)p, (const void **)&d_dv));
+	st.h2d_bytes = 2 * (int64_t)b8 + (src_valid ? p : 0) + (dst_valid ? p : 0);
+	PGQ_TRY((csr->weight_type == 2) ? run_bf<true>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_out, d_ov, &st)
+	                                : run_bf<false>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_out, d_ov, &st));
+	cudaMemcpyAsync(out_cost, d_out, b8, cudaMemcpyDeviceToHost, s);
+	cudaMemcpyAsync(out_valid, d_ov, (size_t)p, cudaMemcpyDeviceToHost, s);
+	st.d2h_bytes = (int64_t)b8 + p;
+	cudaError_t e = cudaStreamSynchronize(s);
+	if (e != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess) {
+		return pgq_fail(PGQ_ERR_CUDA, "cheapest_path_length failed: %s", cudaGetErrorString(e));
 	}
-	cudaGetLastError();
-	pgq_ws_release(csr->ctx, ws);
-	if (rc == PGQ_OK && stats) {
+	g.settled = true;
+	if (stats) {
 		*stats = st;
 	}
-	return rc;
+	return PGQ_OK;
 }

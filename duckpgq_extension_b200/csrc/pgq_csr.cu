@@ -122,7 +122,7 @@ extern "C" int pgq_ctx_create(int device, pgq_ctx **out) {
 }
 
 static void ws_destroy(Workspace *ws) {
-	for (int i = 0; i < PGQ_WS_SLOTS; i++) {
+	for (int i = 0; i < WS_SLOTS; i++) {
 		if (ws->buf[i]) {
 			cudaFree(ws->buf[i]);
 		}
@@ -215,7 +215,7 @@ static void ctx_release_idle(pgq_ctx *ctx) {
 	{
 		std::lock_guard<std::mutex> g(ctx->mu);
 		for (Workspace *w : ctx->free_ws) {
-			for (int i = 0; i < PGQ_WS_SLOTS; i++) {
+			for (int i = 0; i < WS_SLOTS; i++) {
 				if (w->buf[i]) {
 					drop.push_back(w->buf[i]);
 				}
@@ -264,7 +264,7 @@ void pgq_ws_release(pgq_ctx *ctx, Workspace *ws) {
 
 // pgq_ws_reserve that keeps the first keep_bytes of the slot's content when it has to grow
 // (synchronises the stream in that case).
-int pgq_ws_grow(Workspace *ws, int slot, size_t bytes, size_t keep_bytes, cudaStream_t s, void **out) {
+int pgq_ws_grow(Workspace *ws, WsSlot slot, size_t bytes, size_t keep_bytes, cudaStream_t s, void **out) {
 	if (bytes == 0) {
 		bytes = 256;
 	}
@@ -297,7 +297,7 @@ int pgq_ws_grow(Workspace *ws, int slot, size_t bytes, size_t keep_bytes, cudaSt
 	return PGQ_OK;
 }
 
-int pgq_ws_reserve(Workspace *ws, int slot, size_t bytes, void **out) {
+int pgq_ws_reserve(Workspace *ws, WsSlot slot, size_t bytes, void **out) {
 	if (bytes == 0) {
 		bytes = 256;
 	}
@@ -321,6 +321,20 @@ int pgq_ws_reserve(Workspace *ws, int slot, size_t bytes, void **out) {
 		ws->cap[slot] = want;
 	}
 	*out = ws->buf[slot];
+	return PGQ_OK;
+}
+
+int stage_column(Workspace *ws, WsSlot slot, const void *host, size_t bytes, const void **dev) {
+	*dev = nullptr;
+	if (!host) {
+		return PGQ_OK;
+	}
+	void *d;
+	PGQ_TRY(pgq_ws_reserve(ws, slot, bytes, &d));
+	if (bytes > 0) {
+		PGQ_CUDA(cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, ws->stream));
+	}
+	*dev = d;
 	return PGQ_OK;
 }
 
@@ -547,8 +561,8 @@ static int radix_sort_pairs_impl(Workspace *ws, K *keys_a, K *keys_b, int32_t *v
 	const int nblocks = (int)((count + RS_TILE - 1) / RS_TILE);
 	const int64_t hist_elems = (int64_t)RS_BINS * nblocks;
 	int32_t *hist, *scan_tmp;
-	PGQ_TRY(pgq_ws_reserve(ws, 14, (size_t)(hist_elems + 1) * sizeof(int32_t), (void **)&hist));
-	PGQ_TRY(pgq_ws_reserve(ws, 15, pgq_scan_tmp_elems(hist_elems) * sizeof(int32_t), (void **)&scan_tmp));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_RADIX_HIST, (size_t)(hist_elems + 1) * sizeof(int32_t), (void **)&hist));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_RADIX_SCAN, pgq_scan_tmp_elems(hist_elems) * sizeof(int32_t), (void **)&scan_tmp));
 	K *kin = keys_a, *kout = keys_b;
 	int32_t *vin = vals_a, *vout = vals_b;
 	for (int shift = 0; shift < end_bit; shift += RS_BITS) {
@@ -1052,8 +1066,8 @@ static int build_dir_metadata(pgq_csr *csr, DirGraph &g, Workspace *ws, cudaStre
 	PGQ_CUDA(cudaMemsetAsync(g.head, 0, head_words * sizeof(uint32_t), s));
 	PGQ_CUDA(cudaMemsetAsync(g.chunk_rank, 0, (size_t)std::max<int64_t>(g.nchunks, 1) * sizeof(int32_t), s));
 	int32_t *nzflag, *scan_tmp;
-	PGQ_TRY(pgq_ws_reserve(ws, 0, (size_t)(n + 1) * sizeof(int32_t), (void **)&nzflag));
-	PGQ_TRY(pgq_ws_reserve(ws, 1, pgq_scan_tmp_elems(n + 1) * sizeof(int32_t), (void **)&scan_tmp));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_A, (size_t)(n + 1) * sizeof(int32_t), (void **)&nzflag));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_SCAN, pgq_scan_tmp_elems(n + 1) * sizeof(int32_t), (void **)&scan_tmp));
 	PGQ_CUDA(cudaMemsetAsync(nzflag, 0, (size_t)(n + 1) * sizeof(int32_t), s));
 	if (n > 0) {
 		k_mark_heads<<<grid_for(n, 256), 256, 0, s>>>(g.off, n, g.head, nzflag);
@@ -1080,10 +1094,10 @@ static int build_pull_graph(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	g = PullGraph();
 	int32_t *long_deg, *long_flag, *short_flag, *scan_tmp;
 	const size_t row_bytes = (size_t)(n_rows + 2) * sizeof(int32_t);
-	PGQ_TRY(pgq_ws_reserve(ws, 0, row_bytes, (void **)&long_deg));
-	PGQ_TRY(pgq_ws_reserve(ws, 9, row_bytes, (void **)&long_flag));
-	PGQ_TRY(pgq_ws_reserve(ws, 10, row_bytes, (void **)&short_flag));
-	PGQ_TRY(pgq_ws_reserve(ws, 1, pgq_scan_tmp_elems(std::max<int64_t>(n_rows, m / 32) + 2) * sizeof(int32_t), (void **)&scan_tmp));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_A, row_bytes, (void **)&long_deg));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_B, row_bytes, (void **)&long_flag));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_C, row_bytes, (void **)&short_flag));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_SCAN, pgq_scan_tmp_elems(std::max<int64_t>(n_rows, m / 32) + 2) * sizeof(int32_t), (void **)&scan_tmp));
 	k_pull_classify<<<grid_for(n_rows + 1, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->in.off, n_rows, long_deg, long_flag, short_flag);
 	PGQ_CUDA(cudaGetLastError());
 	PGQ_TRY(pgq_scan_exclusive_i32(long_deg, long_deg, n_rows + 1, scan_tmp, s));
@@ -1112,7 +1126,7 @@ static int build_pull_graph(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	PGQ_CUDA(cudaMemsetAsync(g.chunk_rank, 0, (size_t)std::max<int64_t>(g.nchunks, 1) * sizeof(int32_t), s));
 	if (g.n_rows > 0) {
 		int32_t *off_by_rank;
-		PGQ_TRY(pgq_ws_reserve(ws, 11, (size_t)(g.n_rows + 2) * sizeof(int32_t), (void **)&off_by_rank));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_D, (size_t)(g.n_rows + 2) * sizeof(int32_t), (void **)&off_by_rank));
 		k_pull_long_fill<<<grid_for(n_rows * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->in.off, csr->in.adj, n_rows, long_deg,
 		                                                                long_flag, g.adj, g.row, off_by_rank);
 		const int32_t m_long = (int32_t)g.m;
@@ -1127,10 +1141,10 @@ static int build_pull_graph(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	if (g.n_short > 0) {
 		int32_t *key_a, *key_b, *val_a, *val_b, *key_res, *val_res;
 		const size_t kv = (size_t)(g.n_slices * 32 + 32) * sizeof(int32_t);
-		PGQ_TRY(pgq_ws_reserve(ws, 5, std::max(kv, ws->cap[5]), (void **)&key_a));
-		PGQ_TRY(pgq_ws_reserve(ws, 6, std::max(kv, ws->cap[6]), (void **)&key_b));
-		PGQ_TRY(pgq_ws_reserve(ws, 7, std::max(kv, ws->cap[7]), (void **)&val_a));
-		PGQ_TRY(pgq_ws_reserve(ws, 12, kv, (void **)&val_b));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_A, std::max(kv, ws->cap[WS_CSR_EDGE_A]), (void **)&key_a));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_B, std::max(kv, ws->cap[WS_CSR_EDGE_B]), (void **)&key_b));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_C, std::max(kv, ws->cap[WS_CSR_EDGE_C]), (void **)&val_a));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_E, kv, (void **)&val_b));
 		k_pull_short_list<<<grid_for(n_rows, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->in.off, n_rows, short_flag, key_a, val_a);
 		PGQ_CUDA(cudaGetLastError());
 		PGQ_TRY(radix_sort_pairs(ws, key_a, key_b, val_a, val_b, g.n_short, 5, s, &key_res, &val_res));
@@ -1156,7 +1170,7 @@ static int build_pull_graph(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 static int finish_csr(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	int64_t n = csr->n, m = csr->m;
 	int *d_err;
-	PGQ_TRY(pgq_ws_reserve(ws, 2, 256, (void **)&d_err));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_ERR, 256, (void **)&d_err));
 	PGQ_CUDA(cudaMemsetAsync(d_err, 0, sizeof(int), s));
 	k_check_offsets<<<grid_for(n + 1, 256), 256, 0, s>>>(csr->out.off, n, m, d_err);
 	PGQ_CUDA(cudaGetLastError());
@@ -1173,7 +1187,7 @@ static int finish_csr(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	PGQ_TRY(dev_alloc(csr, (void **)&csr->in.off, (size_t)(n + 1) * sizeof(int32_t)));
 	PGQ_TRY(dev_alloc(csr, (void **)&csr->in.adj, (size_t)std::max<int64_t>(m, 1) * sizeof(int32_t)));
 	int32_t *scan_tmp;
-	PGQ_TRY(pgq_ws_reserve(ws, 1, pgq_scan_tmp_elems(n + 1) * sizeof(int32_t), (void **)&scan_tmp));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_SCAN, pgq_scan_tmp_elems(n + 1) * sizeof(int32_t), (void **)&scan_tmp));
 	PGQ_CUDA(cudaMemsetAsync(csr->in.off, 0, (size_t)(n + 1) * sizeof(int32_t), s));
 	if (m > 0) {
 		k_histogram<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->out.adj, m, csr->in.off);
@@ -1182,8 +1196,8 @@ static int finish_csr(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	PGQ_TRY(pgq_scan_exclusive_i32(csr->in.off, csr->in.off, n + 1, scan_tmp, s));
 	if (m > 0) {
 		int32_t *rowid, *keys_out;
-		PGQ_TRY(pgq_ws_reserve(ws, 5, (size_t)m * sizeof(int32_t), (void **)&keys_out));
-		PGQ_TRY(pgq_ws_reserve(ws, 6, (size_t)m * sizeof(int32_t), (void **)&rowid));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_A, (size_t)m * sizeof(int32_t), (void **)&keys_out));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_B, (size_t)m * sizeof(int32_t), (void **)&rowid));
 		int end_bit = 1;
 		while (end_bit < 31 && ((int64_t)1 << end_bit) < n) {
 			end_bit++;
@@ -1191,7 +1205,7 @@ static int finish_csr(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 		k_edge_rows<<<grid_for(csr->out.nchunks * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->out, m, rowid);
 		PGQ_CUDA(cudaGetLastError());
 		int32_t *keys_a, *keys_res, *vals_res;
-		PGQ_TRY(pgq_ws_reserve(ws, 7, (size_t)m * sizeof(int32_t), (void **)&keys_a));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_C, (size_t)m * sizeof(int32_t), (void **)&keys_a));
 		PGQ_CUDA(cudaMemcpyAsync(keys_a, csr->out.adj, (size_t)m * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
 		PGQ_TRY(radix_sort_pairs(ws, keys_a, keys_out, rowid, csr->in.adj, m, end_bit, s, &keys_res, &vals_res));
 		if (vals_res != csr->in.adj) {
@@ -1256,7 +1270,7 @@ static int upload_narrow(Workspace *ws, const int64_t *host, int64_t count, int6
                          int *d_err, cudaStream_t s) {
 	const int64_t piece = (int64_t)1 << 24;
 	int64_t *tmp;
-	PGQ_TRY(pgq_ws_reserve(ws, 4, (size_t)std::min(piece, std::max<int64_t>(count, 1)) * sizeof(int64_t), (void **)&tmp));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_WIDE, (size_t)std::min(piece, std::max<int64_t>(count, 1)) * sizeof(int64_t), (void **)&tmp));
 	for (int64_t o = 0; o < count; o += piece) {
 		int64_t c = std::min(piece, count - o);
 		PGQ_CUDA(cudaMemcpyAsync(tmp, host + o, (size_t)c * sizeof(int64_t), cudaMemcpyHostToDevice, s));
@@ -1521,11 +1535,11 @@ static int finalize_from_rows(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	const int64_t n = csr->n, m = csr->m;
 	int *d_err;
 	int32_t *scan_tmp, *outdeg, *indeg, *flag;
-	PGQ_TRY(pgq_ws_reserve(ws, 2, 256, (void **)&d_err));
-	PGQ_TRY(pgq_ws_reserve(ws, 1, pgq_scan_tmp_elems(n + 1) * sizeof(int32_t), (void **)&scan_tmp));
-	PGQ_TRY(pgq_ws_reserve(ws, 9, (size_t)(n + 1) * sizeof(int32_t), (void **)&outdeg));
-	PGQ_TRY(pgq_ws_reserve(ws, 10, (size_t)(n + 1) * sizeof(int32_t), (void **)&indeg));
-	PGQ_TRY(pgq_ws_reserve(ws, 0, (size_t)(n + 1) * sizeof(int32_t), (void **)&flag));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_ERR, 256, (void **)&d_err));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_SCAN, pgq_scan_tmp_elems(n + 1) * sizeof(int32_t), (void **)&scan_tmp));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_B, (size_t)(n + 1) * sizeof(int32_t), (void **)&outdeg));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_C, (size_t)(n + 1) * sizeof(int32_t), (void **)&indeg));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_A, (size_t)(n + 1) * sizeof(int32_t), (void **)&flag));
 	PGQ_TRY(dev_alloc(csr, (void **)&csr->out.off, (size_t)(n + 1) * sizeof(int32_t)));
 	PGQ_TRY(dev_alloc(csr, (void **)&csr->out.adj, (size_t)std::max<int64_t>(m, 1) * sizeof(int32_t)));
 	PGQ_TRY(dev_alloc(csr, (void **)&csr->edge_ids, (size_t)std::max<int64_t>(m, 1) * sizeof(int64_t)));
@@ -1549,11 +1563,11 @@ static int finalize_from_rows(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 		int32_t *key_a, *key_b, *val_a, *val_b, *key_res, *val_res;
 		int *d_cls;
 		const size_t kv_bytes = (size_t)std::max<int64_t>(std::max<int64_t>(n, m), 1) * sizeof(int32_t);
-		PGQ_TRY(pgq_ws_reserve(ws, 5, kv_bytes, (void **)&key_a));
-		PGQ_TRY(pgq_ws_reserve(ws, 6, kv_bytes, (void **)&key_b));
-		PGQ_TRY(pgq_ws_reserve(ws, 7, kv_bytes, (void **)&val_a));
-		PGQ_TRY(pgq_ws_reserve(ws, 11, (size_t)(n + 2) * sizeof(int32_t), (void **)&val_b));
-		PGQ_TRY(pgq_ws_reserve(ws, 3, 256, (void **)&d_cls));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_A, kv_bytes, (void **)&key_a));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_B, kv_bytes, (void **)&key_b));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_C, kv_bytes, (void **)&val_a));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_D, (size_t)(n + 2) * sizeof(int32_t), (void **)&val_b));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_FLAGS, 256, (void **)&d_cls));
 		PGQ_CUDA(cudaMemsetAsync(d_cls, 0, 4 * sizeof(int), s));
 		k_vertex_keys<<<grid_for(n, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(outdeg, indeg, n, key_a, val_a, d_cls);
 		PGQ_CUDA(cudaGetLastError());
@@ -1585,9 +1599,9 @@ static int finalize_from_rows(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 	PGQ_TRY(pgq_scan_exclusive_i32(csr->out.off, csr->out.off, n + 1, scan_tmp, s));
 	if (m > 0) {
 		int32_t *keys_out, *perm_in, *perm_out, *keys_res;
-		PGQ_TRY(pgq_ws_reserve(ws, 5, (size_t)m * sizeof(int32_t), (void **)&keys_out));
-		PGQ_TRY(pgq_ws_reserve(ws, 6, (size_t)m * sizeof(int32_t), (void **)&perm_in));
-		PGQ_TRY(pgq_ws_reserve(ws, 7, (size_t)m * sizeof(int32_t), (void **)&perm_out));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_A, (size_t)m * sizeof(int32_t), (void **)&keys_out));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_B, (size_t)m * sizeof(int32_t), (void **)&perm_in));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_C, (size_t)m * sizeof(int32_t), (void **)&perm_out));
 		int end_bit = 1;
 		while (end_bit < 31 && ((int64_t)1 << end_bit) < n) {
 			end_bit++;
@@ -1604,7 +1618,7 @@ static int finalize_from_rows(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 		PGQ_CUDA(cudaGetLastError());
 		if (csr->w_bits) {
 			int *d_neg, neg = 0;
-			PGQ_TRY(pgq_ws_reserve(ws, 3, 256, (void **)&d_neg));
+			PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_FLAGS, 256, (void **)&d_neg));
 			PGQ_CUDA(cudaMemsetAsync(d_neg, 0, sizeof(int), s));
 			k_any_negative_weight<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->w_bits, m,
 			                                                                                     csr->weight_type == 2, d_neg);
@@ -1645,14 +1659,34 @@ extern "C" int pgq_csr_finalize(pgq_csr *csr) {
 			                (long long)csr->n);
 		}
 	}
-	Workspace *ws;
-	PGQ_TRY(pgq_ws_acquire(csr->ctx, &ws));
-	int st = finalize_from_rows(csr, ws, ws->stream);
-	pgq_ws_release(csr->ctx, ws);
-	if (st == PGQ_OK) {
-		free_staging(csr);
+	{
+		WsGuard g(csr->ctx);
+		PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+		PGQ_TRY(finalize_from_rows(csr, g.ws, g.ws->stream));
+		g.settled = true;
 	}
-	return st;
+	free_staging(csr);
+	return PGQ_OK;
+}
+
+// The edge rows of pgq_csr_build into the staging columns (ids narrowed and range-checked).
+static int upload_rows(pgq_csr *csr, const int64_t *src, const int64_t *dst, const int64_t *eid) {
+	const int64_t n = csr->n, m = csr->m;
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	cudaStream_t s = g.ws->stream;
+	PGQ_TRY(upload_narrow(g.ws, src, m, 0, n, csr->st_src, csr->d_err, s));
+	PGQ_TRY(upload_narrow(g.ws, dst, m, 0, n, csr->st_dst, csr->d_err, s));
+	cudaError_t e = cudaMemcpyAsync(csr->st_eid, eid, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, s);
+	if (e == cudaSuccess) {
+		e = cudaStreamSynchronize(s);
+	}
+	if (e != cudaSuccess) {
+		cudaGetLastError();
+		return pgq_fail(PGQ_ERR_CUDA, "edge upload failed: %s", cudaGetErrorString(e));
+	}
+	g.settled = true;
+	return PGQ_OK;
 }
 
 extern "C" int pgq_csr_build(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *src, const int64_t *dst,
@@ -1686,24 +1720,7 @@ extern "C" int pgq_csr_build(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *
 		csr->edge_init = true;
 	}
 	if (st == PGQ_OK && m > 0) {
-		Workspace *ws = nullptr;
-		st = pgq_ws_acquire(ctx, &ws);
-		if (st == PGQ_OK) {
-			cudaStream_t s = ws->stream;
-			st = upload_narrow(ws, src, m, 0, n, csr->st_src, csr->d_err, s);
-			if (st == PGQ_OK) st = upload_narrow(ws, dst, m, 0, n, csr->st_dst, csr->d_err, s);
-			if (st == PGQ_OK) {
-				cudaError_t e = cudaMemcpyAsync(csr->st_eid, eid, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, s);
-				if (e == cudaSuccess) {
-					e = cudaStreamSynchronize(s);
-				}
-				if (e != cudaSuccess) {
-					cudaGetLastError();
-					st = pgq_fail(PGQ_ERR_CUDA, "edge upload failed: %s", cudaGetErrorString(e));
-				}
-			}
-			pgq_ws_release(ctx, ws);
-		}
+		st = upload_rows(csr, src, dst, eid);
 	}
 	if (st == PGQ_OK) {
 		st = pgq_csr_finalize(csr);
@@ -1724,6 +1741,43 @@ __global__ void k_range_check_i32(const int32_t *__restrict__ ids, int64_t count
 	}
 }
 
+// Copies the device edge columns of pgq_csr_build_device into the staging columns and builds from them.
+static int build_from_device_rows(pgq_csr *csr, const int32_t *d_src, const int32_t *d_dst, const int64_t *d_eid) {
+	const int64_t n = csr->n, m = csr->m;
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	cudaStream_t s = g.ws->stream;
+	int *d_err;
+	const size_t cap = (size_t)std::max<int64_t>(m, 1);
+	PGQ_TRY(pgq_ws_reserve(g.ws, WS_CSR_ERR, 256, (void **)&d_err));
+	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_src, cap * sizeof(int32_t)));
+	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_dst, cap * sizeof(int32_t)));
+	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_eid, cap * sizeof(int64_t)));
+	cudaMemsetAsync(d_err, 0, sizeof(int), s);
+	// the columns may have been produced on any stream of the caller (torch's, cuDF's): the copies below
+	// run on a stream of ours, so wait for the whole device once rather than race the producer
+	cudaDeviceSynchronize();
+	if (m > 0) {
+		cudaMemcpyAsync(csr->st_src, d_src, (size_t)m * sizeof(int32_t), cudaMemcpyDeviceToDevice, s);
+		cudaMemcpyAsync(csr->st_dst, d_dst, (size_t)m * sizeof(int32_t), cudaMemcpyDeviceToDevice, s);
+		k_range_check_i32<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->st_src, m, n, d_err);
+		k_range_check_i32<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->st_dst, m, n, d_err);
+		if (d_eid) {
+			cudaMemcpyAsync(csr->st_eid, d_eid, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToDevice, s);
+		} else {
+			k_iota64<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->st_eid, m);
+		}
+	}
+	int flag = 0;
+	PGQ_TRY(read_flag(d_err, s, &flag));
+	if (flag) {
+		return pgq_fail(PGQ_ERR_RANGE, "create_csr_edge: vertex rowid outside [0,%lld)", (long long)n);
+	}
+	PGQ_TRY(finalize_from_rows(csr, g.ws, s));
+	g.settled = true;
+	return PGQ_OK;
+}
+
 extern "C" int pgq_csr_build_device(pgq_ctx *ctx, int64_t n, int64_t m, const int32_t *d_src, const int32_t *d_dst,
                                     const int64_t *d_eid, pgq_csr **out) {
 	if (!ctx || !out || (m > 0 && (!d_src || !d_dst))) {
@@ -1742,44 +1796,7 @@ extern "C" int pgq_csr_build_device(pgq_ctx *ctx, int64_t n, int64_t m, const in
 	csr->edge_size = m;
 	csr->staged = m;
 	csr->edge_init = true;
-	Workspace *ws = nullptr;
-	int st = pgq_ws_acquire(ctx, &ws);
-	if (st != PGQ_OK) {
-		delete csr;
-		return st;
-	}
-	cudaStream_t s = ws->stream;
-	do {
-		int *d_err;
-		const size_t cap = (size_t)std::max<int64_t>(m, 1);
-		if ((st = pgq_ws_reserve(ws, 2, 256, (void **)&d_err)) != PGQ_OK) break;
-		if ((st = dev_alloc(csr, (void **)&csr->st_src, cap * sizeof(int32_t))) != PGQ_OK) break;
-		if ((st = dev_alloc(csr, (void **)&csr->st_dst, cap * sizeof(int32_t))) != PGQ_OK) break;
-		if ((st = dev_alloc(csr, (void **)&csr->st_eid, cap * sizeof(int64_t))) != PGQ_OK) break;
-		cudaMemsetAsync(d_err, 0, sizeof(int), s);
-		// the columns may have been produced on any stream of the caller (torch's, cuDF's): the copies below
-		// run on a stream of ours, so wait for the whole device once rather than race the producer
-		cudaDeviceSynchronize();
-		if (m > 0) {
-			cudaMemcpyAsync(csr->st_src, d_src, (size_t)m * sizeof(int32_t), cudaMemcpyDeviceToDevice, s);
-			cudaMemcpyAsync(csr->st_dst, d_dst, (size_t)m * sizeof(int32_t), cudaMemcpyDeviceToDevice, s);
-			k_range_check_i32<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->st_src, m, n, d_err);
-			k_range_check_i32<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->st_dst, m, n, d_err);
-			if (d_eid) {
-				cudaMemcpyAsync(csr->st_eid, d_eid, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToDevice, s);
-			} else {
-				k_iota64<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->st_eid, m);
-			}
-		}
-		int flag = 0;
-		if ((st = read_flag(d_err, s, &flag)) != PGQ_OK) break;
-		if (flag) {
-			st = pgq_fail(PGQ_ERR_RANGE, "create_csr_edge: vertex rowid outside [0,%lld)", (long long)n);
-			break;
-		}
-		st = finalize_from_rows(csr, ws, s);
-	} while (0);
-	pgq_ws_release(ctx, ws);
+	const int st = build_from_device_rows(csr, d_src, d_dst, d_eid);
 	if (st != PGQ_OK) {
 		pgq_csr_free(csr);
 		return st;
@@ -1929,8 +1946,8 @@ __global__ void k_key_expand(const int32_t *__restrict__ off, const int32_t *__r
 	}
 }
 
-// The vertex table's (key, rowid) pairs sorted by key: the nv = (*pos)[n] non-NULL ones first (slots 16-21; the scan
-// scratch in slot 17 has room for max(n, m) + 1 elements).
+// The vertex table's (key, rowid) pairs sorted by key: the nv = (*pos)[n] non-NULL ones first (the scan scratch in
+// WS_KEY_SCAN has room for max(n, m) + 1 elements).
 static int sort_vertex_keys(pgq_csr *csr, Workspace *ws, cudaStream_t s, const int64_t *vkey, const uint8_t *vvalid,
                             int64_t m, int32_t **pos_out, int32_t **scan_tmp_out, uint64_t **sorted_key,
                             int32_t **sorted_row) {
@@ -1939,12 +1956,12 @@ static int sort_vertex_keys(pgq_csr *csr, Workspace *ws, cudaStream_t s, const i
 	int32_t *pos, *scan_tmp, *row_a, *row_b;
 	uint64_t *key_a, *key_b;
 	const size_t vb = (size_t)std::max<int64_t>(n, 1);
-	PGQ_TRY(pgq_ws_reserve(ws, 16, (size_t)(n + 1) * sizeof(int32_t), (void **)&pos));
-	PGQ_TRY(pgq_ws_reserve(ws, 17, pgq_scan_tmp_elems(std::max<int64_t>(n, m) + 1) * sizeof(int32_t), (void **)&scan_tmp));
-	PGQ_TRY(pgq_ws_reserve(ws, 18, vb * sizeof(uint64_t), (void **)&key_a));
-	PGQ_TRY(pgq_ws_reserve(ws, 19, vb * sizeof(uint64_t), (void **)&key_b));
-	PGQ_TRY(pgq_ws_reserve(ws, 20, vb * sizeof(int32_t), (void **)&row_a));
-	PGQ_TRY(pgq_ws_reserve(ws, 21, vb * sizeof(int32_t), (void **)&row_b));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_POS, (size_t)(n + 1) * sizeof(int32_t), (void **)&pos));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_SCAN, pgq_scan_tmp_elems(std::max<int64_t>(n, m) + 1) * sizeof(int32_t), (void **)&scan_tmp));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_SORT_A, vb * sizeof(uint64_t), (void **)&key_a));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_SORT_B, vb * sizeof(uint64_t), (void **)&key_b));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_ROW_A, vb * sizeof(int32_t), (void **)&row_a));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_ROW_B, vb * sizeof(int32_t), (void **)&row_b));
 	*sorted_key = nullptr;
 	*sorted_row = nullptr;
 	k_key_valid<<<grid_n, 256, 0, s>>>(vvalid, n, pos);
@@ -1970,10 +1987,10 @@ static int build_from_keys(pgq_csr *csr, Workspace *ws, cudaStream_t s, const in
 	uint64_t *sorted_key;
 	unsigned long long *d_status;
 	const size_t eb = (size_t)(m + 1);
-	PGQ_TRY(pgq_ws_reserve(ws, 2, 256, (void **)&d_status));
-	PGQ_TRY(pgq_ws_reserve(ws, 22, eb * sizeof(int32_t), (void **)&ms));
-	PGQ_TRY(pgq_ws_reserve(ws, 23, eb * sizeof(int32_t), (void **)&src_lo));
-	PGQ_TRY(pgq_ws_reserve(ws, 24, eb * sizeof(int32_t), (void **)&dst_row));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_STATUS, 256, (void **)&d_status));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_EDGE_A, eb * sizeof(int32_t), (void **)&ms));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_EDGE_B, eb * sizeof(int32_t), (void **)&src_lo));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_EDGE_C, eb * sizeof(int32_t), (void **)&dst_row));
 	PGQ_CUDA(cudaMemsetAsync(d_status, 0, 3 * sizeof(unsigned long long), s));
 	PGQ_TRY(sort_vertex_keys(csr, ws, s, vkey, vvalid, m, &pos, &scan_tmp, &sorted_key, &sorted_row));
 	if (m > 0) {
@@ -2224,9 +2241,8 @@ __global__ void __launch_bounds__(256) k_ukey_check(const uint64_t *__restrict__
 	}
 }
 
-// The undirected CSR CTE on device columns, then the common build.  Sets csr->m.  Workspace slots: 2 the status
-// block, 16-21 the vertex sort, 22-24 and 46-47 per edge, 48-52 the row sort (and before it the half-edge sort),
-// 53-58 per vertex and per half edge.
+// The undirected CSR CTE on device columns, then the common build.  Sets csr->m.  The WS_UKEY_SORT_* / IDX_* / AUX
+// slots hold the row sort, and before it the half-edge sort.
 static int build_from_keys_undirected(pgq_csr *csr, Workspace *ws, cudaStream_t s, const int64_t *vkey,
                                       const uint8_t *vvalid, const int64_t *skey, const int64_t *dkey,
                                       const uint8_t *svalid, const uint8_t *dvalid, int64_t m) {
@@ -2238,16 +2254,16 @@ static int build_from_keys_undirected(pgq_csr *csr, Workspace *ws, cudaStream_t 
 	unsigned long long *d_status;
 	const size_t vb = (size_t)std::max<int64_t>(n, 1) * sizeof(int32_t);
 	const size_t eb = (size_t)(m + 1) * sizeof(int32_t);
-	PGQ_TRY(pgq_ws_reserve(ws, 2, 256, (void **)&d_status));
-	PGQ_TRY(pgq_ws_reserve(ws, 22, eb, (void **)&rows));
-	PGQ_TRY(pgq_ws_reserve(ws, 23, eb, (void **)&slo));
-	PGQ_TRY(pgq_ws_reserve(ws, 24, eb, (void **)&dlo));
-	PGQ_TRY(pgq_ws_reserve(ws, 46, eb, (void **)&ms));
-	PGQ_TRY(pgq_ws_reserve(ws, 47, eb, (void **)&md));
-	PGQ_TRY(pgq_ws_reserve(ws, 53, vb, (void **)&r_row));
-	PGQ_TRY(pgq_ws_reserve(ws, 54, vb, (void **)&m_row));
-	PGQ_TRY(pgq_ws_reserve(ws, 55, vb, (void **)&dcnt));
-	PGQ_TRY(pgq_ws_reserve(ws, 56, vb, (void **)&null_mult));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_STATUS, 256, (void **)&d_status));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_EDGE_A, eb, (void **)&rows));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_EDGE_B, eb, (void **)&slo));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_EDGE_C, eb, (void **)&dlo));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_MS, eb, (void **)&ms));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_MD, eb, (void **)&md));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_R_ROW, vb, (void **)&r_row));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_M_ROW, vb, (void **)&m_row));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_DCNT, vb, (void **)&dcnt));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_NULL_MULT, vb, (void **)&null_mult));
 	PGQ_CUDA(cudaMemsetAsync(d_status, 0, 6 * sizeof(unsigned long long), s));
 	PGQ_CUDA(cudaMemsetAsync(r_row, 0, vb, s));
 	PGQ_CUDA(cudaMemsetAsync(m_row, 0, vb, s));
@@ -2277,13 +2293,13 @@ static int build_from_keys_undirected(pgq_csr *csr, Workspace *ws, cudaStream_t 
 		int32_t *h_lo, *h_mult, *idx_a, *idx_b, *idx, *lo_a, *lo_b, *at_a, *at_b, *lo_sorted, *at;
 		uint64_t *val_a, *val_b, *val_sorted;
 		const size_t hb = (size_t)h * sizeof(int32_t);
-		PGQ_TRY(pgq_ws_reserve(ws, 57, hb, (void **)&h_lo));
-		PGQ_TRY(pgq_ws_reserve(ws, 58, hb, (void **)&h_mult));
-		PGQ_TRY(pgq_ws_reserve(ws, 48, (size_t)h * sizeof(uint64_t), (void **)&val_a));
-		PGQ_TRY(pgq_ws_reserve(ws, 49, (size_t)h * sizeof(uint64_t), (void **)&val_b));
-		PGQ_TRY(pgq_ws_reserve(ws, 50, hb, (void **)&idx_a));
-		PGQ_TRY(pgq_ws_reserve(ws, 51, hb, (void **)&idx_b));
-		PGQ_TRY(pgq_ws_reserve(ws, 52, 4 * hb, (void **)&lo_a));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_H_LO, hb, (void **)&h_lo));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_H_MULT, hb, (void **)&h_mult));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_SORT_A, (size_t)h * sizeof(uint64_t), (void **)&val_a));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_SORT_B, (size_t)h * sizeof(uint64_t), (void **)&val_b));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_IDX_A, hb, (void **)&idx_a));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_IDX_B, hb, (void **)&idx_b));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_AUX, 4 * hb, (void **)&lo_a));
 		lo_b = lo_a + h;
 		at_a = lo_b + h;
 		at_b = at_a + h;
@@ -2304,12 +2320,12 @@ static int build_from_keys_undirected(pgq_csr *csr, Workspace *ws, cudaStream_t 
 		uint64_t *key_a, *key_b, *key_sorted;
 		int32_t *val_a, *val_b, *val_sorted;
 		const size_t tb = (size_t)t * sizeof(int32_t);
-		PGQ_TRY(pgq_ws_reserve(ws, 48, (size_t)t * sizeof(uint64_t), (void **)&key_a));
-		PGQ_TRY(pgq_ws_reserve(ws, 49, (size_t)t * sizeof(uint64_t), (void **)&key_b));
-		PGQ_TRY(pgq_ws_reserve(ws, 50, tb, (void **)&val_a));
-		PGQ_TRY(pgq_ws_reserve(ws, 51, tb, (void **)&val_b));
-		PGQ_TRY(pgq_ws_reserve(ws, 52, tb + sizeof(int32_t), (void **)&flag));
-		PGQ_TRY(pgq_ws_reserve(ws, 17, pgq_scan_tmp_elems(std::max<int64_t>(m, t) + 1) * sizeof(int32_t),
+		PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_SORT_A, (size_t)t * sizeof(uint64_t), (void **)&key_a));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_SORT_B, (size_t)t * sizeof(uint64_t), (void **)&key_b));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_IDX_A, tb, (void **)&val_a));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_IDX_B, tb, (void **)&val_b));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_UKEY_AUX, tb + sizeof(int32_t), (void **)&flag));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_SCAN, pgq_scan_tmp_elems(std::max<int64_t>(m, t) + 1) * sizeof(int32_t),
 		                       (void **)&scan_tmp));
 		PGQ_TRY(pgq_scan_exclusive_i32(rows, rows, m + 1, scan_tmp, s)); // rows -> first row of every edge
 		k_ukey_expand<<<grid_m, 256, 0, s>>>(rows, slo, dlo, ms, md, sorted_row, m, b, key_a, val_a);
@@ -2350,18 +2366,33 @@ static int build_from_keys_undirected(pgq_csr *csr, Workspace *ws, cudaStream_t 
 	return finalize_from_rows(csr, ws, s);
 }
 
-// Copies a host column (NULL = absent) into workspace slot `slot`.
-static int stage_column(Workspace *ws, int slot, const void *host, size_t bytes, cudaStream_t s, const void **dev) {
-	*dev = nullptr;
-	if (!host) {
-		return PGQ_OK;
+// The columns staged on the device when they are on the host, then the directed or the undirected build.
+static int build_from_key_columns(pgq_csr *csr, const int64_t *vkey, const uint8_t *vvalid, int64_t m,
+                                  const int64_t *skey, const int64_t *dkey, const uint8_t *svalid,
+                                  const uint8_t *dvalid, bool host, bool undirected) {
+	const int64_t n = csr->n;
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	Workspace *ws = g.ws;
+	if (host) {
+		const size_t n8 = (size_t)n * sizeof(int64_t), m8 = (size_t)m * sizeof(int64_t);
+		PGQ_TRY(stage_column(ws, WS_KEY_IN_VKEY, vkey, n8, (const void **)&vkey));
+		PGQ_TRY(stage_column(ws, WS_KEY_IN_VVALID, vvalid, (size_t)n, (const void **)&vvalid));
+		PGQ_TRY(stage_column(ws, WS_KEY_IN_SKEY, skey, m8, (const void **)&skey));
+		PGQ_TRY(stage_column(ws, WS_KEY_IN_DKEY, dkey, m8, (const void **)&dkey));
+		PGQ_TRY(stage_column(ws, WS_KEY_IN_SVALID, svalid, (size_t)m, (const void **)&svalid));
+		PGQ_TRY(stage_column(ws, WS_KEY_IN_DVALID, dvalid, (size_t)m, (const void **)&dvalid));
+	} else {
+		// the columns may have been produced on any stream of the caller: wait for the whole device once
+		cudaError_t e = cudaDeviceSynchronize();
+		if (e != cudaSuccess) {
+			cudaGetLastError();
+			return pgq_fail(PGQ_ERR_CUDA, "cudaDeviceSynchronize failed: %s", cudaGetErrorString(e));
+		}
 	}
-	void *d;
-	PGQ_TRY(pgq_ws_reserve(ws, slot, bytes, &d));
-	if (bytes > 0) {
-		PGQ_CUDA(cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, s));
-	}
-	*dev = d;
+	PGQ_TRY(undirected ? build_from_keys_undirected(csr, ws, ws->stream, vkey, vvalid, skey, dkey, svalid, dvalid, m)
+	                   : build_from_keys(csr, ws, ws->stream, vkey, vvalid, skey, dkey, svalid, dvalid, m));
+	g.settled = true;
 	return PGQ_OK;
 }
 
@@ -2381,41 +2412,7 @@ static int csr_build_keys(pgq_ctx *ctx, int64_t n, const int64_t *vkey, const ui
 	csr->ctx = ctx;
 	csr->n = n;
 	csr->edge_init = true;
-	Workspace *ws = nullptr;
-	int st = pgq_ws_acquire(ctx, &ws);
-	if (st != PGQ_OK) {
-		delete csr;
-		return st;
-	}
-	cudaStream_t s = ws->stream;
-	do {
-		if (host) {
-			// (slots 40-45: the searches' lane-mask arrays, slots 28-30, must not be written -- a workspace remembers
-			// which of their rows hold zeros, Workspace::clean_from)
-			const size_t n8 = (size_t)n * sizeof(int64_t), m8 = (size_t)m * sizeof(int64_t);
-			if ((st = stage_column(ws, 40, vkey, n8, s, (const void **)&vkey)) != PGQ_OK) break;
-			if ((st = stage_column(ws, 41, vvalid, (size_t)n, s, (const void **)&vvalid)) != PGQ_OK) break;
-			if ((st = stage_column(ws, 42, skey, m8, s, (const void **)&skey)) != PGQ_OK) break;
-			if ((st = stage_column(ws, 43, dkey, m8, s, (const void **)&dkey)) != PGQ_OK) break;
-			if ((st = stage_column(ws, 44, svalid, (size_t)m, s, (const void **)&svalid)) != PGQ_OK) break;
-			if ((st = stage_column(ws, 45, dvalid, (size_t)m, s, (const void **)&dvalid)) != PGQ_OK) break;
-		} else {
-			// the columns may have been produced on any stream of the caller: wait for the whole device once
-			cudaError_t e = cudaDeviceSynchronize();
-			if (e != cudaSuccess) {
-				cudaGetLastError();
-				st = pgq_fail(PGQ_ERR_CUDA, "cudaDeviceSynchronize failed: %s", cudaGetErrorString(e));
-				break;
-			}
-		}
-		st = undirected ? build_from_keys_undirected(csr, ws, s, vkey, vvalid, skey, dkey, svalid, dvalid, m)
-		                : build_from_keys(csr, ws, s, vkey, vvalid, skey, dkey, svalid, dvalid, m);
-	} while (0);
-	if (st != PGQ_OK) {
-		cudaStreamSynchronize(s); // (queued copies from the caller's columns must not outlive the call)
-		cudaGetLastError();
-	}
-	pgq_ws_release(ctx, ws);
+	const int st = build_from_key_columns(csr, vkey, vvalid, m, skey, dkey, svalid, dvalid, host, undirected);
 	if (st != PGQ_OK) {
 		pgq_csr_free(csr);
 		return st;
@@ -2460,6 +2457,47 @@ extern "C" int pgq_csr_build_keys_undirected_device(pgq_ctx *ctx, int64_t n_vert
 	                      d_edge_dst_keys, d_edge_src_valid, d_edge_dst_valid, false, true, out);
 }
 
+// The finished CSR of pgq_csr_upload is turned back into edge rows in CSR position order (which IS the arrival order
+// per source) and goes through the same pipeline as a device-side build.
+static int build_from_csr_arrays(pgq_csr *csr, const int64_t *v, const int64_t *e, const int64_t *edge_ids) {
+	const int64_t n = csr->n, m = csr->m;
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	Workspace *ws = g.ws;
+	cudaStream_t s = ws->stream;
+	int *d_err;
+	int32_t *off_tmp;
+	const size_t cap = (size_t)std::max<int64_t>(m, 1);
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_ERR, 256, (void **)&d_err));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_D, (size_t)(n + 2) * sizeof(int32_t), (void **)&off_tmp));
+	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_src, cap * sizeof(int32_t)));
+	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_dst, cap * sizeof(int32_t)));
+	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_eid, cap * sizeof(int64_t)));
+	cudaMemsetAsync(d_err, 0, sizeof(int), s);
+	// v[0..n] are the row offsets in the reference layout (v[n+1] == v[n] == m is padding)
+	PGQ_TRY(upload_narrow(ws, v, n + 1, 0, m + 1, off_tmp, d_err, s));
+	if (m > 0) {
+		PGQ_TRY(upload_narrow(ws, e, m, 0, n, csr->st_dst, d_err, s));
+	}
+	k_check_offsets<<<grid_for(n + 1, 256), 256, 0, s>>>(off_tmp, n, m, d_err);
+	int flag = 0;
+	PGQ_TRY(read_flag(d_err, s, &flag));
+	if (flag) {
+		return pgq_fail(PGQ_ERR_RANGE, "CSR arrays hold ids outside [0,n) or offsets that do not run from 0 to m");
+	}
+	if (m > 0) {
+		k_rows_from_offsets<<<grid_for(n * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(off_tmp, n, csr->st_src);
+		if (edge_ids) {
+			cudaMemcpyAsync(csr->st_eid, edge_ids, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, s);
+		} else {
+			k_iota64<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->st_eid, m);
+		}
+	}
+	PGQ_TRY(finalize_from_rows(csr, ws, s));
+	g.settled = true;
+	return PGQ_OK;
+}
+
 extern "C" int pgq_csr_upload(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *v, const int64_t *e,
                               const int64_t *edge_ids, pgq_csr **out) {
 	if (!ctx || !out || !v || (m > 0 && !e)) {
@@ -2478,48 +2516,7 @@ extern "C" int pgq_csr_upload(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t 
 	csr->edge_size = m;
 	csr->staged = m;
 	csr->edge_init = true;
-	Workspace *ws = nullptr;
-	int st = pgq_ws_acquire(ctx, &ws);
-	if (st != PGQ_OK) {
-		delete csr;
-		return st;
-	}
-	cudaStream_t s = ws->stream;
-	do {
-		// the finished CSR is turned back into edge rows in CSR position order (which IS the arrival
-		// order per source) and goes through the same pipeline as a device-side build
-		int *d_err;
-		int32_t *off_tmp;
-		const size_t cap = (size_t)std::max<int64_t>(m, 1);
-		if ((st = pgq_ws_reserve(ws, 2, 256, (void **)&d_err)) != PGQ_OK) break;
-		if ((st = pgq_ws_reserve(ws, 11, (size_t)(n + 2) * sizeof(int32_t), (void **)&off_tmp)) != PGQ_OK) break;
-		if ((st = dev_alloc(csr, (void **)&csr->st_src, cap * sizeof(int32_t))) != PGQ_OK) break;
-		if ((st = dev_alloc(csr, (void **)&csr->st_dst, cap * sizeof(int32_t))) != PGQ_OK) break;
-		if ((st = dev_alloc(csr, (void **)&csr->st_eid, cap * sizeof(int64_t))) != PGQ_OK) break;
-		cudaMemsetAsync(d_err, 0, sizeof(int), s);
-		// v[0..n] are the row offsets in the reference layout (v[n+1] == v[n] == m is padding)
-		if ((st = upload_narrow(ws, v, n + 1, 0, m + 1, off_tmp, d_err, s)) != PGQ_OK) break;
-		if (m > 0) {
-			if ((st = upload_narrow(ws, e, m, 0, n, csr->st_dst, d_err, s)) != PGQ_OK) break;
-		}
-		k_check_offsets<<<grid_for(n + 1, 256), 256, 0, s>>>(off_tmp, n, m, d_err);
-		int flag = 0;
-		if ((st = read_flag(d_err, s, &flag)) != PGQ_OK) break;
-		if (flag) {
-			st = pgq_fail(PGQ_ERR_RANGE, "CSR arrays hold ids outside [0,n) or offsets that do not run from 0 to m");
-			break;
-		}
-		if (m > 0) {
-			k_rows_from_offsets<<<grid_for(n * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(off_tmp, n, csr->st_src);
-			if (edge_ids) {
-				cudaMemcpyAsync(csr->st_eid, edge_ids, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, s);
-			} else {
-				k_iota64<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->st_eid, m);
-			}
-		}
-		st = finalize_from_rows(csr, ws, s);
-	} while (0);
-	pgq_ws_release(ctx, ws);
+	const int st = build_from_csr_arrays(csr, v, e, edge_ids);
 	if (st != PGQ_OK) {
 		pgq_csr_free(csr);
 		return st;
@@ -2538,51 +2535,49 @@ extern "C" int pgq_csr_download(pgq_csr *csr, int64_t *v_out, int64_t *e_out, in
 	}
 	PGQ_CUDA(cudaSetDevice(csr->ctx->device));
 	int64_t n = csr->n, m = csr->m;
-	Workspace *ws;
-	PGQ_TRY(pgq_ws_acquire(csr->ctx, &ws));
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
-	int st = PGQ_OK;
-	do {
-		// back to the reference's layout: original vertex order, original ids
-		int32_t *orig_off, *scan_tmp;
-		int64_t *tmp_e, *tmp_id;
-		if ((st = pgq_ws_reserve(ws, 0, (size_t)(n + 2) * sizeof(int32_t), (void **)&orig_off)) != PGQ_OK) break;
-		if ((st = pgq_ws_reserve(ws, 1, pgq_scan_tmp_elems(n + 1) * sizeof(int32_t), (void **)&scan_tmp)) != PGQ_OK) break;
-		if ((st = pgq_ws_reserve(ws, 4, (size_t)std::max<int64_t>(std::max<int64_t>(m, n + 2), 1) * sizeof(int64_t),
-		                         (void **)&tmp_e)) != PGQ_OK) break;
-		tmp_id = nullptr;
-		if (edge_ids_out &&
-		    (st = pgq_ws_reserve(ws, 5, (size_t)std::max<int64_t>(m, 1) * sizeof(int64_t), (void **)&tmp_id)) != PGQ_OK) break;
-		k_orig_degrees<<<grid_for(n + 1, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->out.off, csr->perm, n, orig_off);
-		if ((st = pgq_scan_exclusive_i32(orig_off, orig_off, n + 1, scan_tmp, s)) != PGQ_OK) break;
-		if (m > 0 && (e_out || edge_ids_out)) {
-			k_orig_rows<<<grid_for(n * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->out.off, csr->out.adj, csr->edge_ids, csr->perm,
-			                                                       csr->inv, orig_off, n, e_out ? tmp_e : nullptr,
-			                                                       edge_ids_out ? tmp_id : nullptr);
-			if (e_out) {
-				cudaMemcpyAsync(e_out, tmp_e, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
-			}
-			if (edge_ids_out) {
-				cudaMemcpyAsync(edge_ids_out, tmp_id, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
-			}
-			cudaStreamSynchronize(s);
+	// back to the reference's layout: original vertex order, original ids
+	int32_t *orig_off, *scan_tmp;
+	int64_t *tmp_e, *tmp_id = nullptr;
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_A, (size_t)(n + 2) * sizeof(int32_t), (void **)&orig_off));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_SCAN, pgq_scan_tmp_elems(n + 1) * sizeof(int32_t), (void **)&scan_tmp));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_WIDE, (size_t)std::max<int64_t>(std::max<int64_t>(m, n + 2), 1) * sizeof(int64_t),
+	                       (void **)&tmp_e));
+	if (edge_ids_out) {
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_A, (size_t)std::max<int64_t>(m, 1) * sizeof(int64_t), (void **)&tmp_id));
+	}
+	k_orig_degrees<<<grid_for(n + 1, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->out.off, csr->perm, n, orig_off);
+	PGQ_TRY(pgq_scan_exclusive_i32(orig_off, orig_off, n + 1, scan_tmp, s));
+	if (m > 0 && (e_out || edge_ids_out)) {
+		k_orig_rows<<<grid_for(n * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->out.off, csr->out.adj, csr->edge_ids, csr->perm,
+		                                                       csr->inv, orig_off, n, e_out ? tmp_e : nullptr,
+		                                                       edge_ids_out ? tmp_id : nullptr);
+		if (e_out) {
+			cudaMemcpyAsync(e_out, tmp_e, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
 		}
-		if (v_out) {
-			k_widen<<<grid_for(n + 1, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(orig_off, tmp_e, n + 1);
-			cudaMemcpyAsync(v_out, tmp_e, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
-			cudaStreamSynchronize(s);
-			v_out[n + 1] = v_out[n]; // the reference's padding slot
+		if (edge_ids_out) {
+			cudaMemcpyAsync(edge_ids_out, tmp_id, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
 		}
-		cudaError_t e = cudaStreamSynchronize(s);
-		if (e == cudaSuccess) {
-			e = cudaGetLastError();
-		}
-		if (e != cudaSuccess) {
-			st = pgq_fail(PGQ_ERR_CUDA, "CSR download failed: %s", cudaGetErrorString(e));
-		}
-	} while (0);
-	pgq_ws_release(csr->ctx, ws);
-	return st;
+		cudaStreamSynchronize(s);
+	}
+	if (v_out) {
+		k_widen<<<grid_for(n + 1, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(orig_off, tmp_e, n + 1);
+		cudaMemcpyAsync(v_out, tmp_e, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+		cudaStreamSynchronize(s);
+		v_out[n + 1] = v_out[n]; // the reference's padding slot
+	}
+	cudaError_t e = cudaStreamSynchronize(s);
+	if (e == cudaSuccess) {
+		e = cudaGetLastError();
+	}
+	if (e != cudaSuccess) {
+		return pgq_fail(PGQ_ERR_CUDA, "CSR download failed: %s", cudaGetErrorString(e));
+	}
+	g.settled = true;
+	return PGQ_OK;
 }
 
 extern "C" int pgq_csr_info(pgq_csr *csr, int64_t *n, int64_t *m, int64_t *device_bytes) {
@@ -2621,31 +2616,29 @@ extern "C" int pgq_csr_download_weights(pgq_csr *csr, void *w_out) {
 	}
 	PGQ_CUDA(cudaSetDevice(csr->ctx->device));
 	const int64_t n = csr->n, m = csr->m;
-	Workspace *ws;
-	PGQ_TRY(pgq_ws_acquire(csr->ctx, &ws));
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
-	int st = PGQ_OK;
-	do {
-		int32_t *orig_off, *scan_tmp;
-		int64_t *tmp_w;
-		if ((st = pgq_ws_reserve(ws, 0, (size_t)(n + 2) * sizeof(int32_t), (void **)&orig_off)) != PGQ_OK) break;
-		if ((st = pgq_ws_reserve(ws, 1, pgq_scan_tmp_elems(n + 1) * sizeof(int32_t), (void **)&scan_tmp)) != PGQ_OK) break;
-		if ((st = pgq_ws_reserve(ws, 5, (size_t)std::max<int64_t>(m, 1) * sizeof(int64_t), (void **)&tmp_w)) != PGQ_OK) break;
-		k_orig_degrees<<<grid_for(n + 1, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->out.off, csr->perm, n, orig_off);
-		if ((st = pgq_scan_exclusive_i32(orig_off, orig_off, n + 1, scan_tmp, s)) != PGQ_OK) break;
-		if (m > 0) {
-			k_orig_rows<<<grid_for(n * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->out.off, csr->out.adj, csr->w_bits, csr->perm,
-			                                                       csr->inv, orig_off, n, nullptr, tmp_w);
-			cudaMemcpyAsync(w_out, tmp_w, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
-		}
-		cudaError_t e = cudaStreamSynchronize(s);
-		if (e == cudaSuccess) {
-			e = cudaGetLastError();
-		}
-		if (e != cudaSuccess) {
-			st = pgq_fail(PGQ_ERR_CUDA, "weight download failed: %s", cudaGetErrorString(e));
-		}
-	} while (0);
-	pgq_ws_release(csr->ctx, ws);
-	return st;
+	int32_t *orig_off, *scan_tmp;
+	int64_t *tmp_w;
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_A, (size_t)(n + 2) * sizeof(int32_t), (void **)&orig_off));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_SCAN, pgq_scan_tmp_elems(n + 1) * sizeof(int32_t), (void **)&scan_tmp));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_A, (size_t)std::max<int64_t>(m, 1) * sizeof(int64_t), (void **)&tmp_w));
+	k_orig_degrees<<<grid_for(n + 1, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->out.off, csr->perm, n, orig_off);
+	PGQ_TRY(pgq_scan_exclusive_i32(orig_off, orig_off, n + 1, scan_tmp, s));
+	if (m > 0) {
+		k_orig_rows<<<grid_for(n * 32, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->out.off, csr->out.adj, csr->w_bits, csr->perm,
+		                                                       csr->inv, orig_off, n, nullptr, tmp_w);
+		cudaMemcpyAsync(w_out, tmp_w, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+	}
+	cudaError_t e = cudaStreamSynchronize(s);
+	if (e == cudaSuccess) {
+		e = cudaGetLastError();
+	}
+	if (e != cudaSuccess) {
+		return pgq_fail(PGQ_ERR_CUDA, "weight download failed: %s", cudaGetErrorString(e));
+	}
+	g.settled = true;
+	return PGQ_OK;
 }

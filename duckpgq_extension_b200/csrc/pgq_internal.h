@@ -79,12 +79,110 @@ struct PullGraph {
 	int64_t n_short = 0, n_slices = 0, s_total = 0;
 };
 
-#define PGQ_WS_SLOTS 60
+// ---- workspace slots ---------------------------------------------------------------------------
+// A workspace holds one device buffer per slot.  The blocks below say who holds a slot and for how long.  Consumers
+// that never run at the same time on one workspace share numbers on purpose, so that a pooled workspace holds the
+// largest of their buffers rather than the sum: one number may have a name in several blocks.
+enum WsSlot : int {
+	// The search masks, persistent across calls: a workspace remembers which of their rows hold zeros
+	// (Workspace::clean_from), so only the BFS drivers may write them.
+	WS_SEEN = 28, WS_VISIT_A = 29, WS_VISIT_B = 30,
+	// radix_sort_pairs' histogram and scan scratch: a caller of it keeps nothing here.
+	WS_RADIX_HIST = 14, WS_RADIX_SCAN = 15,
+	// The host columns of the path entry points (pgq_api.cu, pgq_cheapest.cu) staged on the device, and their results
+	// there.  They live while a driver runs, so no driver uses them.  (WS_OUT_OFFSETS is shortestpath's,
+	// WS_IN_DST_VALID cheapest_path_length's.)
+	WS_IN_SRC = 6, WS_IN_DST = 7, WS_IN_VALID = 8, WS_OUT_LEN = 9, WS_OUT_VALID = 10, WS_OUT_OFFSETS = 11,
+	WS_IN_DST_VALID = 11, WS_OUT_LENGTHS = 12,
+	// The BFS call driver (pgq_bfs.cu), then the second side of iterativelengthbidirectional: its masks, item lists,
+	// lane -> seed vertex map and the meet test's accumulator.  (A bidirectional call leaves the search masks dirty
+	// outside the known-zero rows, and says so through Workspace::clean_from.)
+	WS_ROW_LANE = 3, WS_STATUS = 4, WS_LEVEL = 5, WS_ITEMS_A = 13, WS_ITEMS_B = 14, WS_TLIST = 15, WS_TBITS = 16,
+	WS_WALK = 17, WS_ELEMS = 18, WS_SLOT_OFF = 19, WS_PSRC = 20, WS_PDST = 21, WS_SATBITS = 22, WS_SHARED_ROWS = 23,
+	WS_LANE_SRC = 24, WS_ASSIGN_TMP = 25, WS_BATCH_ROWS = 26, WS_PATH_TOTAL = 27,
+	WS_SEEN_D = 32, WS_VISIT_A_D = 33, WS_VISIT_B_D = 34, WS_LANE_DST = 35, WS_ITEMS_A_D = 36, WS_ITEMS_B_D = 37,
+	WS_MEET = 38,
+	// Scratch of the CSR build (finalize, metadata, bottom-up layout, upload) and of the downloads: a scan's scratch,
+	// the error flag, small flags, an int64 column, O(n + m) temporaries (the sorts' buffers, a download's second
+	// column) and per-vertex arrays.
+	WS_CSR_SCAN = 1, WS_CSR_ERR = 2, WS_CSR_FLAGS = 3, WS_CSR_WIDE = 4, WS_CSR_EDGE_A = 5, WS_CSR_EDGE_B = 6,
+	WS_CSR_EDGE_C = 7, WS_CSR_VERTEX_A = 0, WS_CSR_VERTEX_B = 9, WS_CSR_VERTEX_C = 10, WS_CSR_VERTEX_D = 11,
+	WS_CSR_VERTEX_E = 12,
+	// cheapest_path_length (pgq_cheapest.cu)
+	WS_BF_DIST = 0, WS_BF_DIRTY = 1, WS_BF_FLAGS = 2,
+	// local_clustering_coefficient: its staged column and results
+	WS_LCC_SRC = 16, WS_LCC_OUT = 17, WS_LCC_OUT_VALID = 18, WS_LCC_BIG_ROWS = 19, WS_LCC_BIG_CNT = 20,
+	WS_LCC_SRC_VALID = 21, WS_LCC_BITMAP = 22,
+	// pagerank and weakly_connected_component.  WCC's six edge arrays take WS_WCC_EDGES and the five slots after it;
+	// its merge sort reuses the first three once they are dead.
+	WS_AN_REF_OFF = 16, WS_AN_SCAN = 17, WS_PR_KEY_A = 18, WS_PR_KEY_B = 19, WS_PR_VAL_A = 20, WS_PR_VAL_B = 21,
+	WS_PR_IN_OFF = 22, WS_PR_SCAN = 23, WS_PR_DFLAG = 24, WS_PR_RANK = 25, WS_PR_TEMP = 26, WS_PR_CONTRIB = 27,
+	WS_PR_DANGLING = 12, WS_PR_TOTAL = 13,
+	WS_WCC_EDGES = 18, WS_WCC_COMP = 24, WS_WCC_HOOK = 25, WS_WCC_BEST = 26, WS_WCC_MERGE_POS = 27, WS_WCC_MERGE_A = 11,
+	WS_WCC_MERGE_B = 12, WS_WCC_FLAGS = 13, WS_WCC_SORT_KEY = 18, WS_WCC_SORT_IDX_A = 19, WS_WCC_SORT_IDX_B = 20,
+	// The key builds (pgq_csr_build_keys*), which go on into the CSR build's scratch: the vertex-key sort and the
+	// joins, the host route's staged columns, and the undirected de-duplication.
+	WS_KEY_STATUS = 2, WS_KEY_POS = 16, WS_KEY_SCAN = 17, WS_KEY_SORT_A = 18, WS_KEY_SORT_B = 19, WS_KEY_ROW_A = 20,
+	WS_KEY_ROW_B = 21, WS_KEY_EDGE_A = 22, WS_KEY_EDGE_B = 23, WS_KEY_EDGE_C = 24,
+	WS_KEY_IN_VKEY = 40, WS_KEY_IN_VVALID = 41, WS_KEY_IN_SKEY = 42, WS_KEY_IN_DKEY = 43, WS_KEY_IN_SVALID = 44,
+	WS_KEY_IN_DVALID = 45,
+	WS_UKEY_MS = 46, WS_UKEY_MD = 47, WS_UKEY_SORT_A = 48, WS_UKEY_SORT_B = 49, WS_UKEY_IDX_A = 50, WS_UKEY_IDX_B = 51,
+	WS_UKEY_AUX = 52, WS_UKEY_R_ROW = 53, WS_UKEY_M_ROW = 54, WS_UKEY_DCNT = 55, WS_UKEY_NULL_MULT = 56,
+	WS_UKEY_H_LO = 57, WS_UKEY_H_MULT = 58,
+	WS_SLOTS // (the last block holds the highest numbers)
+};
+
+// The rules between the blocks, checked on their names.
+constexpr int ws_masks[] = {WS_SEEN, WS_VISIT_A, WS_VISIT_B};
+constexpr int ws_radix[] = {WS_RADIX_HIST, WS_RADIX_SCAN};
+constexpr int ws_staging[] = {WS_IN_SRC, WS_IN_DST, WS_IN_VALID, WS_OUT_LEN, WS_OUT_VALID, WS_OUT_OFFSETS,
+                              WS_IN_DST_VALID, WS_OUT_LENGTHS};
+constexpr int ws_driver[] = {WS_ROW_LANE, WS_STATUS, WS_LEVEL, WS_ITEMS_A, WS_ITEMS_B, WS_TLIST, WS_TBITS, WS_WALK,
+                             WS_ELEMS, WS_SLOT_OFF, WS_PSRC, WS_PDST, WS_SATBITS, WS_SHARED_ROWS, WS_LANE_SRC,
+                             WS_ASSIGN_TMP, WS_BATCH_ROWS, WS_PATH_TOTAL, WS_SEEN_D, WS_VISIT_A_D, WS_VISIT_B_D,
+                             WS_LANE_DST, WS_ITEMS_A_D, WS_ITEMS_B_D, WS_MEET};
+constexpr int ws_csr[] = {WS_CSR_SCAN, WS_CSR_ERR, WS_CSR_FLAGS, WS_CSR_WIDE, WS_CSR_EDGE_A, WS_CSR_EDGE_B,
+                          WS_CSR_EDGE_C, WS_CSR_VERTEX_A, WS_CSR_VERTEX_B, WS_CSR_VERTEX_C, WS_CSR_VERTEX_D,
+                          WS_CSR_VERTEX_E};
+constexpr int ws_bf[] = {WS_BF_DIST, WS_BF_DIRTY, WS_BF_FLAGS};
+constexpr int ws_analytics[] = {WS_LCC_SRC, WS_LCC_OUT, WS_LCC_OUT_VALID, WS_LCC_BIG_ROWS, WS_LCC_BIG_CNT,
+                                WS_LCC_SRC_VALID, WS_LCC_BITMAP, WS_AN_REF_OFF, WS_AN_SCAN, WS_PR_KEY_A, WS_PR_KEY_B,
+                                WS_PR_VAL_A, WS_PR_VAL_B, WS_PR_IN_OFF, WS_PR_SCAN, WS_PR_DFLAG, WS_PR_RANK,
+                                WS_PR_TEMP, WS_PR_CONTRIB, WS_PR_DANGLING, WS_PR_TOTAL, WS_WCC_EDGES, WS_WCC_EDGES + 5,
+                                WS_WCC_COMP, WS_WCC_HOOK, WS_WCC_BEST, WS_WCC_MERGE_POS, WS_WCC_MERGE_A,
+                                WS_WCC_MERGE_B, WS_WCC_FLAGS, WS_WCC_SORT_KEY, WS_WCC_SORT_IDX_A, WS_WCC_SORT_IDX_B};
+constexpr int ws_keys[] = {WS_KEY_STATUS, WS_KEY_POS, WS_KEY_SCAN, WS_KEY_SORT_A, WS_KEY_SORT_B, WS_KEY_ROW_A,
+                           WS_KEY_ROW_B, WS_KEY_EDGE_A, WS_KEY_EDGE_B, WS_KEY_EDGE_C, WS_UKEY_MS, WS_UKEY_MD,
+                           WS_UKEY_SORT_A, WS_UKEY_SORT_B, WS_UKEY_IDX_A, WS_UKEY_IDX_B, WS_UKEY_AUX, WS_UKEY_R_ROW,
+                           WS_UKEY_M_ROW, WS_UKEY_DCNT, WS_UKEY_NULL_MULT, WS_UKEY_H_LO, WS_UKEY_H_MULT};
+constexpr int ws_key_staging[] = {WS_KEY_IN_VKEY, WS_KEY_IN_VVALID, WS_KEY_IN_SKEY, WS_KEY_IN_DKEY, WS_KEY_IN_SVALID,
+                                  WS_KEY_IN_DVALID};
+template <size_t A, size_t B>
+constexpr bool ws_disjoint(const int (&a)[A], const int (&b)[B]) {
+	for (int x : a) {
+		for (int y : b) {
+			if (x == y) {
+				return false;
+			}
+		}
+	}
+	return true;
+}
+template <size_t A, size_t... B>
+constexpr bool ws_apart(const int (&a)[A], const int (&...b)[B]) {
+	return (ws_disjoint(a, b) && ...);
+}
+static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_analytics, ws_keys, ws_key_staging),
+              "only the BFS drivers may write the search masks");
+static_assert(ws_apart(ws_staging, ws_driver, ws_bf), "a path entry point's staged columns live while its driver runs");
+static_assert(ws_apart(ws_radix, ws_csr, ws_analytics, ws_keys), "radix_sort_pairs' scratch is apart from its callers'");
+static_assert(ws_apart(ws_key_staging, ws_keys, ws_csr, ws_radix), "a key build's staged columns live while it builds");
+
 // Scratch of one path-function call (mask arrays etc.), pooled per context and grown on demand.
 struct Workspace {
 	pgq_ctx *ctx = nullptr; // the context whose pool it belongs to
-	void *buf[PGQ_WS_SLOTS] = {};
-	size_t cap[PGQ_WS_SLOTS] = {};
+	void *buf[WS_SLOTS] = {};
+	size_t cap[WS_SLOTS] = {};
 	cudaStream_t stream = nullptr; // owned stream for host-pointer calls
 	cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
 	std::vector<cudaEvent_t> ev_pool; // pairs around expansion kernels
@@ -178,18 +276,48 @@ struct pgq_csr {
 // ---- helpers implemented in pgq_csr.cu ---------------------------------------------------------
 int pgq_ws_acquire(pgq_ctx *ctx, Workspace **out);     // blocks while the context's workspace budget is used up
 int pgq_ws_try_acquire(pgq_ctx *ctx, Workspace **out); // PGQ_ERR_OOM instead of blocking
-int pgq_ws_grow(Workspace *ws, int slot, size_t bytes, size_t keep_bytes, cudaStream_t s, void **out);
+int pgq_ws_grow(Workspace *ws, WsSlot slot, size_t bytes, size_t keep_bytes, cudaStream_t s, void **out);
 void pgq_ws_release(pgq_ctx *ctx, Workspace *ws);
-int pgq_ws_reserve(Workspace *ws, int slot, size_t bytes, void **out);
+int pgq_ws_reserve(Workspace *ws, WsSlot slot, size_t bytes, void **out);
+// copies a host column (NULL = absent: *dev = NULL) into the slot on the workspace stream
+int stage_column(Workspace *ws, WsSlot slot, const void *host, size_t bytes, const void **dev);
 int pgq_ws_pinned(Workspace *ws, size_t bytes, void **out);
 int pgq_scan_exclusive_i32(const int32_t *in, int32_t *out, int64_t count, int32_t *block_tmp, cudaStream_t s);
 size_t pgq_scan_tmp_elems(int64_t count);
-// stable LSD radix sort of (int32 or uint64 key, int32 value) pairs by the low end_bit bits; uses workspace slots 14
-// and 15
+// stable LSD radix sort of (int32 or uint64 key, int32 value) pairs by the low end_bit bits; uses WS_RADIX_HIST and
+// WS_RADIX_SCAN
 int radix_sort_pairs(Workspace *ws, int32_t *keys_a, int32_t *keys_b, int32_t *vals_a, int32_t *vals_b, int64_t count,
                      int end_bit, cudaStream_t s, int32_t **keys_res, int32_t **vals_res);
 int radix_sort_pairs(Workspace *ws, uint64_t *keys_a, uint64_t *keys_b, int32_t *vals_a, int32_t *vals_b, int64_t count,
                      int end_bit, cudaStream_t s, uint64_t **keys_res, int32_t **vals_res);
+
+// Holds an acquired workspace (PGQ_TRY(pgq_ws_acquire(ctx, &g.ws))) and releases it on every return.  A call that
+// returns before it marked itself settled first waits for what it queued: copies from / to the caller's buffers and
+// kernels on the caller's stream must not outlive the call, nor leak into the workspace's next user, nor into the
+// buffers a failed build gives back to the cache.
+struct WsGuard {
+	pgq_ctx *ctx;
+	Workspace *ws = nullptr;
+	cudaStream_t used = nullptr; // a caller-provided stream the work was enqueued on, if any
+	bool has_used = false;
+	bool settled = false; // the call has synchronised the workspace stream itself
+	explicit WsGuard(pgq_ctx *c) : ctx(c) {
+	}
+	WsGuard(const WsGuard &) = delete;
+	WsGuard &operator=(const WsGuard &) = delete;
+	~WsGuard() {
+		if (ws) {
+			if (!settled) {
+				cudaStreamSynchronize(ws->stream);
+				if (has_used) {
+					cudaStreamSynchronize(used); // kernels queued on the caller's stream still touch the workspace
+				}
+				cudaGetLastError();
+			}
+			pgq_ws_release(ctx, ws);
+		}
+	}
+};
 
 // ---- BFS drivers implemented in pgq_bfs.cu -----------------------------------------------------
 int pgq_bfs_lengths_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,

@@ -52,6 +52,45 @@ static int clone_dir(pgq_csr *dst, int dd, DirGraph &out, const DirGraph &in, in
 	return PGQ_OK;
 }
 
+// Copies every device array of the finalized csr into c, which lives on device dd.
+static int clone_arrays(pgq_csr *c, const pgq_csr *csr, int sd, int dd) {
+	WsGuard g(c->ctx);
+	PGQ_TRY(pgq_ws_acquire(c->ctx, &g.ws));
+	cudaStream_t s = g.ws->stream;
+	const int64_t n = csr->n, m = csr->m;
+	PGQ_TRY(clone_dir(c, dd, c->out, csr->out, sd, n, m, s));
+	PGQ_TRY(clone_dir(c, dd, c->in, csr->in, sd, n, m, s));
+	// the bottom-up layout
+	const PullGraph &pg = csr->pull;
+	PullGraph &o = c->pull;
+	o = pg; // sizes; every pointer is replaced below (nulled first: a failed clone must not free the source's arrays)
+	o.adj = nullptr;
+	o.head = nullptr;
+	o.chunk_rank = nullptr;
+	o.row = nullptr;
+	o.s_adj = nullptr;
+	o.s_row = nullptr;
+	o.s_off = nullptr;
+	PGQ_TRY(clone_array(c, dd, &o.adj, pg.adj, sd, (size_t)((std::max<int64_t>(pg.m, 1) + 1023) / 1024) * 1024, s));
+	PGQ_TRY(clone_array(c, dd, &o.head, pg.head, sd, (size_t)std::max<int64_t>(pg.nchunks, 1) * PGQ_STEPS, s));
+	PGQ_TRY(clone_array(c, dd, &o.chunk_rank, pg.chunk_rank, sd, (size_t)std::max<int64_t>(pg.nchunks, 1), s));
+	PGQ_TRY(clone_array(c, dd, &o.row, pg.row, sd, (size_t)std::max<int64_t>(pg.n_rows, 1), s));
+	PGQ_TRY(clone_array(c, dd, &o.s_adj, pg.s_adj, sd, (size_t)std::max<int64_t>(pg.s_total, 1), s));
+	PGQ_TRY(clone_array(c, dd, &o.s_row, pg.s_row, sd, (size_t)std::max<int64_t>(pg.n_slices * 32, 1), s));
+	PGQ_TRY(clone_array(c, dd, &o.s_off, pg.s_off, sd, (size_t)(pg.n_slices + 2), s));
+	PGQ_TRY(clone_array(c, dd, &c->edge_ids, csr->edge_ids, sd, (size_t)std::max<int64_t>(m, 1), s));
+	PGQ_TRY(clone_array(c, dd, &c->perm, csr->perm, sd, (size_t)std::max<int64_t>(n, 1), s));
+	PGQ_TRY(clone_array(c, dd, &c->inv, csr->inv, sd, (size_t)std::max<int64_t>(n, 1), s));
+	PGQ_TRY(clone_array(c, dd, &c->w_bits, csr->w_bits, sd, (size_t)std::max<int64_t>(m, 1), s));
+	cudaError_t e = cudaStreamSynchronize(s);
+	if (e != cudaSuccess) {
+		cudaGetLastError();
+		return pgq_fail(PGQ_ERR_CUDA, "CSR replication to device %d failed: %s", dd, cudaGetErrorString(e));
+	}
+	g.settled = true;
+	return PGQ_OK;
+}
+
 extern "C" int pgq_csr_clone(pgq_csr *csr, pgq_ctx *target, pgq_csr **out) {
 	if (!csr || !target || !out) {
 		return pgq_fail(PGQ_ERR_INVALID_ARG, "null argument");
@@ -86,47 +125,7 @@ extern "C" int pgq_csr_clone(pgq_csr *csr, pgq_ctx *target, pgq_csr **out) {
 	c->edge_init = true;
 	c->weight_type = csr->weight_type;
 	c->neg_weights = csr->neg_weights;
-	Workspace *ws = nullptr;
-	int st = pgq_ws_acquire(target, &ws);
-	if (st != PGQ_OK) {
-		delete c;
-		return st;
-	}
-	cudaStream_t s = ws->stream;
-	const int64_t n = csr->n, m = csr->m;
-	do {
-		if ((st = clone_dir(c, dd, c->out, csr->out, sd, n, m, s)) != PGQ_OK) break;
-		if ((st = clone_dir(c, dd, c->in, csr->in, sd, n, m, s)) != PGQ_OK) break;
-		{ // the bottom-up layout
-			const PullGraph &g = csr->pull;
-			PullGraph &o = c->pull;
-			o = g; // sizes; every pointer is replaced below (nulled first: a failed clone must not free the source's arrays)
-			o.adj = nullptr;
-			o.head = nullptr;
-			o.chunk_rank = nullptr;
-			o.row = nullptr;
-			o.s_adj = nullptr;
-			o.s_row = nullptr;
-			o.s_off = nullptr;
-			if ((st = clone_array(c, dd, &o.adj, g.adj, sd, (size_t)((std::max<int64_t>(g.m, 1) + 1023) / 1024) * 1024, s)) != PGQ_OK) break;
-			if ((st = clone_array(c, dd, &o.head, g.head, sd, (size_t)std::max<int64_t>(g.nchunks, 1) * PGQ_STEPS, s)) != PGQ_OK) break;
-			if ((st = clone_array(c, dd, &o.chunk_rank, g.chunk_rank, sd, (size_t)std::max<int64_t>(g.nchunks, 1), s)) != PGQ_OK) break;
-			if ((st = clone_array(c, dd, &o.row, g.row, sd, (size_t)std::max<int64_t>(g.n_rows, 1), s)) != PGQ_OK) break;
-			if ((st = clone_array(c, dd, &o.s_adj, g.s_adj, sd, (size_t)std::max<int64_t>(g.s_total, 1), s)) != PGQ_OK) break;
-			if ((st = clone_array(c, dd, &o.s_row, g.s_row, sd, (size_t)std::max<int64_t>(g.n_slices * 32, 1), s)) != PGQ_OK) break;
-			if ((st = clone_array(c, dd, &o.s_off, g.s_off, sd, (size_t)(g.n_slices + 2), s)) != PGQ_OK) break;
-		}
-		if ((st = clone_array(c, dd, &c->edge_ids, csr->edge_ids, sd, (size_t)std::max<int64_t>(m, 1), s)) != PGQ_OK) break;
-		if ((st = clone_array(c, dd, &c->perm, csr->perm, sd, (size_t)std::max<int64_t>(n, 1), s)) != PGQ_OK) break;
-		if ((st = clone_array(c, dd, &c->inv, csr->inv, sd, (size_t)std::max<int64_t>(n, 1), s)) != PGQ_OK) break;
-		if ((st = clone_array(c, dd, &c->w_bits, csr->w_bits, sd, (size_t)std::max<int64_t>(m, 1), s)) != PGQ_OK) break;
-		cudaError_t e = cudaStreamSynchronize(s);
-		if (e != cudaSuccess) {
-			cudaGetLastError();
-			st = pgq_fail(PGQ_ERR_CUDA, "CSR replication to device %d failed: %s", dd, cudaGetErrorString(e));
-		}
-	} while (0);
-	pgq_ws_release(target, ws);
+	const int st = clone_arrays(c, csr, sd, dd);
 	if (st != PGQ_OK) {
 		pgq_csr_free(c);
 		return st;
