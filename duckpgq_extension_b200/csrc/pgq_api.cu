@@ -23,6 +23,30 @@ static int check_call(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t
 	return PGQ_OK;
 }
 
+// The rows of a host-column call on the device: src, dst and valid (NULL: every row) copied from the host, and the
+// row outputs reserved
+struct DeviceRows {
+	const int64_t *src = nullptr, *dst = nullptr;
+	const uint8_t *valid = nullptr;
+	int64_t *len = nullptr; // (not reserved for shortestpath, which returns lists)
+	uint8_t *out_valid = nullptr;
+	int64_t h2d = 0; // bytes copied to the device
+};
+
+static int stage_rows(Workspace *ws, int64_t p, const int64_t *src, const int64_t *dst, const uint8_t *valid,
+                      bool lengths, DeviceRows *d) {
+	const size_t b8 = (size_t)p * sizeof(int64_t);
+	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d->src));
+	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d->dst));
+	if (lengths) {
+		PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LEN, b8, (void **)&d->len));
+	}
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d->out_valid));
+	PGQ_TRY(stage_column(ws, WS_IN_VALID, valid, (size_t)p, (const void **)&d->valid));
+	d->h2d = 2 * (int64_t)b8 + (valid ? p : 0);
+	return PGQ_OK;
+}
+
 extern "C" int pgq_iterativelength_device(pgq_csr *csr, int64_t p, const int64_t *d_src, const int64_t *d_dst,
                                           const uint8_t *d_src_valid, const pgq_options *opts, int64_t *d_out_len,
                                           uint8_t *d_out_valid, void *stream, pgq_stats *stats) {
@@ -59,23 +83,17 @@ extern "C" int pgq_iterativelength(pgq_csr *csr, int64_t p, const int64_t *src, 
 	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
 	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
-	int64_t *d_src, *d_dst, *d_len;
-	uint8_t *d_sv, *d_ov;
 	const size_t b8 = (size_t)p * sizeof(int64_t);
-	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
-	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d_dst));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LEN, b8, (void **)&d_len));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_ov));
-	PGQ_TRY(stage_column(ws, WS_IN_VALID, src_valid, (size_t)p, (const void **)&d_sv));
-	const int64_t h2d = 2 * (int64_t)b8 + (src_valid ? p : 0);
+	DeviceRows d;
+	PGQ_TRY(stage_rows(ws, p, src, dst, src_valid, true, &d));
 	pgq_stats st;
 	memset(&st, 0, sizeof(st));
-	PGQ_TRY(pgq_bfs_lengths_device(csr, ws, p, d_src, d_dst, d_sv, opts, d_len, d_ov, s, &st));
-	PGQ_CUDA(cudaMemcpyAsync(out_len, d_len, b8, cudaMemcpyDeviceToHost, s));
-	PGQ_CUDA(cudaMemcpyAsync(out_valid, d_ov, (size_t)p, cudaMemcpyDeviceToHost, s));
+	PGQ_TRY(pgq_bfs_lengths_device(csr, ws, p, d.src, d.dst, d.valid, opts, d.len, d.out_valid, s, &st));
+	PGQ_CUDA(cudaMemcpyAsync(out_len, d.len, b8, cudaMemcpyDeviceToHost, s));
+	PGQ_CUDA(cudaMemcpyAsync(out_valid, d.out_valid, (size_t)p, cudaMemcpyDeviceToHost, s));
 	PGQ_CUDA(cudaStreamSynchronize(s));
 	g.settled = true;
-	st.h2d_bytes += h2d;
+	st.h2d_bytes += d.h2d;
 	st.d2h_bytes += (int64_t)b8 + p;
 	if (stats) {
 		*stats = st;
@@ -97,35 +115,27 @@ extern "C" int pgq_iterativelength_bidirectional(pgq_csr *csr, int64_t p, const 
 	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
 	const size_t b8 = (size_t)p * sizeof(int64_t);
-	int64_t *d_src = nullptr, *d_dst = nullptr, *d_len = nullptr;
-	uint8_t *d_v = nullptr, *d_ov = nullptr;
-	int64_t h2d = 0;
+	DeviceRows d;
 	std::vector<uint8_t> valid; // a row searches only when both of its ids are valid
 	if (p > 0) {
-		PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
-		PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d_dst));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LEN, b8, (void **)&d_len));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_ov));
-		h2d = 2 * (int64_t)b8;
 		if (src_valid || dst_valid) {
 			valid.resize((size_t)p);
 			for (int64_t i = 0; i < p; i++) {
 				valid[(size_t)i] = (!src_valid || src_valid[i]) && (!dst_valid || dst_valid[i]) ? 1 : 0;
 			}
-			PGQ_TRY(stage_column(ws, WS_IN_VALID, valid.data(), (size_t)p, (const void **)&d_v));
-			h2d += p;
 		}
+		PGQ_TRY(stage_rows(ws, p, src, dst, valid.empty() ? nullptr : valid.data(), true, &d));
 	}
 	pgq_stats st;
 	memset(&st, 0, sizeof(st));
-	PGQ_TRY(pgq_bfs_bidirectional_device(csr, ws, p, d_src, d_dst, d_v, opts, d_len, d_ov, s, &st));
+	PGQ_TRY(pgq_bfs_bidirectional_device(csr, ws, p, d.src, d.dst, d.valid, opts, d.len, d.out_valid, s, &st));
 	if (p > 0) {
-		PGQ_CUDA(cudaMemcpyAsync(out_len, d_len, b8, cudaMemcpyDeviceToHost, s));
-		PGQ_CUDA(cudaMemcpyAsync(out_valid, d_ov, (size_t)p, cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaMemcpyAsync(out_len, d.len, b8, cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaMemcpyAsync(out_valid, d.out_valid, (size_t)p, cudaMemcpyDeviceToHost, s));
 	}
 	PGQ_CUDA(cudaStreamSynchronize(s));
 	g.settled = true;
-	st.h2d_bytes += h2d;
+	st.h2d_bytes += d.h2d;
 	st.d2h_bytes += p > 0 ? (int64_t)b8 + p : 0;
 	if (stats) {
 		*stats = st;
@@ -174,26 +184,20 @@ extern "C" int pgq_reachability(pgq_csr *csr, int64_t p, const int64_t *src, con
 	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
 	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
-	int64_t *d_src, *d_dst, *d_len;
-	uint8_t *d_sv, *d_ov;
-	const size_t b8 = (size_t)p * sizeof(int64_t);
-	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
-	PGQ_TRY(stage_column(ws, WS_IN_DST, h_dst, b8, (const void **)&d_dst));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LEN, b8, (void **)&d_len));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_ov));
-	PGQ_TRY(stage_column(ws, WS_IN_VALID, h_sv, (size_t)p, (const void **)&d_sv));
-	const int64_t h2d = 2 * (int64_t)b8 + (h_sv ? p : 0);
+	DeviceRows d;
+	PGQ_TRY(stage_rows(ws, p, src, h_dst, h_sv, true, &d));
 	pgq_stats st;
 	memset(&st, 0, sizeof(st));
-	PGQ_TRY(pgq_bfs_reachability_device(csr, ws, p, d_src, d_dst, d_sv, src, h_sv, opts, d_len, d_ov, s, &st));
-	PGQ_CUDA(cudaMemcpyAsync(out, d_ov, (size_t)p, cudaMemcpyDeviceToHost, s));
+	PGQ_TRY(pgq_bfs_reachability_device(csr, ws, p, d.src, d.dst, d.valid, src, h_sv, opts, d.len, d.out_valid, s,
+	                                    &st));
+	PGQ_CUDA(cudaMemcpyAsync(out, d.out_valid, (size_t)p, cudaMemcpyDeviceToHost, s));
 	PGQ_CUDA(cudaStreamSynchronize(s));
 	g.settled = true;
 	for (int64_t i = 0; i < p; i++) {
 		out[i] &= valid[(size_t)i];
 		out_valid[i] = valid[(size_t)i];
 	}
-	st.h2d_bytes += h2d;
+	st.h2d_bytes += d.h2d;
 	st.d2h_bytes += p;
 	if (stats) {
 		*stats = st;
@@ -222,22 +226,19 @@ extern "C" int pgq_shortestpath(pgq_csr *csr, int64_t p, const int64_t *src, con
 	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
 	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
-	int64_t *d_src, *d_dst, *d_off, *d_lens;
-	uint8_t *d_sv, *d_ov;
+	int64_t *d_off, *d_lens;
 	const size_t b8 = (size_t)p * sizeof(int64_t);
-	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
-	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d_dst));
+	DeviceRows d;
+	PGQ_TRY(stage_rows(ws, p, src, dst, src_valid, false, &d));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_OFFSETS, b8, (void **)&d_off));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LENGTHS, b8, (void **)&d_lens));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_ov));
-	PGQ_TRY(stage_column(ws, WS_IN_VALID, src_valid, (size_t)p, (const void **)&d_sv));
-	const int64_t h2d = 2 * (int64_t)b8 + (src_valid ? p : 0);
 	pgq_stats st;
 	memset(&st, 0, sizeof(st));
 	int64_t *d_elems = nullptr;
 	int64_t total = 0;
 	// (d_elems points into the workspace)
-	int rc = pgq_bfs_paths_device(csr, ws, p, d_src, d_dst, d_sv, opts, d_off, d_lens, d_ov, &d_elems, &total, s, &st);
+	int rc = pgq_bfs_paths_device(csr, ws, p, d.src, d.dst, d.valid, opts, d_off, d_lens, d.out_valid, &d_elems, &total,
+	                              s, &st);
 	if (rc != PGQ_OK) {
 		return rc;
 	}
@@ -251,7 +252,7 @@ extern "C" int pgq_shortestpath(pgq_csr *csr, int64_t p, const int64_t *src, con
 	}
 	if (e == cudaSuccess) e = cudaMemcpyAsync(out_offsets, d_off, b8, cudaMemcpyDeviceToHost, s);
 	if (e == cudaSuccess) e = cudaMemcpyAsync(out_lengths, d_lens, b8, cudaMemcpyDeviceToHost, s);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(out_valid, d_ov, (size_t)p, cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(out_valid, d.out_valid, (size_t)p, cudaMemcpyDeviceToHost, s);
 	if (e == cudaSuccess) e = cudaStreamSynchronize(s);
 	g.settled = (e == cudaSuccess);
 	if (e != cudaSuccess) {
@@ -259,7 +260,7 @@ extern "C" int pgq_shortestpath(pgq_csr *csr, int64_t p, const int64_t *src, con
 		free(h_elems);
 		return pgq_fail(PGQ_ERR_CUDA, "copying paths back failed: %s", cudaGetErrorString(e));
 	}
-	st.h2d_bytes += h2d;
+	st.h2d_bytes += d.h2d;
 	st.d2h_bytes += 2 * (int64_t)b8 + p + total * (int64_t)sizeof(int64_t);
 	*out_elems = h_elems;
 	*out_total = total;

@@ -1456,17 +1456,49 @@ struct LevelTrace {
 	int side = -1;       // iterativelengthbidirectional: 0 = the source side, 1 = the destination side
 };
 
+// The batches one stream of a call runs, with their counters and level trace
 struct Run {
 	std::vector<LevelTrace> trace;
 	int64_t walk_bound = 0; // shortestpath: upper bound of the walk-buffer elements handed out so far
-	pgq_csr *csr = nullptr;
-	Workspace *ws = nullptr;
-	cudaStream_t s = nullptr;
+	pgq_csr *csr;
+	Workspace *ws;
+	cudaStream_t s;
 	pgq_stats st = {};
 	size_t ev_used = 0;
-	int sms = 0;
+	int sms;
 	int seq = 0; // sequence number of the last level status the device was asked to publish
+	Run(pgq_csr *c, Workspace *w, cudaStream_t stream) : csr(c), ws(w), s(stream), sms(c->ctx->sm_count) {
+	}
 };
+
+// Adds every additive field of b to a (lanes is the width of a batch, not a count)
+static void stats_add(pgq_stats &a, const pgq_stats &b) {
+	a.batches += b.batches;
+	a.levels += b.levels;
+	a.edges_traversed += b.edges_traversed;
+	a.frontier_vertices += b.frontier_vertices;
+	a.push_levels += b.push_levels;
+	a.pull_levels += b.pull_levels;
+	a.kernel_launches += b.kernel_launches;
+	a.h2d_bytes += b.h2d_bytes;
+	a.d2h_bytes += b.d2h_bytes;
+	a.expand_ms += b.expand_ms;
+	a.total_ms += b.total_ms;
+	a.searches += b.searches;
+	a.pruned += b.pruned;
+	a.search_rows += b.search_rows;
+	a.pull_ms += b.pull_ms;
+	a.pull_edges += b.pull_edges;
+}
+
+// The level status of one stream: a block on the device, zeroed, and the mapped host block it is published into, with
+// `extra` bytes behind it
+static int status_blocks(Run &r, size_t extra, LevelStatus **d_st, LevelStatus **h_st) {
+	PGQ_TRY(pgq_ws_reserve(r.ws, WS_STATUS, sizeof(LevelStatus), (void **)d_st));
+	PGQ_TRY(pgq_ws_pinned(r.ws, sizeof(LevelStatus) + extra, (void **)h_st));
+	PGQ_CUDA(cudaMemsetAsync(*d_st, 0, sizeof(LevelStatus), r.s));
+	return PGQ_OK;
+}
 
 // Spins until the device has published status number `seq` into the mapped host block.
 static int wait_status(Run &r, LevelStatus *h_st, int seq) {
@@ -1546,6 +1578,10 @@ struct CallCtx {
 	// reachability with the reference's batches (reachability.cpp:15-39,194-235): the sources are seen from the start
 	// and a batch runs until a level adds no bit, however many of its rows are answered
 	bool reach = false;
+	CallCtx(int64_t p_, const int64_t *src, const int64_t *dst, const pgq_options *o, int64_t *out_len,
+	        uint8_t *out_valid)
+	    : p(p_), d_src(src), d_dst(dst), opts(o), d_out_len(out_len), d_out_valid(out_valid) {
+	}
 };
 
 // What every level of a batch shares, whichever search side it expands
@@ -1590,13 +1626,18 @@ struct BfsSide {
 	}
 };
 
-// The per-batch set-up both batch drivers share: direction knobs, the top-down scratch (tlist / tbits), the
-// bottom-up range scratch and `sides` finished-rows bitmaps with their snapshots, all zeroed
-static int level_env(Run &r, const pgq_options *opts, int sides, LevelEnv *e, uint32_t **satbits) {
+// The per-batch set-up both batch drivers share: the device address of the mapped status block h_st, direction knobs,
+// the top-down scratch (tlist / tbits), the bottom-up range scratch and `sides` finished-rows bitmaps with their
+// snapshots, the bitmaps zeroed
+static int level_env(Run &r, const pgq_options *opts, LevelStatus *h_st, int sides, LevelEnv *e, uint32_t **satbits) {
 	pgq_csr *csr = r.csr;
 	Workspace *ws = r.ws;
 	const int64_t n = csr->n;
 	const size_t tbits_bytes = ((size_t)n / 32 + 1) * sizeof(uint32_t);
+	PGQ_CUDA(cudaHostGetDevicePointer((void **)&e->hd_st, h_st, 0));
+	if (r.seq == 0) {
+		*reinterpret_cast<volatile int *>(&h_st->seq) = 0; // forget whatever an earlier call left behind
+	}
 	PGQ_TRY(pgq_ws_reserve(ws, WS_TLIST, (size_t)std::max<int64_t>(n, 1) * sizeof(int32_t), (void **)&e->tlist));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_TBITS, tbits_bytes, (void **)&e->tbits));
 	// PGQ_B200_SCHEDULE (tests): the kind of every level, whatever the heuristic would pick.  Character (iter - 1) % len
@@ -1625,6 +1666,59 @@ static int level_env(Run &r, const pgq_options *opts, int sides, LevelEnv *e, ui
 	PGQ_TRY(pgq_ws_reserve(ws, WS_SHARED_ROWS, (size_t)std::max<int64_t>(e->nranges, 1) * sizeof(int32_t),
 	                       (void **)&e->shared_rows));
 	PGQ_CUDA(cudaMemsetAsync(*satbits, 0, sat_bytes, r.s));
+	PGQ_CUDA(cudaMemsetAsync(e->tbits, 0, tbits_bytes, r.s));
+	return PGQ_OK;
+}
+
+// The workspace slots of a batch's sides (seen, visit, cand, items, items_next): iterativelength runs side 0,
+// iterativelengthbidirectional both
+static const WsSlot side_slots[2][5] = {{WS_SEEN, WS_VISIT_A, WS_VISIT_B, WS_ITEMS_A, WS_ITEMS_B},
+                                        {WS_SEEN_D, WS_VISIT_A_D, WS_VISIT_B_D, WS_ITEMS_A_D, WS_ITEMS_B_D}};
+
+template <int W>
+static int reserve_side(Run &r, int k, BfsSide<W> &sd) {
+	const int64_t n = r.csr->n;
+	const size_t mask_bytes = (size_t)std::max<int64_t>(n, 1) * W * sizeof(u64);
+	const size_t items_cap = (size_t)n + (size_t)(r.csr->m / PGQ_ITEM_EDGES) + 64;
+	PGQ_TRY(pgq_ws_reserve(r.ws, side_slots[k][0], mask_bytes, (void **)&sd.seen));
+	PGQ_TRY(pgq_ws_reserve(r.ws, side_slots[k][1], mask_bytes, (void **)&sd.visit));
+	PGQ_TRY(pgq_ws_reserve(r.ws, side_slots[k][2], mask_bytes, (void **)&sd.cand));
+	PGQ_TRY(pgq_ws_reserve(r.ws, side_slots[k][3], items_cap * sizeof(int2), (void **)&sd.items));
+	PGQ_TRY(pgq_ws_reserve(r.ws, side_slots[k][4], items_cap * sizeof(int2), (void **)&sd.items_next));
+	return PGQ_OK;
+}
+
+// Level 0 of one side of the batch chk names: k_init_batch lists the batch's rows in batch_rows (= chk.batch_rows) and
+// puts the seeds of lane map lm into the side's frontier; k_update_sparse publishes that frontier, marking the seeds
+// seen when mark_seen is set.  Rows are answered at level 0 only when `answer` is set: otherwise LevelStatus::batch_n
+// is zeroed behind k_init_batch, and the update kernel finds no row to check.
+template <int W, bool PATH>
+static int seed_side(Run &r, const LevelEnv &env, BfsSide<W> &sd, const LaneMap &lm, bool mark_seen, bool answer,
+                     CheckArgs chk, int32_t *batch_rows, LevelStatus *d_st, LevelStatus *h_st) {
+	cudaStream_t s = r.s;
+	const int cnt = chk.cnt;
+	PGQ_CUDA(cudaMemsetAsync(&d_st->batch_n, 0, sizeof(int), s));
+	k_init_batch<W, PATH><<<grid_cap((std::max<int64_t>(cnt, lm.p) + 255) / 256, env.wide_grid), 256, 0, s>>>(
+	    chk.b0, cnt, lm, sd.cand, env.tbits, env.tlist, batch_rows, d_st, env.level);
+	if (!answer) {
+		PGQ_CUDA(cudaMemsetAsync(&d_st->batch_n, 0, sizeof(int), s));
+	}
+	chk.seq = ++r.seq;
+	k_update_sparse<W, PATH><<<grid_cap((cnt + 255) / 256, env.wide_grid), 256, 0, s>>>(
+	    env.tlist, sd.cand, sd.seen, sd.visit, sd.items, 0, r.csr->out.off, env.tbits, sd.items_next, d_st,
+	    mark_seen ? 1 : 0, env.level, 0, chk);
+	r.st.kernel_launches += 2;
+	PGQ_CUDA(cudaGetLastError());
+	std::swap(sd.visit, sd.cand);
+	std::swap(sd.items, sd.items_next);
+	PGQ_TRY(wait_status(r, h_st, r.seq));
+	r.st.d2h_bytes += 64;
+	for (int i = 0; i < W; i++) { // the batch's lanes whose frontier is not empty
+		const int bits = std::min(64, std::max(0, cnt - 64 * i));
+		sd.live.w[i] = (bits >= 64 ? ~0ull : ((1ull << bits) - 1)) & h_st->pub_live[i];
+	}
+	sd.pull_cost = r.csr->m;
+	sd.take_status(h_st);
 	return PGQ_OK;
 }
 
@@ -1795,41 +1889,24 @@ static int run_batch(Run &r, const CallCtx &cc, LevelStatus *d_st, LevelStatus *
 	Workspace *ws = r.ws;
 	cudaStream_t s = r.s;
 	const pgq_options *opts = cc.opts;
-	const int64_t n = csr->n, m = csr->m, p = cc.p;
+	const int64_t n = csr->n, p = cc.p;
 	const int L = 64 * W;
 	const size_t mask_bytes = (size_t)std::max<int64_t>(n, 1) * W * sizeof(u64);
-	const size_t items_cap = (size_t)n + (size_t)(m / PGQ_ITEM_EDGES) + 64;
-	const size_t tbits_bytes = ((size_t)n / 32 + 1) * sizeof(uint32_t);
 	BfsSide<W> sd;
 	int32_t *batch_rows;
-	PGQ_TRY(pgq_ws_reserve(ws, WS_SEEN, mask_bytes, (void **)&sd.seen));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_VISIT_A, mask_bytes, (void **)&sd.visit));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_VISIT_B, mask_bytes, (void **)&sd.cand));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_ITEMS_A, items_cap * sizeof(int2), (void **)&sd.items));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_ITEMS_B, items_cap * sizeof(int2), (void **)&sd.items_next));
+	PGQ_TRY(reserve_side<W>(r, 0, sd));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_BATCH_ROWS, (size_t)std::max<int64_t>(p, 1) * sizeof(int32_t), (void **)&batch_rows));
 	LevelEnv env;
 	if (PATH) {
 		PGQ_TRY(pgq_ws_reserve(ws, WS_LEVEL, (size_t)std::max<int64_t>(n, 1) * L * sizeof(uint16_t), (void **)&env.level));
 	}
 	uint16_t *level = env.level;
-	PGQ_CUDA(cudaHostGetDevicePointer((void **)&env.hd_st, h_st, 0));
-	LevelStatus *hd_st = env.hd_st;
-	if (r.seq == 0) {
-		*reinterpret_cast<volatile int *>(&h_st->seq) = 0; // forget whatever an earlier call left behind
-	}
-	PGQ_TRY(level_env(r, opts, 1, &env, &sd.satbits));
+	PGQ_TRY(level_env(r, opts, h_st, 1, &env, &sd.satbits));
 	const int64_t n_reach = env.n_reach;
-	LaneMask<W> active;
-	for (int i = 0; i < W; i++) {
-		int bits = std::min(64, std::max(0, cnt - 64 * i));
-		active.w[i] = bits >= 64 ? ~0ull : ((1ull << bits) - 1);
-	}
 	// may the batch end as soon as every row has its destination?  The reference only stops a FULL path
 	// batch early (finished_searches == LANE_LIMIT, shortest_path.cpp:144); stopping never changes a path.
 	// reachability's batches never stop early (reachability.cpp:205-234)
 	const int stop_answered = PATH ? ((!cc.ref_batching || cnt == L) ? 1 : 0) : (cc.reach ? 0 : 1);
-	PGQ_CUDA(cudaMemsetAsync(env.tbits, 0, tbits_bytes, s));
 	{
 		// A batch writes mask rows of vertices with in-edges only (rows < n_reach), except for the source bits of
 		// its first level, which that level clears again: once the arrays have been zeroed for this CSR and lane
@@ -1845,30 +1922,13 @@ static int run_batch(Run &r, const CallCtx &cc, LevelStatus *d_st, LevelStatus *
 			PGQ_CUDA(cudaMemsetAsync(sd.cand, 0, clear_bytes, s));
 		}
 	}
-	PGQ_CUDA(cudaMemsetAsync(&d_st->batch_n, 0, sizeof(int), s));
 	if (PATH) {
 		PGQ_CUDA(cudaMemsetAsync(level, 0xFF, (size_t)std::max<int64_t>(n, 1) * L * sizeof(uint16_t), s));
 	}
-	k_init_batch<W, PATH><<<grid_cap((std::max<int64_t>(cnt, p) + 255) / 256, env.wide_grid), 256, 0, s>>>(
-	    b0, cnt, cc.lm, sd.cand, env.tbits, env.tlist, batch_rows, d_st, level);
-	CheckArgs chk0 {b0, cnt, batch_rows, cc.lm, cc.d_out_len, cc.d_out_valid, 0, hd_st, ++r.seq, stop_answered};
+	const CheckArgs chk {b0, cnt, batch_rows, cc.lm, cc.d_out_len, cc.d_out_valid, 0, env.hd_st, 0, stop_answered};
 	// (mark_seen: reachability's sources are seen from the start, reachability.cpp:30, iterativelength's are not)
-	k_update_sparse<W, PATH><<<grid_cap((cnt + 255) / 256, env.wide_grid), 256, 0, s>>>(
-	    env.tlist, sd.cand, sd.seen, sd.visit, sd.items, 0, csr->out.off, env.tbits, sd.items_next, d_st, cc.reach ? 1 : 0,
-	    level, 0, chk0);
-	r.st.kernel_launches += 2;
-	PGQ_CUDA(cudaGetLastError());
-	std::swap(sd.visit, sd.cand);
-	std::swap(sd.items, sd.items_next);
-	PGQ_TRY(wait_status(r, h_st, r.seq));
-	r.st.d2h_bytes += 64;
+	PGQ_TRY((seed_side<W, PATH>(r, env, sd, cc.lm, cc.reach, true, chk, batch_rows, d_st, h_st)));
 	r.st.batches++;
-	sd.live = active;
-	for (int i = 0; i < W; i++) {
-		sd.live.w[i] &= h_st->pub_live[i];
-	}
-	sd.pull_cost = m;
-	sd.take_status(h_st);
 	int iter = 1;
 	// Path mode records the level that discovers a vertex in a uint16 array (0xFFFF = unvisited) and supports depths up
 	// to 0xFFFD.  A level 0xFFFE still runs: with reference batching a batch ends only at the level that finds its
@@ -1878,7 +1938,6 @@ static int run_batch(Run &r, const CallCtx &cc, LevelStatus *d_st, LevelStatus *
 		           ? pgq_fail(PGQ_ERR_UNSUPPORTED, "BFS deeper than 65533 levels is not supported in path mode")
 		           : PGQ_OK;
 	};
-	const CheckArgs chk {b0, cnt, batch_rows, cc.lm, cc.d_out_len, cc.d_out_valid, 0, hd_st, 0, stop_answered};
 	const auto no_more = [](const u64 *, const int2 *) { return PGQ_OK; };
 	for (;; iter++) {
 		int done = 1;
@@ -1940,19 +1999,28 @@ struct EventGuard { // (error paths must not leak the event)
 	}
 };
 
-// Lane assignment of a call (k_assign, one cooperative launch): fills the lane map in aa, the call's row outputs and
-// the counters in h_st, and h_grp_rows (rows per group of 64 lanes)
+// Start of a call of cc.p > 0 rows: its begin event, the level status (the host block followed by the rows per group of
+// 64 lanes) and the lane assignment (k_assign, one cooperative launch), which fills the call's row outputs, cc's lane
+// map and the counters of searches, pruned rows and search rows
 template <bool PATH>
-static int assign_lanes(Run &r, int64_t p, const int64_t *d_src, const int64_t *d_dst, const uint8_t *d_src_valid,
-                        int prune, int dedup, int shard_index, int shard_count, int64_t *d_out_len, uint8_t *d_out_valid,
-                        int64_t *d_out_lengths, LevelStatus *d_st, LevelStatus *h_st, int32_t *h_grp_rows, AssignArgs &aa) {
+static int start_call(Run &r, CallCtx &cc, const uint8_t *d_src_valid, int prune, int dedup, int shard_index,
+                      int shard_count, LevelStatus **d_st_out, LevelStatus **h_st_out) {
 	pgq_csr *csr = r.csr;
 	Workspace *ws = r.ws;
 	cudaStream_t s = r.s;
+	const int64_t p = cc.p;
+	PGQ_CUDA(cudaEventRecord(ws->ev_begin, s));
+	LevelStatus *d_st, *h_st;
+	PGQ_TRY(status_blocks(r, ((size_t)p / 64 + 2) * sizeof(int32_t), &d_st, &h_st));
+	*d_st_out = d_st;
+	*h_st_out = h_st;
+	int32_t *h_grp_rows = reinterpret_cast<int32_t *>(h_st + 1);
+	AssignArgs aa;
+	aa.trivial_lanes = cc.reach ? 1 : 0;
 	aa.p = p;
 	aa.n = csr->n;
-	aa.src = d_src;
-	aa.dst = d_dst;
+	aa.src = cc.d_src;
+	aa.dst = cc.d_dst;
 	aa.src_valid = d_src_valid;
 	aa.out_off = csr->out.off;
 	aa.in_off = csr->in.off;
@@ -1980,9 +2048,9 @@ static int assign_lanes(Run &r, int64_t p, const int64_t *d_src, const int64_t *
 	aa.hash_lane = tmp + p + 2 * (size_t)hash_size;
 	aa.tile_sum = tmp + p + 3 * (size_t)hash_size;
 	aa.grp_rows = aa.tile_sum + tiles;
-	aa.out_len = d_out_len;
-	aa.out_valid = d_out_valid;
-	aa.out_lengths = d_out_lengths;
+	aa.out_len = cc.d_out_len;
+	aa.out_valid = cc.d_out_valid;
+	aa.out_lengths = cc.d_out_lengths;
 	aa.st = d_st;
 	{
 		void *kargs[] = {(void *)&aa};
@@ -1995,6 +2063,18 @@ static int assign_lanes(Run &r, int64_t p, const int64_t *d_src, const int64_t *
 	PGQ_CUDA(cudaStreamSynchronize(s));
 	if (h_st->err) {
 		return pgq_fail(PGQ_ERR_RANGE, "source or destination rowid outside [0,%lld)", (long long)csr->n);
+	}
+	r.st.searches = h_st->total;
+	r.st.pruned = h_st->pruned;
+	r.st.search_rows = h_st->search_rows;
+	cc.lm = LaneMap {aa.row_lane, aa.lane_src, aa.psrc, aa.pdst, p};
+	cc.h_grp_rows = h_grp_rows;
+	return PGQ_OK;
+}
+
+static int check_direction(const pgq_options *opts) {
+	if (opts && (opts->direction < 0 || opts->direction > 2)) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "direction must be 0, 1 or 2");
 	}
 	return PGQ_OK;
 }
@@ -2012,8 +2092,36 @@ static int count_empty_batch(Run &r, const int32_t *row_lane, int64_t p) {
 	return PGQ_OK;
 }
 
+// The expansion time of a Run's levels (its event pairs), and the time and out-edges of its bottom-up levels, added to
+// its stats.  A pair whose time cannot be read is left out; the first such error is returned.
+static cudaError_t add_level_times(Run &r, double *expand_ms) {
+	const std::vector<cudaEvent_t> &ev = r.ws->ev_pool;
+	cudaError_t first = cudaSuccess;
+	double acc = 0.0;
+	for (size_t i = 0; i + 1 < r.ev_used; i += 2) {
+		float t = 0.f;
+		const cudaError_t e = cudaEventElapsedTime(&t, ev[i], ev[i + 1]);
+		first = first != cudaSuccess ? first : e;
+		acc += e == cudaSuccess ? t : 0.f;
+	}
+	for (const LevelTrace &lt : r.trace) {
+		float t = 0.f;
+		if (lt.kind == 1 && lt.ev >= 0 && (size_t)(2 * lt.ev + 1) < r.ev_used) {
+			const cudaError_t e = cudaEventElapsedTime(&t, ev[2 * lt.ev], ev[2 * lt.ev + 1]);
+			first = first != cudaSuccess ? first : e;
+			if (e == cudaSuccess) {
+				r.st.pull_ms += t;
+				r.st.pull_edges += lt.fe;
+			}
+		}
+	}
+	r.st.expand_ms += acc;
+	*expand_ms = acc;
+	return first;
+}
+
 // End of a call: its time, the expansion time, the level trace (PGQ_B200_TRACE) and the counters
-static int finish_call(Run &r, double extra_expand_ms, pgq_stats *stats) {
+static int finish_call(Run &r, pgq_stats *stats) {
 	Workspace *ws = r.ws;
 	cudaStream_t s = r.s;
 	PGQ_CUDA(cudaEventRecord(ws->ev_end, s));
@@ -2022,20 +2130,7 @@ static int finish_call(Run &r, double extra_expand_ms, pgq_stats *stats) {
 	PGQ_CUDA(cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end));
 	r.st.total_ms = ms;
 	double acc = 0.0;
-	for (size_t i = 0; i + 1 < r.ev_used; i += 2) {
-		float t = 0.f;
-		PGQ_CUDA(cudaEventElapsedTime(&t, ws->ev_pool[i], ws->ev_pool[i + 1]));
-		acc += t;
-	}
-	r.st.expand_ms = acc + extra_expand_ms;
-	for (const LevelTrace &lt : r.trace) {
-		float t = 0.f;
-		if (lt.kind == 1 && lt.ev >= 0 && (size_t)(2 * lt.ev + 1) < r.ev_used) {
-			PGQ_CUDA(cudaEventElapsedTime(&t, ws->ev_pool[2 * lt.ev], ws->ev_pool[2 * lt.ev + 1]));
-			r.st.pull_ms += t;
-			r.st.pull_edges += lt.fe;
-		}
-	}
+	PGQ_CUDA(add_level_times(r, &acc));
 	if (getenv("PGQ_B200_TRACE")) { // development aid: one line per level on stderr
 		for (size_t i = 0; i < r.trace.size(); i++) {
 			const LevelTrace &lt = r.trace[i];
@@ -2076,17 +2171,9 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 		if (l != 0 && l != 64 && l != 128 && l != 256 && l != 512) {
 			return pgq_fail(PGQ_ERR_INVALID_ARG, "lanes must be 0, 64, 128, 256 or 512");
 		}
-		if (opts->direction < 0 || opts->direction > 2) {
-			return pgq_fail(PGQ_ERR_INVALID_ARG, "direction must be 0, 1 or 2");
-		}
 	}
-	Run r;
-	r.csr = csr;
-	r.ws = ws;
-	r.s = s;
-	memset(&r.st, 0, sizeof(r.st));
-	r.ev_used = 0;
-	r.sms = csr->ctx->sm_count;
+	PGQ_TRY(check_direction(opts));
+	Run r(csr, ws, s);
 	if (PATH) {
 		*d_elems = nullptr;
 		*total_out = 0;
@@ -2097,16 +2184,6 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 		}
 		return PGQ_OK;
 	}
-	PGQ_CUDA(cudaEventRecord(ws->ev_begin, s));
-	LevelStatus *d_st, *h_st;
-	PGQ_TRY(pgq_ws_reserve(ws, WS_STATUS, sizeof(LevelStatus), (void **)&d_st));
-	PGQ_TRY(pgq_ws_pinned(ws, sizeof(LevelStatus) + ((size_t)p / 64 + 2) * sizeof(int32_t), (void **)&h_st));
-	int32_t *h_grp_rows = reinterpret_cast<int32_t *>(h_st + 1);
-	PGQ_CUDA(cudaMemsetAsync(d_st, 0, sizeof(LevelStatus), s));
-	if (PATH) {
-		PGQ_CUDA(cudaMemsetAsync(d_out_offsets, 0, (size_t)p * sizeof(int64_t), s));
-		PGQ_CUDA(cudaMemsetAsync(d_out_lengths, 0, (size_t)p * sizeof(int64_t), s));
-	}
 	const int flags = opts ? opts->flags : 0;
 	const bool ref_batching = (flags & PGQ_OPT_REFERENCE_BATCHING) != 0;
 	const int shard_count = (opts && opts->shard_count > 1) ? opts->shard_count : 1;
@@ -2114,35 +2191,24 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 	if (shard_index < 0 || shard_index >= shard_count) {
 		return pgq_fail(PGQ_ERR_INVALID_ARG, "shard_index must lie in [0, shard_count)");
 	}
-	// ---- lane assignment (one cooperative launch)
-	AssignArgs aa;
-	aa.trivial_lanes = reach ? 1 : 0;
-	PGQ_TRY(assign_lanes<PATH>(r, p, d_src, d_dst, d_src_valid, (ref_batching || (flags & PGQ_OPT_NO_PRUNE)) ? 0 : 1,
-	                          (ref_batching || (flags & PGQ_OPT_NO_DEDUP)) ? 0 : 1, shard_index, shard_count, d_out_len,
-	                          d_out_valid, d_out_lengths, d_st, h_st, h_grp_rows, aa));
-	const int total = h_st->total;
-	r.st.searches = total;
-	r.st.pruned = h_st->pruned;
-	r.st.search_rows = h_st->search_rows;
-	const int lanes = pick_lanes(opts, csr->n, total, PATH);
-	r.st.lanes = lanes;
-	CallCtx cc;
-	cc.p = p;
-	cc.d_src = d_src;
-	cc.d_dst = d_dst;
-	cc.opts = opts;
-	cc.d_out_len = d_out_len;
-	cc.d_out_valid = d_out_valid;
+	if (PATH) {
+		PGQ_CUDA(cudaMemsetAsync(d_out_offsets, 0, (size_t)p * sizeof(int64_t), s));
+		PGQ_CUDA(cudaMemsetAsync(d_out_lengths, 0, (size_t)p * sizeof(int64_t), s));
+	}
+	CallCtx cc(p, d_src, d_dst, opts, d_out_len, d_out_valid);
 	cc.d_out_lengths = d_out_lengths;
-	cc.lm = LaneMap {aa.row_lane, aa.lane_src, aa.psrc, aa.pdst, p};
-	cc.h_grp_rows = h_grp_rows;
 	cc.ref_batching = ref_batching;
 	cc.reach = reach;
+	LevelStatus *d_st = nullptr, *h_st = nullptr;
+	PGQ_TRY(start_call<PATH>(r, cc, d_src_valid, (ref_batching || (flags & PGQ_OPT_NO_PRUNE)) ? 0 : 1,
+	                         (ref_batching || (flags & PGQ_OPT_NO_DEDUP)) ? 0 : 1, shard_index, shard_count, &d_st,
+	                         &h_st));
+	const int total = h_st->total;
+	const int lanes = pick_lanes(opts, csr->n, total, PATH);
+	r.st.lanes = lanes;
 	if (PATH) {
 		PGQ_TRY(pgq_ws_reserve(ws, WS_SLOT_OFF, (size_t)p * sizeof(int64_t), (void **)&cc.slot_off));
 	}
-	int rc = PGQ_OK;
-	double extra_expand_ms = 0.0;
 	// batches of lanes in assignment order; with lanes = auto the last, partly filled batch uses the
 	// narrowest mask that holds it (a 64-lane batch costs about half of a 256-lane one per level)
 	struct Batch {
@@ -2187,12 +2253,16 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 		}
 	}
 	n_streams = PATH ? 1 : 1 + (int)extra_ws.size();
-	if (n_streams == 1) {
-		for (size_t i = 0; i < batches.size() && rc == PGQ_OK; i++) {
-			rc = run_one(r, d_st, h_st, batches[i]);
+	// stream t runs batches t, t + n_streams, ...: stream 0 on this thread, every other one on a worker thread
+	const auto run_stream = [&](Run &rr, LevelStatus *dst, LevelStatus *hst, int t) -> int {
+		int st = PGQ_OK;
+		for (size_t i = (size_t)t; i < batches.size() && st == PGQ_OK; i += (size_t)n_streams) {
+			st = run_one(rr, dst, hst, batches[i]);
 		}
-	} else {
-		EventGuard assigned;
+		return st;
+	};
+	EventGuard assigned; // (the worker streams wait for the lane assignment)
+	if (n_streams > 1) {
 		cudaError_t ce = cudaEventCreateWithFlags(&assigned.ev, cudaEventDisableTiming);
 		if (ce == cudaSuccess) {
 			ce = cudaEventRecord(assigned.ev, s);
@@ -2201,84 +2271,50 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 			cudaGetLastError();
 			return pgq_fail(PGQ_ERR_CUDA, "event setup failed: %s", cudaGetErrorString(ce));
 		}
-		std::vector<Run> runs((size_t)n_streams);
-		std::vector<int> rcs((size_t)n_streams, PGQ_OK);
-		std::vector<std::string> errs((size_t)n_streams);
-		std::vector<std::thread> threads;
-		for (int t = 1; t < n_streams; t++) { // worker t takes batches t, t + n_streams, ...
-			Workspace *w2 = extra_ws[(size_t)t - 1].ws;
-			Run &rr = runs[(size_t)t];
-			rr.csr = csr;
-			rr.ws = w2;
-			rr.s = w2->stream;
-			memset(&rr.st, 0, sizeof(rr.st));
-			rr.ev_used = 0;
-			rr.sms = r.sms;
-			threads.emplace_back([&, t, w2]() {
-				Run &rw = runs[(size_t)t];
-				int st = PGQ_OK;
-				LevelStatus *dst2 = nullptr, *hst2 = nullptr;
-				if (cudaSetDevice(csr->ctx->device) != cudaSuccess ||
-				    cudaStreamWaitEvent(w2->stream, assigned.ev, 0) != cudaSuccess) {
-					st = pgq_fail(PGQ_ERR_CUDA, "worker stream setup failed");
-				}
-				if (st == PGQ_OK) st = pgq_ws_reserve(w2, WS_STATUS, sizeof(LevelStatus), (void **)&dst2);
-				if (st == PGQ_OK) st = pgq_ws_pinned(w2, sizeof(LevelStatus), (void **)&hst2);
-				if (st == PGQ_OK && cudaMemsetAsync(dst2, 0, sizeof(LevelStatus), w2->stream) != cudaSuccess) {
-					st = pgq_fail(PGQ_ERR_CUDA, "cudaMemsetAsync failed");
-				}
-				for (size_t i = (size_t)t; i < batches.size() && st == PGQ_OK; i += (size_t)n_streams) {
-					st = run_one(rw, dst2, hst2, batches[i]);
-				}
-				if (cudaStreamSynchronize(w2->stream) != cudaSuccess && st == PGQ_OK) {
-					st = pgq_fail(PGQ_ERR_CUDA, "worker stream failed");
-				}
-				if (st != PGQ_OK) {
-					errs[(size_t)t] = pgq_last_error(); // thread-local message of this worker
-				}
-				rcs[(size_t)t] = st;
-			});
-		}
-		for (size_t i = 0; i < batches.size() && rc == PGQ_OK; i += (size_t)n_streams) {
-			rc = run_one(r, d_st, h_st, batches[i]);
-		}
-		for (auto &th : threads) {
-			th.join();
-		}
-		for (WsGuard &g : extra_ws) {
-			g.settled = true; // (its worker has waited for its stream)
-		}
-		for (int t = 1; t < n_streams; t++) {
-			Run &rw = runs[(size_t)t];
-			// fold the worker's counters and expansion times into the call's
-			for (size_t i = 0; i + 1 < rw.ev_used; i += 2) {
-				float tms = 0.f;
-				if (cudaEventElapsedTime(&tms, rw.ws->ev_pool[i], rw.ws->ev_pool[i + 1]) == cudaSuccess) {
-					extra_expand_ms += tms;
-				}
-			}
-			for (const LevelTrace &lt : rw.trace) {
-				float tms = 0.f;
-				if (lt.kind == 1 && lt.ev >= 0 && (size_t)(2 * lt.ev + 1) < rw.ev_used &&
-				    cudaEventElapsedTime(&tms, rw.ws->ev_pool[2 * lt.ev], rw.ws->ev_pool[2 * lt.ev + 1]) == cudaSuccess) {
-					r.st.pull_ms += tms;
-					r.st.pull_edges += lt.fe;
-				}
-			}
-			r.st.batches += rw.st.batches;
-			r.st.levels += rw.st.levels;
-			r.st.edges_traversed += rw.st.edges_traversed;
-			r.st.frontier_vertices += rw.st.frontier_vertices;
-			r.st.push_levels += rw.st.push_levels;
-			r.st.pull_levels += rw.st.pull_levels;
-			r.st.kernel_launches += rw.st.kernel_launches;
-			r.st.d2h_bytes += rw.st.d2h_bytes;
-			if (rc == PGQ_OK && rcs[(size_t)t] != PGQ_OK) {
-				rc = pgq_fail(rcs[(size_t)t], "%s", errs[(size_t)t].c_str());
-			}
-		}
-		extra_ws.clear(); // (back to the pool)
 	}
+	std::vector<Run> runs; // the workers'
+	for (WsGuard &g : extra_ws) {
+		runs.emplace_back(csr, g.ws, g.ws->stream);
+	}
+	std::vector<int> rcs(runs.size(), PGQ_OK);
+	std::vector<std::string> errs(runs.size());
+	std::vector<std::thread> threads;
+	for (size_t t = 0; t < runs.size(); t++) {
+		threads.emplace_back([&, t]() {
+			Run &rw = runs[t];
+			int st = PGQ_OK;
+			LevelStatus *dst2 = nullptr, *hst2 = nullptr;
+			if (cudaSetDevice(csr->ctx->device) != cudaSuccess ||
+			    cudaStreamWaitEvent(rw.s, assigned.ev, 0) != cudaSuccess) {
+				st = pgq_fail(PGQ_ERR_CUDA, "worker stream setup failed");
+			}
+			if (st == PGQ_OK) st = status_blocks(rw, 0, &dst2, &hst2);
+			if (st == PGQ_OK) st = run_stream(rw, dst2, hst2, (int)t + 1);
+			if (cudaStreamSynchronize(rw.s) != cudaSuccess && st == PGQ_OK) {
+				st = pgq_fail(PGQ_ERR_CUDA, "worker stream failed");
+			}
+			if (st != PGQ_OK) {
+				errs[t] = pgq_last_error(); // thread-local message of this worker
+			}
+			rcs[t] = st;
+		});
+	}
+	int rc = run_stream(r, d_st, h_st, 0);
+	for (auto &th : threads) {
+		th.join();
+	}
+	for (WsGuard &g : extra_ws) {
+		g.settled = true; // (its worker has waited for its stream)
+	}
+	for (size_t t = 0; t < runs.size(); t++) { // fold the workers' counters and level times into the call's
+		double expand_ms;
+		(void)add_level_times(runs[t], &expand_ms); // (a failed worker may leave a pair unrecorded: it is left out)
+		stats_add(r.st, runs[t].st);
+		if (rc == PGQ_OK && rcs[t] != PGQ_OK) {
+			rc = pgq_fail(rcs[t], "%s", errs[t].c_str());
+		}
+	}
+	extra_ws.clear(); // (back to the pool)
 	if (rc != PGQ_OK) {
 		return rc;
 	}
@@ -2286,7 +2322,7 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 	// nothing about the reference's batches.)
 	if (ref_batching && opts && opts->lanes && p > 0 && shard_count <= 1 &&
 	    (batches.empty() || batches.back().take == batches.back().lanes)) {
-		PGQ_TRY(count_empty_batch(r, aa.row_lane, p));
+		PGQ_TRY(count_empty_batch(r, cc.lm.row_lane, p));
 	}
 	if (PATH) {
 		// list offsets over ALL rows in row order, then move every walked path to its place
@@ -2309,7 +2345,7 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 		*d_elems = elems; // lives in the workspace: valid until the caller releases it
 		*total_out = list_total;
 	}
-	return finish_call(r, extra_expand_ms, stats);
+	return finish_call(r, stats);
 }
 
 int pgq_bfs_lengths_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,
@@ -2370,22 +2406,7 @@ int pgq_bfs_reachability_device(pgq_csr *csr, Workspace *ws, int64_t p, const in
 		pgq_stats st;
 		PGQ_TRY(run_call<false>(csr, ws, end - b0, d_src + b0, d_dst + b0, d_src_valid ? d_src_valid + b0 : nullptr, &bo,
 		                        d_out_len + b0, d_out_valid + b0, nullptr, nullptr, nullptr, nullptr, s, &st, true));
-		sum.batches += st.batches;
-		sum.levels += st.levels;
-		sum.edges_traversed += st.edges_traversed;
-		sum.frontier_vertices += st.frontier_vertices;
-		sum.push_levels += st.push_levels;
-		sum.pull_levels += st.pull_levels;
-		sum.kernel_launches += st.kernel_launches;
-		sum.h2d_bytes += st.h2d_bytes;
-		sum.d2h_bytes += st.d2h_bytes;
-		sum.expand_ms += st.expand_ms;
-		sum.total_ms += st.total_ms;
-		sum.searches += st.searches;
-		sum.pruned += st.pruned;
-		sum.search_rows += st.search_rows;
-		sum.pull_ms += st.pull_ms;
-		sum.pull_edges += st.pull_edges;
+		stats_add(sum, st);
 		b0 = end;
 	}
 	if (stats) {
@@ -2405,76 +2426,36 @@ static int run_bidir_batch(Run &r, const CallCtx &cc, const LaneMap &lm_dst, Lev
 	pgq_csr *csr = r.csr;
 	Workspace *ws = r.ws;
 	cudaStream_t s = r.s;
-	const int64_t n = csr->n, m = csr->m, p = cc.p;
+	const int64_t n = csr->n, p = cc.p;
 	const size_t mask_bytes = (size_t)std::max<int64_t>(n, 1) * W * sizeof(u64);
-	const size_t items_cap = (size_t)n + (size_t)(m / PGQ_ITEM_EDGES) + 64;
-	const size_t tbits_bytes = ((size_t)n / 32 + 1) * sizeof(uint32_t);
-	static const WsSlot slots[2][5] = {{WS_SEEN, WS_VISIT_A, WS_VISIT_B, WS_ITEMS_A, WS_ITEMS_B},
-	                                {WS_SEEN_D, WS_VISIT_A_D, WS_VISIT_B_D, WS_ITEMS_A_D, WS_ITEMS_B_D}};
 	BfsSide<W> side[2];
 	for (int k = 0; k < 2; k++) {
-		PGQ_TRY(pgq_ws_reserve(ws, slots[k][0], mask_bytes, (void **)&side[k].seen));
-		PGQ_TRY(pgq_ws_reserve(ws, slots[k][1], mask_bytes, (void **)&side[k].visit));
-		PGQ_TRY(pgq_ws_reserve(ws, slots[k][2], mask_bytes, (void **)&side[k].cand));
-		PGQ_TRY(pgq_ws_reserve(ws, slots[k][3], items_cap * sizeof(int2), (void **)&side[k].items));
-		PGQ_TRY(pgq_ws_reserve(ws, slots[k][4], items_cap * sizeof(int2), (void **)&side[k].items_next));
+		PGQ_TRY(reserve_side<W>(r, k, side[k]));
 	}
 	int32_t *batch_rows;
 	u64 *meet;
 	PGQ_TRY(pgq_ws_reserve(ws, WS_BATCH_ROWS, (size_t)std::max<int64_t>(p, 1) * sizeof(int32_t), (void **)&batch_rows));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_MEET, (W + 1) * sizeof(u64), (void **)&meet));
 	LevelEnv env;
-	PGQ_CUDA(cudaHostGetDevicePointer((void **)&env.hd_st, h_st, 0));
-	if (r.seq == 0) {
-		*reinterpret_cast<volatile int *>(&h_st->seq) = 0; // forget whatever an earlier call left behind
-	}
 	uint32_t *satbits = nullptr;
-	PGQ_TRY(level_env(r, cc.opts, 2, &env, &satbits));
+	PGQ_TRY(level_env(r, cc.opts, h_st, 2, &env, &satbits));
 	side[0].satbits = satbits;
 	side[1].satbits = satbits + 3 * env.sat_words;
-	LaneMask<W> active;
-	for (int i = 0; i < W; i++) {
-		const int bits = std::min(64, std::max(0, cnt - 64 * i));
-		active.w[i] = bits >= 64 ? ~0ull : ((1ull << bits) - 1);
-	}
 	// Seeds stay seen, so rows beyond n_reach get written: the known-zero rows of the search slots are not kept up here,
 	// and both mask sets are cleared whole.
 	ws->clean_from = -1;
-	PGQ_CUDA(cudaMemsetAsync(env.tbits, 0, tbits_bytes, s));
 	PGQ_CUDA(cudaMemsetAsync(meet, 0, (W + 1) * sizeof(u64), s));
 	for (int k = 0; k < 2; k++) {
 		PGQ_CUDA(cudaMemsetAsync(side[k].seen, 0, mask_bytes, s));
 		PGQ_CUDA(cudaMemsetAsync(side[k].visit, 0, mask_bytes, s));
 		PGQ_CUDA(cudaMemsetAsync(side[k].cand, 0, mask_bytes, s));
 	}
-	// no row is answered by the update kernels: batch_n is zeroed behind each k_init_batch (which lists the batch's
-	// rows, one per lane, in batch_rows for k_meet)
+	// no row is answered by the update kernels, k_meet answers them: each k_init_batch lists the batch's rows, one per
+	// lane, in batch_rows, and the seeds are seen from the start
 	const CheckArgs chk {b0, cnt, batch_rows, cc.lm, cc.d_out_len, cc.d_out_valid, 0, env.hd_st, 0, 0};
-	const unsigned init_grid = grid_cap((std::max<int64_t>(cnt, p) + 255) / 256, env.wide_grid);
 	for (int k = 0; k < 2; k++) {
-		BfsSide<W> &sd = side[k];
-		PGQ_CUDA(cudaMemsetAsync(&d_st->batch_n, 0, sizeof(int), s));
-		k_init_batch<W, false><<<init_grid, 256, 0, s>>>(b0, cnt, k ? lm_dst : cc.lm, sd.cand, env.tbits, env.tlist,
-		                                                batch_rows, d_st, nullptr);
-		PGQ_CUDA(cudaMemsetAsync(&d_st->batch_n, 0, sizeof(int), s));
-		CheckArgs chk0 = chk;
-		chk0.seq = ++r.seq;
-		// mark_seen = 1: the seeds are seen from the start
-		k_update_sparse<W, false><<<grid_cap((cnt + 255) / 256, env.wide_grid), 256, 0, s>>>(
-		    env.tlist, sd.cand, sd.seen, sd.visit, sd.items, 0, csr->out.off, env.tbits, sd.items_next, d_st, 1, nullptr,
-		    0, chk0);
-		r.st.kernel_launches += 2;
-		PGQ_CUDA(cudaGetLastError());
-		std::swap(sd.visit, sd.cand);
-		std::swap(sd.items, sd.items_next);
-		PGQ_TRY(wait_status(r, h_st, r.seq));
-		r.st.d2h_bytes += 64;
-		sd.live = active;
-		for (int i = 0; i < W; i++) {
-			sd.live.w[i] &= h_st->pub_live[i];
-		}
-		sd.pull_cost = m;
-		sd.take_status(h_st);
+		PGQ_TRY((seed_side<W, false>(r, env, side[k], k ? lm_dst : cc.lm, true, false, chk, batch_rows, d_st,
+		                                    h_st)));
 	}
 	r.st.batches++;
 	for (int it = 0;; it++) {
@@ -2510,24 +2491,15 @@ int pgq_bfs_bidirectional_device(pgq_csr *csr, Workspace *ws, int64_t p, const i
 	if (!csr->finalized) {
 		return pgq_fail(PGQ_ERR_NOT_INITIALIZED, "%s", pgq_status_text(PGQ_ERR_NOT_INITIALIZED));
 	}
-	if (opts) {
-		if (opts->lanes != 0 && opts->lanes != 512) {
-			return pgq_fail(PGQ_ERR_INVALID_ARG, "iterativelengthbidirectional runs 512 lanes per batch: lanes must be 0 or 512");
-		}
-		if (opts->direction < 0 || opts->direction > 2) {
-			return pgq_fail(PGQ_ERR_INVALID_ARG, "direction must be 0, 1 or 2");
-		}
-		if (opts->flags != 0 || opts->shard_count > 1) {
-			return pgq_fail(PGQ_ERR_UNSUPPORTED, "iterativelengthbidirectional takes no flags and no sharding");
-		}
+	if (opts && opts->lanes != 0 && opts->lanes != 512) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "iterativelengthbidirectional runs 512 lanes per batch: lanes must be 0 or 512");
+	}
+	PGQ_TRY(check_direction(opts));
+	if (opts && (opts->flags != 0 || opts->shard_count > 1)) {
+		return pgq_fail(PGQ_ERR_UNSUPPORTED, "iterativelengthbidirectional takes no flags and no sharding");
 	}
 	constexpr int W = 8; // LANE_LIMIT: a row's answer depends on the rows sharing its batch
-	Run r;
-	r.csr = csr;
-	r.ws = ws;
-	r.s = s;
-	memset(&r.st, 0, sizeof(r.st));
-	r.sms = csr->ctx->sm_count;
+	Run r(csr, ws, s);
 	r.st.lanes = 64 * W;
 	if (p == 0) {
 		if (stats) {
@@ -2535,41 +2507,24 @@ int pgq_bfs_bidirectional_device(pgq_csr *csr, Workspace *ws, int64_t p, const i
 		}
 		return PGQ_OK;
 	}
-	PGQ_CUDA(cudaEventRecord(ws->ev_begin, s));
-	LevelStatus *d_st, *h_st;
-	PGQ_TRY(pgq_ws_reserve(ws, WS_STATUS, sizeof(LevelStatus), (void **)&d_st));
-	PGQ_TRY(pgq_ws_pinned(ws, sizeof(LevelStatus) + ((size_t)p / 64 + 2) * sizeof(int32_t), (void **)&h_st));
-	int32_t *h_grp_rows = reinterpret_cast<int32_t *>(h_st + 1);
-	PGQ_CUDA(cudaMemsetAsync(d_st, 0, sizeof(LevelStatus), s));
+	CallCtx cc(p, d_src, d_dst, opts, d_out_len, d_out_valid);
+	cc.ref_batching = true;
 	// every row with a valid source and destination and src != dst takes a lane, in input order (l.93-116)
-	AssignArgs aa;
-	PGQ_TRY(assign_lanes<false>(r, p, d_src, d_dst, d_valid, 0, 0, 0, 1, d_out_len, d_out_valid, nullptr, d_st, h_st,
-	                            h_grp_rows, aa));
+	LevelStatus *d_st = nullptr, *h_st = nullptr;
+	PGQ_TRY(start_call<false>(r, cc, d_valid, 0, 0, 0, 1, &d_st, &h_st));
 	const int total = h_st->total;
-	r.st.searches = total;
-	r.st.search_rows = h_st->search_rows;
 	int32_t *lane_dst;
 	PGQ_TRY(pgq_ws_reserve(ws, WS_LANE_DST, (size_t)std::max(total, 1) * sizeof(int32_t), (void **)&lane_dst));
-	k_lane_dst<<<grid_cap((p + 255) / 256, (int64_t)r.sms * 8), 256, 0, s>>>(p, aa.row_lane, aa.pdst, lane_dst);
+	k_lane_dst<<<grid_cap((p + 255) / 256, (int64_t)r.sms * 8), 256, 0, s>>>(p, cc.lm.row_lane, cc.lm.pdst, lane_dst);
 	r.st.kernel_launches++;
 	PGQ_CUDA(cudaGetLastError());
-	CallCtx cc;
-	cc.p = p;
-	cc.d_src = d_src;
-	cc.d_dst = d_dst;
-	cc.opts = opts;
-	cc.d_out_len = d_out_len;
-	cc.d_out_valid = d_out_valid;
-	cc.lm = LaneMap {aa.row_lane, aa.lane_src, aa.psrc, aa.pdst, p};
-	cc.h_grp_rows = h_grp_rows;
-	cc.ref_batching = true;
-	const LaneMap lm_dst {aa.row_lane, lane_dst, aa.psrc, aa.pdst, p};
+	const LaneMap lm_dst {cc.lm.row_lane, lane_dst, cc.lm.psrc, cc.lm.pdst, p};
 	const int L = 64 * W;
 	for (int pos = 0; pos < total; pos += L) {
 		PGQ_TRY(run_bidir_batch<W>(r, cc, lm_dst, d_st, h_st, pos, std::min(L, total - pos)));
 	}
 	if (total == 0 || total % L == 0) {
-		PGQ_TRY(count_empty_batch(r, aa.row_lane, p));
+		PGQ_TRY(count_empty_batch(r, cc.lm.row_lane, p));
 	}
-	return finish_call(r, 0.0, stats);
+	return finish_call(r, stats);
 }

@@ -997,6 +997,30 @@ def test_two_streams_give_the_same_totals(gpu_ctx):
         csr.free()
 
 
+TIMINGS = ("expand_ms", "total_ms", "pull_ms")
+
+
+@pytest.mark.gpu
+def test_two_streams_fold_every_counter(gpu_ctx, monkeypatch):
+    """The second stream's counters are folded into the call's: one stream and two give the same answers and every
+    stats field but the timings, launches, levels and copied bytes included."""
+    csr = build_csr(gpu_ctx, "base")
+    try:
+        for name in ("lanes_513", "lanes_1025", "lanes_1100", "lanes_712", "class_mix", "distinct_2049"):
+            c = case(name)
+            for oname, flags, w in configs(c, False):
+                runs = []
+                for streams in ("1", "2"):
+                    monkeypatch.setenv("PGQ_B200_BATCH_STREAMS", streams)
+                    runs.append(csr.iterativelength(c.ps, c.pd, c.sv, options(w, flags)))
+                (out1, valid1, st1), (out2, valid2, st2) = runs
+                assert np.array_equal(valid1, valid2) and np.array_equal(out1, out2), (name, oname, w)
+                assert {k: v for k, v in st1.items() if k not in TIMINGS} == \
+                       {k: v for k, v in st2.items() if k not in TIMINGS}, (name, oname, w)
+    finally:
+        csr.free()
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("fn", ["iterativelength", "shortestpath"])
 @pytest.mark.parametrize("flags", [0, NO_DEDUP])
