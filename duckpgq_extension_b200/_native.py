@@ -112,6 +112,8 @@ SYMBOLS = {
                                    C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
     "pgq_free": (None, [_VP]),
     "pgq_cheapest_path_length": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, _PU8, C.POINTER(PgqStats)]),
+    "pgq_cheapest_path": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _P64, _P64, _PU8, C.POINTER(_P64), _P64,
+                                    C.POINTER(PgqStats)]),
     "pgq_local_clustering_coefficient": (C.c_int, [_VP, C.c_int64, _P64, _PU8, C.POINTER(C.c_float), _PU8,
                                                    C.POINTER(PgqStats)]),
     "pgq_pagerank": (C.c_int, [_VP, C.c_int64, _P64, _PU8, C.POINTER(C.c_double), _PU8, _P64, C.POINTER(PgqStats)]),

@@ -1243,6 +1243,11 @@ __global__ void __launch_bounds__(1024) k_path_offsets(int64_t p, int64_t base, 
 	}
 }
 
+void pgq_path_offsets(int64_t base, int64_t lo, int64_t hi, int64_t *out_offsets, int64_t *out_lengths,
+                      uint8_t *out_valid, int64_t *d_range_total, cudaStream_t s) {
+	k_path_offsets<<<1, 1024, 0, s>>>(hi, base, lo, hi, out_offsets, out_lengths, out_valid, d_range_total);
+}
+
 // [src] lists of the rows that took no lane (pruned src == dst)
 __global__ void k_path_trivial(int64_t p, const int64_t *__restrict__ src, const int64_t *__restrict__ dst,
                                const uint8_t *__restrict__ out_valid, const int64_t *__restrict__ out_offsets,

@@ -17,6 +17,19 @@
 // A NaN sum is never better (new_dist < n_dist is false), so an edge of NaN weight never relaxes; without
 // that test a NaN with the sign bit set would win every atomicMin.  A negative cycle anywhere in the graph,
 // reachable or not, keeps improving for ~2^62 sweeps here as in the reference: there is no cap.
+//
+// cheapest_path (no reference function: the weighted form of shortestpath's list) runs the same sweeps and then,
+// per batch, a BFS over the edges its final distances d make TIGHT for a lane: the edge at out-CSR position e, v -> u,
+// with d(v) + w(e) == d(u), the sum in the weight type's arithmetic (k_bf_sweep's int64 addition; a double sum rounded
+// to nearest) and the comparison one of values (so -0.0 == 0.0, and a NaN is equal to nothing).  h(u) is u's BFS depth
+// from the source over the lane's tight edges (h(s) = 0; the source is never entered again), and the path is
+// shortestpath's tie-break on the tight-edge graph: walking back from t, parent(u) is the smallest ORIGINAL vertex id
+// v with h(v) = h(u) - 1 and a tight edge v -> u, and the edge is the first tight position of u in v's adjacency.
+// One 64-bit atomicMin of (original id << 32 | position in v's adjacency) per tight edge picks exactly that pair.
+// When d(s) = 0, the path's weights summed left to right from 0 in the weight type's arithmetic give the row's
+// cheapest_path_length cost bit for bit, and the path has the fewest edges among the cheapest.  d(s) != 0 only through
+// the sentinel arithmetic of a weight of -inf (or, for BIGINT, below about -max/2) on an edge into s, or a DOUBLE cycle
+// through a -inf edge: the path follows the same rule, but its sum is not promised to be the cost.
 #include <algorithm>
 #include <cstring>
 
@@ -150,9 +163,19 @@ __global__ void k_bf_results(int b0, int cnt, int L, const int64_t *__restrict__
 	}
 }
 
-template <bool F64>
+// What a call does with a batch's distances once its sweeps have ended (cheapest_path_length: nothing more)
+struct NoTightSearch {
+	int operator()(int b0, int cnt, int L, const u64 *dist) const {
+		return PGQ_OK;
+	}
+};
+
+// Runs the batches.  after(b0, cnt, L, dist) is called behind each batch's results, while dist still holds its
+// distances.
+template <bool F64, class AfterSweeps>
 static int run_bf(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,
-                  const uint8_t *d_sv, const uint8_t *d_dv, int64_t *d_out, uint8_t *d_ov, pgq_stats *st) {
+                  const uint8_t *d_sv, const uint8_t *d_dv, int64_t *d_out, uint8_t *d_ov, pgq_stats *st,
+                  const AfterSweeps &after) {
 	cudaStream_t s = ws->stream;
 	const int64_t n = csr->n;
 	// lanes per batch: as many as a 2 GB distance array allows, at most 256 (the reference's largest batch)
@@ -201,6 +224,7 @@ static int run_bf(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, 
 		k_bf_results<F64><<<(cnt + 127) / 128, 128, 0, s>>>((int)b0, cnt, L, d_dst, d_sv, d_dv, csr->perm, n, dist, d_out,
 		                                                   d_ov, flags + 1);
 		st->kernel_launches++;
+		PGQ_TRY(after((int)b0, cnt, L, dist));
 	}
 	PGQ_CUDA(cudaMemcpyAsync(h_flags, flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
 	PGQ_CUDA(cudaStreamSynchronize(s));
@@ -247,8 +271,8 @@ extern "C" int pgq_cheapest_path_length(pgq_csr *csr, int64_t p, const int64_t *
 	PGQ_TRY(stage_column(ws, WS_IN_VALID, src_valid, (size_t)p, (const void **)&d_sv));
 	PGQ_TRY(stage_column(ws, WS_IN_DST_VALID, dst_valid, (size_t)p, (const void **)&d_dv));
 	st.h2d_bytes = 2 * (int64_t)b8 + (src_valid ? p : 0) + (dst_valid ? p : 0);
-	PGQ_TRY((csr->weight_type == 2) ? run_bf<true>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_out, d_ov, &st)
-	                                : run_bf<false>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_out, d_ov, &st));
+	PGQ_TRY((csr->weight_type == 2) ? run_bf<true>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_out, d_ov, &st, NoTightSearch())
+	                                : run_bf<false>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_out, d_ov, &st, NoTightSearch()));
 	cudaMemcpyAsync(out_cost, d_out, b8, cudaMemcpyDeviceToHost, s);
 	cudaMemcpyAsync(out_valid, d_ov, (size_t)p, cudaMemcpyDeviceToHost, s);
 	st.d2h_bytes = (int64_t)b8 + p;
@@ -257,6 +281,335 @@ extern "C" int pgq_cheapest_path_length(pgq_csr *csr, int64_t p, const int64_t *
 		return pgq_fail(PGQ_ERR_CUDA, "cheapest_path_length failed: %s", cudaGetErrorString(e));
 	}
 	g.settled = true;
+	if (stats) {
+		*stats = st;
+	}
+	return PGQ_OK;
+}
+
+// ---- cheapest_path: the BFS over the tight edges of a batch (see the top) --------------------------------------------
+#define TIGHT_UNSET 0xFFFFu   // h not set; a level is at most 0xFFFE
+#define TIGHT_NO_PARENT (~0ull) // a parent key no tight edge has written yet
+
+// The counters a seed or level kernel publishes for the host: [0] |F| of the frontier it marked, [1] that frontier's
+// out-edges, [2] rows whose target it reached, [3] (seed only) rows open: cost valid, s != t.
+enum { TC_FRONTIER = 0, TC_EDGES = 1, TC_REACHED = 2, TC_OPEN = 3 };
+
+// h(s) = 0 for every lane with a source, F_0 = the sources, and each lane's target: its internal id while the row is
+// open, -2 for [s] (s == t), -1 for NULL (a NULL or outside id, or a NULL cost).  One thread per lane of the batch.
+template <bool F64>
+__global__ void k_tight_seed(int b0, int cnt, int L, const int64_t *__restrict__ src, const int64_t *__restrict__ dst,
+                             const uint8_t *__restrict__ src_valid, const uint8_t *__restrict__ dst_valid,
+                             const int32_t *__restrict__ perm, const int32_t *__restrict__ off, int64_t n,
+                             const u64 *__restrict__ dist, uint16_t *level, uint32_t *front, int32_t *lane_tgt,
+                             unsigned long long *cnt_out) {
+	const int l = blockIdx.x * blockDim.x + threadIdx.x;
+	if (l >= L) {
+		return;
+	}
+	int tgt = -1;
+	if (l < cnt) {
+		const int64_t row = b0 + l;
+		const int64_t s = src[row], t = dst[row];
+		if ((!src_valid || src_valid[row]) && s >= 0 && s < n) { // (an id outside [0, n) fails the call)
+			const int ps = perm[s];
+			level[(int64_t)ps * L + l] = 0;
+			const uint32_t bit = 1u << (ps & 31);
+			if (!(atomicOr(&front[ps >> 5], bit) & bit)) {
+				atomicAdd(&cnt_out[TC_FRONTIER], 1ull);
+				atomicAdd(&cnt_out[TC_EDGES], (unsigned long long)(off[ps + 1] - off[ps]));
+			}
+			if ((!dst_valid || dst_valid[row]) && t >= 0 && t < n) {
+				const int pt = perm[t];
+				const u64 k = dist[(int64_t)pt * L + l];
+				if (s == t) {
+					tgt = -2;
+				} else if (F64 ? key_f64(k) != 1.7976931348623157e308 / 2 : (long long)k != BF_INF_I64) {
+					tgt = pt;
+					atomicAdd(&cnt_out[TC_OPEN], 1ull);
+				}
+			}
+		}
+	}
+	lane_tgt[l] = tgt;
+}
+
+// Expands F_k: a warp per frontier vertex v, 32 lanes at a time (k_bf_sweep's layout).  For each out-edge v -> u tight
+// in a lane with h(v) = k, where h(u) is unset or k + 1: h(u) = k + 1 and the parent key of (u, lane) takes the
+// minimum of (original id of v << 32 | position of the edge in v's adjacency).  The one thread whose atomicMin finds
+// no key yet has put u into F_k+1 for that lane; the first to set u's bit in `next` counts u and its out-degree.
+template <bool F64>
+__global__ void __launch_bounds__(256) k_tight_level(int k, int64_t n, int L, const int32_t *__restrict__ off,
+                                                     const int32_t *__restrict__ adj, const int64_t *__restrict__ w_bits,
+                                                     const int32_t *__restrict__ inv, const u64 *__restrict__ dist,
+                                                     uint16_t *level, u64 *pkey, const uint32_t *__restrict__ cur,
+                                                     uint32_t *next, const int32_t *__restrict__ lane_tgt,
+                                                     unsigned long long *cnt_out) {
+	const int lane = threadIdx.x & 31;
+	const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+	const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+	const uint16_t hk = (uint16_t)k, hk1 = (uint16_t)(k + 1);
+	unsigned long long nf = 0, ne = 0;
+	unsigned reached = 0;
+	for (int64_t v = warp; v < n; v += nwarps) {
+		if (!(cur[v >> 5] & (1u << (v & 31)))) {
+			continue;
+		}
+		const int e0 = off[v], e1 = off[v + 1];
+		const u64 base = (u64)(uint32_t)inv[v] << 32;
+		for (int g = 0; g < L; g += 32) {
+			const int l = g + lane;
+			const bool act = level[v * L + l] == hk;
+			if (!__any_sync(FULL_MASK, act)) {
+				continue;
+			}
+			const u64 dk = dist[v * L + l];
+			const int tgt = lane_tgt[l];
+			for (int e = e0; e < e1; e++) {
+				const int u = adj[e];
+				bool fresh = false;
+				if (act) {
+					const int64_t slot = (int64_t)u * L + l;
+					const uint16_t hu = level[slot];
+					if (hu == TIGHT_UNSET || hu == hk1) {
+						bool tight;
+						if (F64) {
+							tight = key_f64(dk) + __longlong_as_double(w_bits[e]) == key_f64(dist[slot]);
+						} else {
+							tight = dk + (u64)w_bits[e] == dist[slot];
+						}
+						if (tight) {
+							if (hu == TIGHT_UNSET) {
+								level[slot] = hk1;
+							}
+							if (atomicMin(&pkey[slot], base | (u64)(e - e0)) == TIGHT_NO_PARENT) {
+								fresh = true;
+								reached += (u == tgt);
+							}
+						}
+					}
+				}
+				if (__any_sync(FULL_MASK, fresh) && lane == 0) {
+					const uint32_t bit = 1u << (u & 31);
+					if (!(atomicOr(&next[u >> 5], bit) & bit)) {
+						nf++;
+						ne += (unsigned long long)(off[u + 1] - off[u]);
+					}
+				}
+			}
+		}
+	}
+	reached = __reduce_add_sync(FULL_MASK, reached);
+	if (lane == 0 && (nf | reached)) {
+		atomicAdd(&cnt_out[TC_FRONTIER], nf);
+		atomicAdd(&cnt_out[TC_EDGES], ne);
+		atomicAdd(&cnt_out[TC_REACHED], (unsigned long long)reached);
+	}
+}
+
+// list lengths of the batch's rows: 2 h(t) + 1, 1 for [s], 0 for NULL (k_path_offsets turns them into offsets)
+__global__ void k_tight_lengths(int b0, int cnt, int L, const int32_t *__restrict__ lane_tgt,
+                                const uint16_t *__restrict__ level, int64_t *out_lengths) {
+	const int l = blockIdx.x * blockDim.x + threadIdx.x;
+	if (l < cnt) {
+		const int tgt = lane_tgt[l];
+		int64_t len = 0;
+		if (tgt == -2) {
+			len = 1;
+		} else if (tgt >= 0) {
+			const uint16_t h = level[(int64_t)tgt * L + l];
+			len = h == TIGHT_UNSET ? 0 : 2 * (int64_t)h + 1;
+		}
+		out_lengths[b0 + l] = len;
+	}
+}
+
+// One thread per row of the batch: follows the parent keys back from t and writes [s, e1, v1, ..., ek, t] (original
+// vertex ids, edge rowids) at the row's offset.
+__global__ void k_tight_walk(int b0, int cnt, int L, const int64_t *__restrict__ src, const int64_t *__restrict__ dst,
+                             const int32_t *__restrict__ lane_tgt, const u64 *__restrict__ pkey,
+                             const int32_t *__restrict__ perm, const int32_t *__restrict__ off,
+                             const int64_t *__restrict__ edge_ids, const int64_t *__restrict__ out_offsets,
+                             const int64_t *__restrict__ out_lengths, int64_t *elems) {
+	const int l = blockIdx.x * blockDim.x + threadIdx.x;
+	if (l >= cnt) {
+		return;
+	}
+	const int64_t row = b0 + l;
+	const int64_t len = out_lengths[row];
+	if (len == 0) {
+		return;
+	}
+	int64_t *out = elems + out_offsets[row];
+	if (len == 1) {
+		out[0] = src[row];
+		return;
+	}
+	out[len - 1] = dst[row];
+	int cur = lane_tgt[l];
+	for (int64_t j = (len - 1) / 2; j >= 1; j--) {
+		const u64 key = pkey[(int64_t)cur * L + l];
+		const int v_orig = (int)(key >> 32);
+		const int v = perm[v_orig];
+		out[2 * j - 1] = edge_ids[off[v] + (int)(uint32_t)key];
+		out[2 * j - 2] = v_orig;
+		cur = v;
+	}
+}
+
+// The tight search of every batch, behind its sweeps (run_bf's AfterSweeps): levels, parent keys and the walk of the
+// batch's rows into the element array, whose offsets continue the previous batch's (rows take lanes in input order).
+template <bool F64>
+struct TightSearch {
+	pgq_csr *csr;
+	Workspace *ws;
+	const int64_t *d_src, *d_dst;
+	const uint8_t *d_sv, *d_dv;
+	int64_t *d_offsets, *d_lengths;
+	uint8_t *d_valid;
+	pgq_stats *st;
+	int64_t *total; // elements written so far
+	int operator()(int b0, int cnt, int L, const u64 *dist) const {
+		cudaStream_t s = ws->stream;
+		const int64_t n = csr->n;
+		const size_t cells = (size_t)std::max<int64_t>(n, 1) * L;
+		const size_t words = (size_t)n / 32 + 1;
+		uint16_t *level;
+		u64 *pkey;
+		uint32_t *front;
+		int32_t *lane_tgt;
+		unsigned long long *cnt_d, *cnt_h;
+		int64_t *d_range;
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CP_LEVEL, cells * sizeof(uint16_t), (void **)&level));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CP_PKEY, cells * sizeof(u64), (void **)&pkey));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CP_FRONTIER, 2 * words * sizeof(uint32_t), (void **)&front));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CP_LANE_TGT, (size_t)L * sizeof(int32_t), (void **)&lane_tgt));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_CP_COUNTERS, 256, (void **)&cnt_d));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_PATH_TOTAL, 256, (void **)&d_range));
+		PGQ_TRY(pgq_ws_pinned(ws, 256, (void **)&cnt_h));
+		PGQ_CUDA(cudaMemsetAsync(level, 0xff, cells * sizeof(uint16_t), s));
+		PGQ_CUDA(cudaMemsetAsync(pkey, 0xff, cells * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(front, 0, 2 * words * sizeof(uint32_t), s));
+		PGQ_CUDA(cudaMemsetAsync(cnt_d, 0, 4 * sizeof(unsigned long long), s));
+		k_tight_seed<F64><<<(L + 127) / 128, 128, 0, s>>>(b0, cnt, L, d_src, d_dst, d_sv, d_dv, csr->perm, csr->out.off, n,
+		                                                 dist, level, front, lane_tgt, cnt_d);
+		st->kernel_launches++;
+		PGQ_CUDA(cudaMemcpyAsync(cnt_h, cnt_d, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaStreamSynchronize(s));
+		unsigned long long nf = cnt_h[TC_FRONTIER], ne = cnt_h[TC_EDGES], open = cnt_h[TC_OPEN];
+		const int sms = csr->ctx->sm_count;
+		uint32_t *cur = front, *next = front + words;
+		// F_k is expanded while it holds a vertex and some row is still open; h is uint16 with 0xFFFF for "unset"
+		for (int k = 0; nf > 0 && open > 0; k++) {
+			if (k >= 0xFFFE) {
+				return pgq_fail(PGQ_ERR_UNSUPPORTED, "cheapest path deeper than 65534 edges is not supported");
+			}
+			st->push_levels++;
+			st->frontier_vertices += (int64_t)nf;
+			st->edges_traversed += (int64_t)ne;
+			PGQ_CUDA(cudaMemsetAsync(next, 0, words * sizeof(uint32_t), s));
+			PGQ_CUDA(cudaMemsetAsync(cnt_d, 0, 3 * sizeof(unsigned long long), s));
+			k_tight_level<F64><<<(unsigned)std::max<int64_t>(1, std::min<int64_t>((n + 7) / 8, (int64_t)sms * 8)), 256, 0, s>>>(
+			    k, n, L, csr->out.off, csr->out.adj, csr->w_bits, csr->inv, dist, level, pkey, cur, next, lane_tgt, cnt_d);
+			PGQ_CUDA(cudaGetLastError());
+			PGQ_CUDA(cudaMemcpyAsync(cnt_h, cnt_d, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+			PGQ_CUDA(cudaStreamSynchronize(s));
+			st->kernel_launches++;
+			nf = cnt_h[TC_FRONTIER];
+			ne = cnt_h[TC_EDGES];
+			open -= cnt_h[TC_REACHED];
+			std::swap(cur, next);
+		}
+		k_tight_lengths<<<(cnt + 127) / 128, 128, 0, s>>>(b0, cnt, L, lane_tgt, level, d_lengths);
+		pgq_path_offsets(*total, b0, (int64_t)b0 + cnt, d_offsets, d_lengths, d_valid, d_range, s);
+		int64_t range = 0;
+		PGQ_CUDA(cudaMemcpyAsync(&range, d_range, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaStreamSynchronize(s));
+		int64_t *elems;
+		PGQ_TRY(pgq_ws_grow(ws, WS_ELEMS, (size_t)(*total + range) * sizeof(int64_t), (size_t)*total * sizeof(int64_t), s,
+		                    (void **)&elems));
+		k_tight_walk<<<(cnt + 127) / 128, 128, 0, s>>>(b0, cnt, L, d_src, d_dst, lane_tgt, pkey, csr->perm, csr->out.off,
+		                                              csr->edge_ids, d_offsets, d_lengths, elems);
+		PGQ_CUDA(cudaGetLastError());
+		st->kernel_launches += 3;
+		*total += range;
+		return PGQ_OK;
+	}
+};
+
+extern "C" int pgq_cheapest_path(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
+                                 const uint8_t *src_valid, const uint8_t *dst_valid, int64_t *out_offsets,
+                                 int64_t *out_lengths, uint8_t *out_valid, int64_t **out_elems, int64_t *out_total,
+                                 pgq_stats *stats) {
+	if (!csr) {
+		return pgq_fail(PGQ_ERR_INVALID_ID, "%s", pgq_status_text(PGQ_ERR_INVALID_ID));
+	}
+	if (p < 0 || !out_elems || !out_total || (p > 0 && (!src || !dst || !out_offsets || !out_lengths || !out_valid))) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "null or negative argument");
+	}
+	*out_elems = nullptr;
+	*out_total = 0;
+	if (!csr->finalized || !csr->w_bits || csr->weight_type == 0) {
+		return pgq_fail(PGQ_ERR_NOT_INITIALIZED, "Need to initialize CSR before doing cheapest path");
+	}
+	if (p >= 0x7fffffffLL) {
+		return pgq_fail(PGQ_ERR_RANGE, "too many pairs in one call");
+	}
+	pgq_stats st;
+	memset(&st, 0, sizeof(st));
+	if (p == 0) {
+		if (stats) {
+			*stats = st;
+		}
+		return PGQ_OK;
+	}
+	PGQ_CUDA(cudaSetDevice(csr->ctx->device));
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	Workspace *ws = g.ws;
+	cudaStream_t s = ws->stream;
+	int64_t *d_src, *d_dst, *d_cost, *d_off, *d_lens;
+	uint8_t *d_sv, *d_dv, *d_cv, *d_ov;
+	const size_t b8 = (size_t)p * sizeof(int64_t);
+	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
+	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d_dst));
+	PGQ_TRY(stage_column(ws, WS_IN_VALID, src_valid, (size_t)p, (const void **)&d_sv));
+	PGQ_TRY(stage_column(ws, WS_IN_DST_VALID, dst_valid, (size_t)p, (const void **)&d_dv));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LEN, b8, (void **)&d_cost)); // the costs, which the sweeps write as for the lengths
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_cv));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_PATH_OFFSETS, b8, (void **)&d_off));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LENGTHS, b8, (void **)&d_lens));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_PATH_VALID, (size_t)p, (void **)&d_ov));
+	st.h2d_bytes = 2 * (int64_t)b8 + (src_valid ? p : 0) + (dst_valid ? p : 0);
+	int64_t total = 0;
+	if (csr->weight_type == 2) {
+		const TightSearch<true> tight {csr, ws, d_src, d_dst, d_sv, d_dv, d_off, d_lens, d_ov, &st, &total};
+		PGQ_TRY(run_bf<true>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_cost, d_cv, &st, tight));
+	} else {
+		const TightSearch<false> tight {csr, ws, d_src, d_dst, d_sv, d_dv, d_off, d_lens, d_ov, &st, &total};
+		PGQ_TRY(run_bf<false>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_cost, d_cv, &st, tight));
+	}
+	int64_t *h_elems = (int64_t *)malloc((size_t)(total > 0 ? total : 1) * sizeof(int64_t));
+	if (!h_elems) {
+		return pgq_fail(PGQ_ERR_OOM, "host allocation of %lld path elements failed", (long long)total);
+	}
+	cudaError_t e = cudaSuccess;
+	if (total > 0) {
+		e = cudaMemcpyAsync(h_elems, ws->buf[WS_ELEMS], (size_t)total * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+	}
+	if (e == cudaSuccess) e = cudaMemcpyAsync(out_offsets, d_off, b8, cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(out_lengths, d_lens, b8, cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(out_valid, d_ov, (size_t)p, cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+	g.settled = (e == cudaSuccess);
+	if (e != cudaSuccess) {
+		cudaGetLastError();
+		free(h_elems);
+		return pgq_fail(PGQ_ERR_CUDA, "copying cheapest paths back failed: %s", cudaGetErrorString(e));
+	}
+	st.d2h_bytes = 2 * (int64_t)b8 + p + total * (int64_t)sizeof(int64_t);
+	*out_elems = h_elems;
+	*out_total = total;
 	if (stats) {
 		*stats = st;
 	}

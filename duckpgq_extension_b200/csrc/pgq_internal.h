@@ -91,9 +91,10 @@ enum WsSlot : int {
 	WS_RADIX_HIST = 14, WS_RADIX_SCAN = 15,
 	// The host columns of the path entry points (pgq_api.cu, pgq_cheapest.cu) staged on the device, and their results
 	// there.  They live while a driver runs, so no driver uses them.  (WS_OUT_OFFSETS is shortestpath's,
-	// WS_IN_DST_VALID cheapest_path_length's.)
+	// WS_IN_DST_VALID cheapest_path_length's and cheapest_path's; cheapest_path keeps its costs in WS_OUT_LEN / _VALID
+	// and returns its lists in WS_OUT_PATH_OFFSETS, WS_OUT_LENGTHS and WS_OUT_PATH_VALID.)
 	WS_IN_SRC = 6, WS_IN_DST = 7, WS_IN_VALID = 8, WS_OUT_LEN = 9, WS_OUT_VALID = 10, WS_OUT_OFFSETS = 11,
-	WS_IN_DST_VALID = 11, WS_OUT_LENGTHS = 12,
+	WS_IN_DST_VALID = 11, WS_OUT_LENGTHS = 12, WS_OUT_PATH_OFFSETS = 31, WS_OUT_PATH_VALID = 39,
 	// The BFS call driver (pgq_bfs.cu), then the second side of iterativelengthbidirectional: its masks, item lists,
 	// lane -> seed vertex map and the meet test's accumulator.  (A bidirectional call leaves the search masks dirty
 	// outside the known-zero rows, and says so through Workspace::clean_from.)
@@ -110,6 +111,10 @@ enum WsSlot : int {
 	WS_CSR_VERTEX_E = 12,
 	// cheapest_path_length (pgq_cheapest.cu)
 	WS_BF_DIST = 0, WS_BF_DIRTY = 1, WS_BF_FLAGS = 2,
+	// cheapest_path's tight search, behind each batch's sweeps (pgq_cheapest.cu): the levels h, the parent keys, the
+	// two frontier maps, each lane's target and the level counters; the lists go to shortestpath's element array
+	// (WS_ELEMS), the element count of a batch's rows to WS_PATH_TOTAL.
+	WS_CP_LEVEL = 3, WS_CP_PKEY = 4, WS_CP_FRONTIER = 5, WS_CP_LANE_TGT = 13, WS_CP_COUNTERS = 15,
 	// local_clustering_coefficient: its staged column and results
 	WS_LCC_SRC = 16, WS_LCC_OUT = 17, WS_LCC_OUT_VALID = 18, WS_LCC_BIG_ROWS = 19, WS_LCC_BIG_CNT = 20,
 	WS_LCC_SRC_VALID = 21, WS_LCC_BITMAP = 22,
@@ -136,7 +141,7 @@ enum WsSlot : int {
 constexpr int ws_masks[] = {WS_SEEN, WS_VISIT_A, WS_VISIT_B};
 constexpr int ws_radix[] = {WS_RADIX_HIST, WS_RADIX_SCAN};
 constexpr int ws_staging[] = {WS_IN_SRC, WS_IN_DST, WS_IN_VALID, WS_OUT_LEN, WS_OUT_VALID, WS_OUT_OFFSETS,
-                              WS_IN_DST_VALID, WS_OUT_LENGTHS};
+                              WS_IN_DST_VALID, WS_OUT_LENGTHS, WS_OUT_PATH_OFFSETS, WS_OUT_PATH_VALID};
 constexpr int ws_driver[] = {WS_ROW_LANE, WS_STATUS, WS_LEVEL, WS_ITEMS_A, WS_ITEMS_B, WS_TLIST, WS_TBITS, WS_WALK,
                              WS_ELEMS, WS_SLOT_OFF, WS_PSRC, WS_PDST, WS_SATBITS, WS_SHARED_ROWS, WS_LANE_SRC,
                              WS_ASSIGN_TMP, WS_BATCH_ROWS, WS_PATH_TOTAL, WS_SEEN_D, WS_VISIT_A_D, WS_VISIT_B_D,
@@ -145,6 +150,8 @@ constexpr int ws_csr[] = {WS_CSR_SCAN, WS_CSR_ERR, WS_CSR_FLAGS, WS_CSR_WIDE, WS
                           WS_CSR_EDGE_C, WS_CSR_VERTEX_A, WS_CSR_VERTEX_B, WS_CSR_VERTEX_C, WS_CSR_VERTEX_D,
                           WS_CSR_VERTEX_E};
 constexpr int ws_bf[] = {WS_BF_DIST, WS_BF_DIRTY, WS_BF_FLAGS};
+constexpr int ws_cp[] = {WS_CP_LEVEL, WS_CP_PKEY, WS_CP_FRONTIER, WS_CP_LANE_TGT, WS_CP_COUNTERS, WS_ELEMS,
+                         WS_PATH_TOTAL};
 constexpr int ws_analytics[] = {WS_LCC_SRC, WS_LCC_OUT, WS_LCC_OUT_VALID, WS_LCC_BIG_ROWS, WS_LCC_BIG_CNT,
                                 WS_LCC_SRC_VALID, WS_LCC_BITMAP, WS_AN_REF_OFF, WS_AN_SCAN, WS_PR_KEY_A, WS_PR_KEY_B,
                                 WS_PR_VAL_A, WS_PR_VAL_B, WS_PR_IN_OFF, WS_PR_SCAN, WS_PR_DFLAG, WS_PR_RANK,
@@ -172,9 +179,12 @@ template <size_t A, size_t... B>
 constexpr bool ws_apart(const int (&a)[A], const int (&...b)[B]) {
 	return (ws_disjoint(a, b) && ...);
 }
-static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_analytics, ws_keys, ws_key_staging),
+static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_cp, ws_analytics, ws_keys,
+                       ws_key_staging),
               "only the BFS drivers may write the search masks");
 static_assert(ws_apart(ws_staging, ws_driver, ws_bf), "a path entry point's staged columns live while its driver runs");
+static_assert(ws_apart(ws_cp, ws_staging, ws_bf), "the tight search runs on the distances and columns of its call");
+static_assert(WS_OUT_PATH_OFFSETS < WS_SLOTS && WS_OUT_PATH_VALID < WS_SLOTS, "every slot has a buffer");
 static_assert(ws_apart(ws_radix, ws_csr, ws_analytics, ws_keys), "radix_sort_pairs' scratch is apart from its callers'");
 static_assert(ws_apart(ws_key_staging, ws_keys, ws_csr, ws_radix), "a key build's staged columns live while it builds");
 
@@ -320,6 +330,10 @@ struct WsGuard {
 };
 
 // ---- BFS drivers implemented in pgq_bfs.cu -----------------------------------------------------
+// shortestpath's list offsets (k_path_offsets, one block): rows [lo, hi) get offsets from `base` on, in row order, from
+// their out_lengths (0 = NULL, -1 = [src] -> 1) and out_valid = length > 0; *d_range_total = the rows' element count
+void pgq_path_offsets(int64_t base, int64_t lo, int64_t hi, int64_t *out_offsets, int64_t *out_lengths,
+                      uint8_t *out_valid, int64_t *d_range_total, cudaStream_t s);
 int pgq_bfs_lengths_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,
                            const uint8_t *d_src_valid, const pgq_options *opts, int64_t *d_out_len,
                            uint8_t *d_out_valid, cudaStream_t stream, pgq_stats *stats);

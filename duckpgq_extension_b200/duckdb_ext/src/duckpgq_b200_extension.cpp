@@ -69,6 +69,7 @@ namespace duckdb {
 // ---- process-wide device context ----------------------------------------------------------------
 static std::mutex g_ctx_lock;
 static pgq_ctx *g_ctx = nullptr;
+static std::atomic<int64_t> g_calls_cheapest_path {0};
 static std::atomic<int64_t> g_calls_lengths {0}, g_calls_paths {0}, g_calls_cheapest {0}, g_pairs {0}, g_uploads {0},
     g_device_builds {0}, g_chunks {0}, g_materialized {0}, g_calls_lcc {0}, g_calls_pagerank {0}, g_calls_wcc {0},
     g_calls_bidirectional {0}, g_calls_w_type {0}, g_calls_reachability {0};
@@ -904,6 +905,82 @@ static void CheapestPathLengthB200Function(DataChunk &args, ExpressionState &sta
 	duckpgq_state->csr_to_delete.insert(info.csr_id); // cheapest_path_length.cpp:160
 }
 
+// ---- cheapest_path (no reference function) ----------------------------------------------------------------
+// The cheapest path itself as shortestpath's list (include/duckpgq_b200.h, pgq_cheapest_path).  The bind does what
+// CheapestPathLengthBind does (cheapest_path_length_function_data.cpp:7-31: constant id, GetCSR, the mark for
+// deletion, the weights check), then returns LIST(BIGINT) whatever the weight type.
+static unique_ptr<FunctionData> CheapestPathBind(BindScalarFunctionInput &input) {
+	auto &context = input.GetClientContext();
+	auto &arguments = input.GetArguments();
+	if (!arguments[0]->IsFoldable()) {
+		throw InvalidInputException("Id must be constant.");
+	}
+	auto duckpgq_state = GetDuckPGQState(context);
+	int32_t csr_id = ExpressionExecutor::EvaluateScalar(context, *arguments[0]).GetValue<int32_t>();
+	CSR *csr = duckpgq_state->GetCSR(csr_id);
+	duckpgq_state->csr_to_delete.insert(csr_id);
+	if (!(csr->initialized_v && csr->initialized_e && csr->initialized_w)) {
+		throw ConstraintException("Need to initialize CSR before doing cheapest path");
+	}
+	input.GetBoundFunction().SetReturnType(LogicalType::LIST(LogicalType::BIGINT));
+	return make_uniq<CheapestPathLengthFunctionData>(context, csr_id);
+}
+
+static void CheapestPathB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
+	auto &info = func_expr.BindInfo()->Cast<CheapestPathLengthFunctionData>();
+	auto duckpgq_state = GetDuckPGQState(info.context);
+	(void)duckpgq_state->GetCSR(info.csr_id); // "CSR not found with ID", duckpgq_state.cpp:180-186
+	auto entry = GetB200State(info.context)->Find(info.csr_id);
+	int wt = 0;
+	if (!entry || !entry->error.empty() || pgq_csr_finalize(entry->csr) != PGQ_OK ||
+	    pgq_csr_weight_type(entry->csr, &wt) != PGQ_OK || wt == 0) {
+		throw InvalidInputException("duckpgq_b200: cheapest_path needs a weighted CSR built through create_csr_edge");
+	}
+	idx_t count = args.size();
+	UnifiedVectorFormat vsrc, vdst;
+	args.data[2].ToUnifiedFormat(vsrc);
+	args.data[3].ToUnifiedFormat(vdst);
+	auto src_data = reinterpret_cast<const int64_t *>(vsrc.data);
+	auto dst_data = reinterpret_cast<const int64_t *>(vdst.data);
+	vector<int64_t> src(count), dst(count), offsets(count), lengths(count);
+	vector<uint8_t> src_valid(count), dst_valid(count), out_valid(count);
+	for (idx_t i = 0; i < count; i++) {
+		auto sp = vsrc.sel->get_index(i), dp = vdst.sel->get_index(i);
+		src_valid[i] = vsrc.validity.RowIsValid(sp);
+		dst_valid[i] = vdst.validity.RowIsValid(dp);
+		src[i] = src_valid[i] ? src_data[sp] : 0;
+		dst[i] = dst_valid[i] ? dst_data[dp] : 0;
+	}
+	int64_t *elems = nullptr;
+	int64_t total = 0;
+	int st = pgq_cheapest_path(entry->csr, static_cast<int64_t>(count), src.data(), dst.data(), src_valid.data(),
+	                           dst_valid.data(), offsets.data(), lengths.data(), out_valid.data(), &elems, &total, nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_cheapest_path++;
+	g_pairs += static_cast<int64_t>(count);
+	result.SetVectorType(VectorType::FLAT_VECTOR);
+	auto result_data = FlatVector::GetDataMutable<list_entry_t>(result);
+	ValidityMask &result_validity = FlatVector::ValidityMutable(result);
+	ListVector::Reserve(result, static_cast<idx_t>(total));
+	if (total > 0) {
+		auto child_data = FlatVector::GetDataMutable<int64_t>(ListVector::GetChildMutable(result));
+		memcpy(child_data, elems, static_cast<size_t>(total) * sizeof(int64_t));
+	}
+	ListVector::SetListSize(result, static_cast<idx_t>(total));
+	pgq_free(elems);
+	for (idx_t i = 0; i < count; i++) {
+		result_data[i].offset = static_cast<idx_t>(offsets[i]);
+		result_data[i].length = static_cast<idx_t>(lengths[i]);
+		if (!out_valid[i]) {
+			result_validity.SetInvalid(i);
+		}
+	}
+	duckpgq_state->csr_to_delete.insert(info.csr_id);
+}
+
 // ---- local_clustering_coefficient / pagerank / weakly_connected_component ---------------------------------------
 // Registered through WrapScalar, so the signatures and binds are the reference's; the reference callback is not
 // called.  The device CSR is found like a path function's (the device build, or an upload of the host CSR).
@@ -1018,7 +1095,8 @@ static void B200StatsFunction(DataChunk &args, ExpressionState &state, Vector &r
 	              ",weakly_connected_component_calls=" + std::to_string(g_calls_wcc.load()) +
 	              ",iterativelengthbidirectional_calls=" + std::to_string(g_calls_bidirectional.load()) +
 	              ",csr_get_w_type_calls=" + std::to_string(g_calls_w_type.load()) +
-	              ",reachability_calls=" + std::to_string(g_calls_reachability.load());
+	              ",reachability_calls=" + std::to_string(g_calls_reachability.load()) +
+	              ",cheapest_path_calls=" + std::to_string(g_calls_cheapest_path.load());
 	result.SetVectorType(VectorType::CONSTANT_VECTOR);
 	ConstantVector::GetData<string_t>(result)[0] = StringVector::AddString(result, text);
 }
@@ -1119,6 +1197,11 @@ static void LoadInternal(ExtensionLoader &loader) {
 	loader.RegisterFunction(ScalarFunction(
 	    "cheapest_path_length", {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
 	    LogicalType::ANY, CheapestPathLengthB200Function, CheapestPathLengthFunctionData::CheapestPathLengthBind));
+	// cheapest_path: no reference function is replaced; called as a raw UDF over the CSR CTE (the MATCH rewriter has
+	// no CHEAPEST)
+	loader.RegisterFunction(ScalarFunction(
+	    "cheapest_path", {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
+	    LogicalType::LIST(LogicalType::BIGINT), CheapestPathB200Function, CheapestPathBind));
 	ScalarFunction stats("duckpgq_b200_stats", {}, LogicalType::VARCHAR, B200StatsFunction);
 	stats.SetVolatile();
 	loader.RegisterFunction(stats);

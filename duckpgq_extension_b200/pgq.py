@@ -7,6 +7,7 @@ like the reference's own sqllogictests:
     create_csr_edge(id, v_size, sum_cnt, edge_count, src, dst, edge)  csr_creation.cpp:112-198,210-238
     iterativelength(id, v_size, src, dst)                             iterativelength.cpp:34-152
     shortestpath(id, v_size, src, dst)                                shortest_path.cpp:43-217
+    cheapest_path(id, v_size, src, dst)                               (no reference function: the cheapest path's list)
     delete_csr(id)                                                    csr_deletion.cpp:10-29
     DuckPGQState.{csr_list, csr_to_delete, get_csr, query_end}        duckpgq_state.hpp:12-39, duckpgq_state.cpp:162-186
 
@@ -262,6 +263,28 @@ class DeviceCSR:
                                                   out.ctypes.data_as(C.c_void_p), _pu8(ov), C.byref(st)))
         return out[:p], ov[:p], st.as_dict()
 
+    def cheapest_path(self, src, dst, src_valid=None, dst_valid=None):
+        """-> (list of [src, e1, v1, ..., dst] lists or None, stats dict): the cheapest path itself, with
+        shortestpath's tie-break over the edges the costs make tight (include/duckpgq_b200.h, pgq_cheapest_path)."""
+        src, dst = _i64(src), _i64(dst)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        dv = None if dst_valid is None else np.ascontiguousarray(dst_valid, dtype=np.uint8)
+        offs = np.zeros(max(p, 1), dtype=np.int64)
+        lens = np.zeros(max(p, 1), dtype=np.int64)
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        elems = C.POINTER(C.c_int64)()
+        total = C.c_int64(0)
+        st = _native.PgqStats()
+        _check(self._lib.pgq_cheapest_path(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv), _p64(offs),
+                                           _p64(lens), _pu8(ov), C.byref(elems), C.byref(total), C.byref(st)))
+        try:  # (no rows: no element array)
+            flat = np.ctypeslib.as_array(elems, shape=(total.value,)).copy() if elems else np.zeros(0, np.int64)
+        finally:
+            self._lib.pgq_free(elems)
+        paths = [flat[offs[i]: offs[i] + lens[i]].tolist() if ov[i] else None for i in range(p)]
+        return paths, st.as_dict()
+
     def finalize(self):
         _check(self._lib.pgq_csr_finalize(self._h))
 
@@ -514,6 +537,21 @@ def cheapest_path_length(state: DuckPGQState, csr_id: int, v_size: int, src, dst
     cost, valid, _ = csr.cheapest_path_length(src, dst, src_valid, dst_valid)
     state.csr_to_delete.add(csr_id)  # cheapest_path_length.cpp:160
     return cost, valid
+
+
+def cheapest_path(state: DuckPGQState, csr_id: int, v_size: int, src, dst, src_valid=None, dst_valid=None):
+    """cheapest_path(INT, BIGINT, BIGINT, BIGINT) -> LIST(BIGINT): the cheapest path as [src, e1, v1, ..., ek, dst]
+    rowids or None (no reference function; looked up and marked as cheapest_path_length is)."""
+    csr = state.csr_list.get(csr_id)
+    if csr is None:  # DuckPGQState::GetCSR, duckpgq_state.cpp:180-186
+        raise ConstraintException(PGQ_ERR_INVALID_ID, f"CSR not found with ID {csr_id}")
+    state.csr_to_delete.add(csr_id)
+    csr.finalize()
+    if csr.weight_type() == 0:  # CheapestPathLengthBind's check, cheapest_path_length_function_data.cpp:22-24
+        raise ConstraintException(PGQ_ERR_NOT_INITIALIZED, "Need to initialize CSR before doing cheapest path")
+    paths, _ = csr.cheapest_path(src, dst, src_valid, dst_valid)
+    state.csr_to_delete.add(csr_id)
+    return paths
 
 
 def _lookup_for_path(state: DuckPGQState, csr_id: int, lengths: bool) -> DeviceCSR:

@@ -281,6 +281,25 @@ int pgq_cheapest_path_length(pgq_csr *csr, int64_t n_pairs, const int64_t *src, 
                              const uint8_t *src_valid, const uint8_t *dst_valid, void *out_cost, uint8_t *out_valid,
                              pgq_stats *stats);
 
+/* pgq_cheapest_path: the cheapest path itself, as pgq_shortestpath's list [src, e1, v1, ..., ek, dst] (vertex rowids,
+ * edge rowids), over a CSR built with pgq_csr_add_edges_weighted.  No reference function: it is the weighted form of
+ * shortestpath (SQL/PGQ's ANY CHEAPEST).
+ *   Rows take lanes and batches exactly as in pgq_cheapest_path_length, whose distances d the call computes first.
+ *   An edge v -> u is tight for a row when d(v) + w == d(u) in the weight type's arithmetic (int64 addition; double
+ *   addition rounded to nearest, compared as values: -0.0 == 0.0, a NaN equals nothing).  The path is shortestpath's
+ *   tie-break on the tight edges: fewest edges from src, and walking back from dst, the parent is the smallest vertex
+ *   id one level closer to src with a tight edge to the node, and the edge its first tight one in adjacency order.
+ *   out_valid[i] = 0 (NULL) when the source or destination is NULL, when pgq_cheapest_path_length's cost is NULL, or
+ *   when dst is not reached over tight edges (a valid but meaningless cost at a negative weight, DESIGN.md section 7);
+ *   src == dst -> [src].  When d(src) = 0 the path's weights summed from 0, left to right, give the cost bit for bit.
+ *   *out_elems is allocated by the library: release with pgq_free().  Errors as pgq_cheapest_path_length's; a tight
+ *   path deeper than 65534 edges -> PGQ_ERR_UNSUPPORTED.
+ *   stats: batches, levels (Bellman-Ford sweeps) and lanes as pgq_cheapest_path_length's; push_levels (tight levels
+ *   expanded), frontier_vertices (sum of their sizes) and edges_traversed (their out-edges). */
+int pgq_cheapest_path(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const int64_t *dst, const uint8_t *src_valid,
+                      const uint8_t *dst_valid, int64_t *out_offsets, int64_t *out_lengths, uint8_t *out_valid,
+                      int64_t **out_elems, int64_t *out_total, pgq_stats *stats);
+
 /* ---- the other consumers of the CSR ------------------------------------------------------------------------
  * Host pointers in and out.  As in the reference, "v_size" is n + 2: the two entries n and n + 1 behind the
  * vertices have no edges and take part where the reference lets them.  Results are bit-identical to the reference's.
