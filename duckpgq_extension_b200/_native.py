@@ -16,7 +16,8 @@ CSRC = os.path.join(_PKG, "csrc")
 INCLUDE = os.path.join(ROOT, "include")
 LIB_DIR = os.path.join(_PKG, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libduckpgq_b200.so")
-SOURCES = ["pgq_csr.cu", "pgq_bfs.cu", "pgq_api.cu", "pgq_cheapest.cu", "pgq_multi.cu", "pgq_analytics.cu"]
+SOURCES = ["pgq_csr.cu", "pgq_bfs.cu", "pgq_api.cu", "pgq_cheapest.cu", "pgq_allshortest.cu", "pgq_multi.cu",
+           "pgq_analytics.cu"]
 HEADERS = ["pgq_internal.h", "pgq_tile.cuh", "pgq_pull.cuh"]
 
 NVCC_FLAGS = [
@@ -114,6 +115,10 @@ SYMBOLS = {
     "pgq_cheapest_path_length": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, _PU8, C.POINTER(PgqStats)]),
     "pgq_cheapest_path": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _P64, _P64, _PU8, C.POINTER(_P64), _P64,
                                     C.POINTER(PgqStats)]),
+    "pgq_shortest_path_count": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, _P64, _PU8,
+                                          C.POINTER(PgqStats)]),
+    "pgq_all_shortest_paths": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, C.c_int64, _P64, _P64, _P64, _P64,
+                                         _PU8, C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
     "pgq_local_clustering_coefficient": (C.c_int, [_VP, C.c_int64, _P64, _PU8, C.POINTER(C.c_float), _PU8,
                                                    C.POINTER(PgqStats)]),
     "pgq_pagerank": (C.c_int, [_VP, C.c_int64, _P64, _PU8, C.POINTER(C.c_double), _PU8, _P64, C.POINTER(PgqStats)]),

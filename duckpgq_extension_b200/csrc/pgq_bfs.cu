@@ -1577,6 +1577,7 @@ struct CallCtx {
 	uint8_t *d_out_valid = nullptr;
 	int64_t *d_out_lengths = nullptr; // path mode
 	int64_t *slot_off = nullptr;      // path mode: [p] slot of a row's walked path in the walk buffer
+	PathHook *hook = nullptr;         // path mode: what each batch does instead of shortestpath's walk (nullptr: the walk)
 	LaneMap lm;
 	const int32_t *h_grp_rows = nullptr; // host copy: rows attached to each group of 64 lanes
 	bool ref_batching = false;
@@ -1958,7 +1959,20 @@ static int run_batch(Run &r, const CallCtx &cc, LevelStatus *d_st, LevelStatus *
 			break;
 		}
 	}
-	if (PATH) {
+	if (PATH && cc.hook) {
+		int64_t rows_ub = 0;
+		for (int g = b0 / 64; g <= (b0 + cnt - 1) / 64; g++) {
+			rows_ub += cc.h_grp_rows[g];
+		}
+		if (rows_ub > 0) {
+			k_path_fix_sources<<<(cnt + 127) / 128, 128, 0, s>>>(b0, cnt, L, cc.lm.lane_src, level);
+			r.st.kernel_launches++;
+			PGQ_CUDA(cudaGetLastError());
+			const PathBatch pb {b0, cnt, L, iter, rows_ub, level, batch_rows, &d_st->batch_n, cc.lm.row_lane,
+			                    cc.lm.psrc, cc.lm.pdst, cc.d_out_lengths, cc.slot_off, &r.walk_bound, ws, s, &r.st};
+			PGQ_TRY(cc.hook->batch(pb));
+		}
+	} else if (PATH) {
 		// Walk this batch's paths into the call's walk buffer (the level array is reused by the next
 		// batch).  Slots are handed out on the device; the host only bounds them: a path of this batch
 		// has at most 2 * levels + 1 elements, and the rows hanging on its lanes were counted by k_assign.
@@ -2167,7 +2181,7 @@ template <bool PATH>
 static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,
                     const uint8_t *d_src_valid, const pgq_options *opts, int64_t *d_out_len, uint8_t *d_out_valid,
                     int64_t *d_out_offsets, int64_t *d_out_lengths, int64_t **d_elems, int64_t *total_out,
-                    cudaStream_t s, pgq_stats *stats, bool reach = false) {
+                    cudaStream_t s, pgq_stats *stats, bool reach = false, PathHook *hook = nullptr) {
 	if (!csr->finalized) {
 		return pgq_fail(PGQ_ERR_NOT_INITIALIZED, "%s", pgq_status_text(PGQ_ERR_NOT_INITIALIZED));
 	}
@@ -2204,6 +2218,7 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 	cc.d_out_lengths = d_out_lengths;
 	cc.ref_batching = ref_batching;
 	cc.reach = reach;
+	cc.hook = hook;
 	LevelStatus *d_st = nullptr, *h_st = nullptr;
 	PGQ_TRY(start_call<PATH>(r, cc, d_src_valid, (ref_batching || (flags & PGQ_OPT_NO_PRUNE)) ? 0 : 1,
 	                         (ref_batching || (flags & PGQ_OPT_NO_DEDUP)) ? 0 : 1, shard_index, shard_count, &d_st,
@@ -2329,7 +2344,7 @@ static int run_call(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src
 	    (batches.empty() || batches.back().take == batches.back().lanes)) {
 		PGQ_TRY(count_empty_batch(r, cc.lm.row_lane, p));
 	}
-	if (PATH) {
+	if (PATH && (!hook || hook->lists)) {
 		// list offsets over ALL rows in row order, then move every walked path to its place
 		int64_t *d_total;
 		PGQ_TRY(pgq_ws_reserve(ws, WS_PATH_TOTAL, 256, (void **)&d_total));
@@ -2366,6 +2381,14 @@ int pgq_bfs_paths_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *
                          cudaStream_t stream, pgq_stats *stats) {
 	return run_call<true>(csr, ws, p, d_src, d_dst, d_src_valid, opts, nullptr, d_out_valid, d_out_offsets,
 	                      d_out_lengths, d_out_elems, out_total, stream, stats);
+}
+
+int pgq_bfs_paths_hooked(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,
+                         const uint8_t *d_src_valid, const pgq_options *opts, int64_t *d_out_offsets,
+                         int64_t *d_out_lengths, uint8_t *d_out_valid, int64_t **d_out_elems, int64_t *out_total,
+                         PathHook *hook, cudaStream_t stream, pgq_stats *stats) {
+	return run_call<true>(csr, ws, p, d_src, d_dst, d_src_valid, opts, nullptr, d_out_valid, d_out_offsets,
+	                      d_out_lengths, d_out_elems, out_total, stream, stats, false, hook);
 }
 
 // reachability (reachability.cpp:165-254): row i is true when its search finds dst[i] (d_out_valid[i] = 1).

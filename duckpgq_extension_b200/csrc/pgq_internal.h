@@ -134,6 +134,14 @@ enum WsSlot : int {
 	WS_UKEY_MS = 46, WS_UKEY_MD = 47, WS_UKEY_SORT_A = 48, WS_UKEY_SORT_B = 49, WS_UKEY_IDX_A = 50, WS_UKEY_IDX_B = 51,
 	WS_UKEY_AUX = 52, WS_UKEY_R_ROW = 53, WS_UKEY_M_ROW = 54, WS_UKEY_DCNT = 55, WS_UKEY_NULL_MULT = 56,
 	WS_UKEY_H_LO = 57, WS_UKEY_H_MULT = 58,
+	// shortest_path_count and all_shortest_paths (pgq_allshortest.cu): behind each batch's levels, the path counts
+	// sigma [n_ab][L] int64 (with WS_LEVEL, which the driver keeps), the batch counters, the step-ordered in-lists
+	// (built once per all_shortest_paths call: sorted keys and in-CSR positions, each with the sort's second buffer),
+	// and the per-row results the entry points return: counts and list lengths in WS_AS_COUNT / WS_AS_PATH_LEN, the
+	// number of lists in WS_AS_NPATHS (their element counts and offsets are shortestpath's WS_OUT_LENGTHS and
+	// WS_OUT_OFFSETS).
+	WS_AS_SIGMA = 59, WS_AS_COUNTERS = 60, WS_AS_STEP_KEY_A = 61, WS_AS_STEP_KEY_B = 62, WS_AS_STEP_POS_A = 63,
+	WS_AS_STEP_POS_B = 64, WS_AS_COUNT = 65, WS_AS_NPATHS = 66, WS_AS_PATH_LEN = 67,
 	WS_SLOTS // (the last block holds the highest numbers)
 };
 
@@ -141,7 +149,8 @@ enum WsSlot : int {
 constexpr int ws_masks[] = {WS_SEEN, WS_VISIT_A, WS_VISIT_B};
 constexpr int ws_radix[] = {WS_RADIX_HIST, WS_RADIX_SCAN};
 constexpr int ws_staging[] = {WS_IN_SRC, WS_IN_DST, WS_IN_VALID, WS_OUT_LEN, WS_OUT_VALID, WS_OUT_OFFSETS,
-                              WS_IN_DST_VALID, WS_OUT_LENGTHS, WS_OUT_PATH_OFFSETS, WS_OUT_PATH_VALID};
+                              WS_IN_DST_VALID, WS_OUT_LENGTHS, WS_OUT_PATH_OFFSETS, WS_OUT_PATH_VALID, WS_AS_COUNT,
+                              WS_AS_NPATHS, WS_AS_PATH_LEN};
 constexpr int ws_driver[] = {WS_ROW_LANE, WS_STATUS, WS_LEVEL, WS_ITEMS_A, WS_ITEMS_B, WS_TLIST, WS_TBITS, WS_WALK,
                              WS_ELEMS, WS_SLOT_OFF, WS_PSRC, WS_PDST, WS_SATBITS, WS_SHARED_ROWS, WS_LANE_SRC,
                              WS_ASSIGN_TMP, WS_BATCH_ROWS, WS_PATH_TOTAL, WS_SEEN_D, WS_VISIT_A_D, WS_VISIT_B_D,
@@ -152,6 +161,8 @@ constexpr int ws_csr[] = {WS_CSR_SCAN, WS_CSR_ERR, WS_CSR_FLAGS, WS_CSR_WIDE, WS
 constexpr int ws_bf[] = {WS_BF_DIST, WS_BF_DIRTY, WS_BF_FLAGS};
 constexpr int ws_cp[] = {WS_CP_LEVEL, WS_CP_PKEY, WS_CP_FRONTIER, WS_CP_LANE_TGT, WS_CP_COUNTERS, WS_ELEMS,
                          WS_PATH_TOTAL};
+constexpr int ws_as[] = {WS_AS_SIGMA, WS_AS_COUNTERS, WS_AS_STEP_KEY_A, WS_AS_STEP_KEY_B, WS_AS_STEP_POS_A,
+                         WS_AS_STEP_POS_B};
 constexpr int ws_analytics[] = {WS_LCC_SRC, WS_LCC_OUT, WS_LCC_OUT_VALID, WS_LCC_BIG_ROWS, WS_LCC_BIG_CNT,
                                 WS_LCC_SRC_VALID, WS_LCC_BITMAP, WS_AN_REF_OFF, WS_AN_SCAN, WS_PR_KEY_A, WS_PR_KEY_B,
                                 WS_PR_VAL_A, WS_PR_VAL_B, WS_PR_IN_OFF, WS_PR_SCAN, WS_PR_DFLAG, WS_PR_RANK,
@@ -179,11 +190,13 @@ template <size_t A, size_t... B>
 constexpr bool ws_apart(const int (&a)[A], const int (&...b)[B]) {
 	return (ws_disjoint(a, b) && ...);
 }
-static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_cp, ws_analytics, ws_keys,
+static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_cp, ws_as, ws_analytics, ws_keys,
                        ws_key_staging),
               "only the BFS drivers may write the search masks");
 static_assert(ws_apart(ws_staging, ws_driver, ws_bf), "a path entry point's staged columns live while its driver runs");
 static_assert(ws_apart(ws_cp, ws_staging, ws_bf), "the tight search runs on the distances and columns of its call");
+static_assert(ws_apart(ws_as, ws_staging, ws_driver, ws_radix),
+              "path counts and step lists live across the batches of their driver, over the columns of their call");
 static_assert(WS_OUT_PATH_OFFSETS < WS_SLOTS && WS_OUT_PATH_VALID < WS_SLOTS, "every slot has a buffer");
 static_assert(ws_apart(ws_radix, ws_csr, ws_analytics, ws_keys), "radix_sort_pairs' scratch is apart from its callers'");
 static_assert(ws_apart(ws_key_staging, ws_keys, ws_csr, ws_radix), "a key build's staged columns live while it builds");
@@ -330,6 +343,30 @@ struct WsGuard {
 };
 
 // ---- BFS drivers implemented in pgq_bfs.cu -----------------------------------------------------
+// One batch of a path-mode BFS call, as the driver hands it to a PathHook behind the batch's last level, while its
+// level array is live.  The sources' levels are 0 again (k_path_fix_sources).
+struct PathBatch {
+	int b0, cnt, L;            // lanes [b0, b0 + cnt) of the call, in a batch L lanes wide
+	int levels;                // BFS levels the batch ran
+	int64_t rows_ub;           // upper bound of the rows on its lanes (> 0)
+	const uint16_t *level;     // [n][L] BFS level of (vertex, lane) in internal ids, 0xFFFF = not reached
+	const int32_t *batch_rows; // the batch's rows, *batch_n (device) of them
+	const int *batch_n;
+	const int32_t *row_lane, *psrc, *pdst; // the call's lane map: lane of each row (-1 = none) and internal ids
+	int64_t *out_lengths;      // [p] element count of each row's lists
+	int64_t *slot_off;         // [p] each row's slot in the walk buffer (WS_WALK)
+	int64_t *walk_bound;       // elements of the walk buffer handed out so far
+	Workspace *ws;
+	cudaStream_t s;
+	pgq_stats *st;
+};
+// What a path-mode call does with each batch instead of shortestpath's walk.  With `lists` set, the batches leave
+// lists in the walk buffer as shortestpath's walk does (a row's element count in out_lengths, its slot in slot_off,
+// the buffer grown by the hook), and the driver places them behind the last batch as it places shortestpath's.
+struct PathHook {
+	bool lists = false;
+	virtual int batch(const PathBatch &b) = 0;
+};
 // shortestpath's list offsets (k_path_offsets, one block): rows [lo, hi) get offsets from `base` on, in row order, from
 // their out_lengths (0 = NULL, -1 = [src] -> 1) and out_valid = length > 0; *d_range_total = the rows' element count
 void pgq_path_offsets(int64_t base, int64_t lo, int64_t hi, int64_t *out_offsets, int64_t *out_lengths,
@@ -341,6 +378,11 @@ int pgq_bfs_paths_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *
                          const uint8_t *d_src_valid, const pgq_options *opts, int64_t *d_out_offsets,
                          int64_t *d_out_lengths, uint8_t *d_out_valid, int64_t **d_out_elems, int64_t *out_total,
                          cudaStream_t stream, pgq_stats *stats);
+// shortestpath's BFS (lane assignment, batches, level loop, path mode) with hook->batch in place of the walk
+int pgq_bfs_paths_hooked(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,
+                         const uint8_t *d_src_valid, const pgq_options *opts, int64_t *d_out_offsets,
+                         int64_t *d_out_lengths, uint8_t *d_out_valid, int64_t **d_out_elems, int64_t *out_total,
+                         PathHook *hook, cudaStream_t stream, pgq_stats *stats);
 // h_src / h_src_valid: host copies of d_src / d_src_valid (PGQ_OPT_REFERENCE_BATCHING cuts the batches on the host)
 int pgq_bfs_reachability_device(pgq_csr *csr, Workspace *ws, int64_t p, const int64_t *d_src, const int64_t *d_dst,
                                 const uint8_t *d_src_valid, const int64_t *h_src, const uint8_t *h_src_valid,

@@ -70,6 +70,8 @@ namespace duckdb {
 static std::mutex g_ctx_lock;
 static pgq_ctx *g_ctx = nullptr;
 static std::atomic<int64_t> g_calls_cheapest_path {0};
+static std::atomic<int64_t> g_calls_path_count {0};
+static std::atomic<int64_t> g_calls_all_shortest {0};
 static std::atomic<int64_t> g_calls_lengths {0}, g_calls_paths {0}, g_calls_cheapest {0}, g_pairs {0}, g_uploads {0},
     g_device_builds {0}, g_chunks {0}, g_materialized {0}, g_calls_lcc {0}, g_calls_pagerank {0}, g_calls_wcc {0},
     g_calls_bidirectional {0}, g_calls_w_type {0}, g_calls_reachability {0};
@@ -854,6 +856,121 @@ static void ShortestPathB200Function(DataChunk &args, ExpressionState &state, Ve
 	duckpgq_state->csr_to_delete.insert(info.csr_id); // shortest_path.cpp:206
 }
 
+// ---- shortest_path_count / all_shortest_paths (no reference function) ----------------------------------------
+// Every shortest path of a row (include/duckpgq_b200.h, pgq_shortest_path_count / pgq_all_shortest_paths), called as
+// raw UDFs over the CSR CTE: the MATCH rewriter stays the reference's, which rejects ALL SHORTEST.  The binds are
+// shortestpath's (IterativeLengthBind: constant id, the mark for deletion); all_shortest_paths' also wants a constant
+// max_paths >= 0 (0 = every path).  The CSR lookups are shortestpath's (shortest_path.cpp:49-57).
+static CSR &ShortestPathCsr(DuckPGQState &duckpgq_state, int32_t csr_id) {
+	auto csr_entry = duckpgq_state.csr_list.find(csr_id);
+	if (csr_entry == duckpgq_state.csr_list.end()) {
+		throw ConstraintException("Invalid ID");
+	}
+	if (!csr_entry->second->initialized_v) {
+		throw ConstraintException("Need to initialize CSR before doing shortest path");
+	}
+	return *csr_entry->second;
+}
+
+static void ShortestPathCountB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
+	auto &info = func_expr.BindInfo()->Cast<IterativeLengthFunctionData>();
+	auto duckpgq_state = GetDuckPGQState(info.context);
+	CSR &csr = ShortestPathCsr(*duckpgq_state, info.csr_id);
+	int64_t v_size = args.data[1].GetValue(0).GetValue<int64_t>();
+	PairColumns pairs(args);
+	idx_t count = args.size();
+	auto device_csr = GetB200State(info.context)->ForPathFunction(info.csr_id, csr, v_size);
+	vector<int64_t> out_count(count);
+	vector<uint8_t> out_valid(count);
+	pgq_options opts = OptionsFromEnv();
+	int st = pgq_shortest_path_count(device_csr, static_cast<int64_t>(count), pairs.src.data(), pairs.dst.data(),
+	                                 pairs.valid.data(), nullptr, &opts, out_count.data(), out_valid.data(), nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_path_count++;
+	g_pairs += static_cast<int64_t>(count);
+	result.SetVectorType(VectorType::FLAT_VECTOR);
+	auto result_data = FlatVector::GetDataMutable<int64_t>(result);
+	ValidityMask &result_validity = FlatVector::ValidityMutable(result);
+	for (idx_t i = 0; i < count; i++) {
+		result_data[i] = out_count[i];
+		if (!out_valid[i]) {
+			result_validity.SetInvalid(i);
+		}
+	}
+	duckpgq_state->csr_to_delete.insert(info.csr_id);
+}
+
+static unique_ptr<FunctionData> AllShortestPathsBind(BindScalarFunctionInput &input) {
+	auto &arguments = input.GetArguments();
+	if (!arguments[4]->IsFoldable()) {
+		throw InvalidInputException("max_paths must be constant.");
+	}
+	auto max_paths = ExpressionExecutor::EvaluateScalar(input.GetClientContext(), *arguments[4]);
+	if (max_paths.IsNull() || max_paths.GetValue<int64_t>() < 0) {
+		throw InvalidInputException("max_paths must be 0 (every path) or more.");
+	}
+	return IterativeLengthFunctionData::IterativeLengthBind(input);
+}
+
+static void AllShortestPathsB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
+	auto &info = func_expr.BindInfo()->Cast<IterativeLengthFunctionData>();
+	auto duckpgq_state = GetDuckPGQState(info.context);
+	CSR &csr = ShortestPathCsr(*duckpgq_state, info.csr_id);
+	int64_t v_size = args.data[1].GetValue(0).GetValue<int64_t>();
+	int64_t max_paths = args.data[4].GetValue(0).GetValue<int64_t>(); // (constant: AllShortestPathsBind)
+	PairColumns pairs(args);
+	idx_t count = args.size();
+	auto device_csr = GetB200State(info.context)->ForPathFunction(info.csr_id, csr, v_size);
+	vector<int64_t> out_count(count), npaths(count), path_len(count), offsets(count);
+	vector<uint8_t> out_valid(count);
+	int64_t *elems = nullptr;
+	int64_t total = 0;
+	pgq_options opts = OptionsFromEnv();
+	int st = pgq_all_shortest_paths(device_csr, static_cast<int64_t>(count), pairs.src.data(), pairs.dst.data(),
+	                                pairs.valid.data(), nullptr, &opts, max_paths, out_count.data(), npaths.data(),
+	                                path_len.data(), offsets.data(), out_valid.data(), &elems, &total, nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_all_shortest++;
+	g_pairs += static_cast<int64_t>(count);
+	idx_t lists = 0;
+	for (idx_t i = 0; i < count; i++) {
+		lists += static_cast<idx_t>(npaths[i]);
+	}
+	result.SetVectorType(VectorType::FLAT_VECTOR);
+	auto result_data = FlatVector::GetDataMutable<list_entry_t>(result);
+	ValidityMask &result_validity = FlatVector::ValidityMutable(result);
+	ListVector::Reserve(result, lists);
+	auto &inner = ListVector::GetChildMutable(result);
+	ListVector::Reserve(inner, static_cast<idx_t>(total));
+	if (total > 0) {
+		auto leaf = FlatVector::GetDataMutable<int64_t>(ListVector::GetChildMutable(inner));
+		memcpy(leaf, elems, static_cast<size_t>(total) * sizeof(int64_t));
+	}
+	ListVector::SetListSize(inner, static_cast<idx_t>(total));
+	pgq_free(elems);
+	auto inner_data = FlatVector::GetDataMutable<list_entry_t>(inner);
+	idx_t li = 0;
+	for (idx_t i = 0; i < count; i++) {
+		result_data[i].offset = li;
+		result_data[i].length = static_cast<idx_t>(npaths[i]);
+		for (int64_t k = 0; k < npaths[i]; k++, li++) {
+			inner_data[li].offset = static_cast<idx_t>(offsets[i] + k * path_len[i]);
+			inner_data[li].length = static_cast<idx_t>(path_len[i]);
+		}
+		if (!out_valid[i]) {
+			result_validity.SetInvalid(i);
+		}
+	}
+	ListVector::SetListSize(result, lists);
+	duckpgq_state->csr_to_delete.insert(info.csr_id);
+}
+
 // ---- cheapest_path_length -------------------------------------------------------------------------------
 // cheapest_path_length.cpp:138-160: batched Bellman-Ford over the weighted CSR, BIGINT or DOUBLE result as
 // the bind decided (cheapest_path_length_function_data.cpp:26-30).  The bind stays the reference's.
@@ -1096,7 +1213,9 @@ static void B200StatsFunction(DataChunk &args, ExpressionState &state, Vector &r
 	              ",iterativelengthbidirectional_calls=" + std::to_string(g_calls_bidirectional.load()) +
 	              ",csr_get_w_type_calls=" + std::to_string(g_calls_w_type.load()) +
 	              ",reachability_calls=" + std::to_string(g_calls_reachability.load()) +
-	              ",cheapest_path_calls=" + std::to_string(g_calls_cheapest_path.load());
+	              ",cheapest_path_calls=" + std::to_string(g_calls_cheapest_path.load()) +
+	              ",shortest_path_count_calls=" + std::to_string(g_calls_path_count.load()) +
+	              ",all_shortest_paths_calls=" + std::to_string(g_calls_all_shortest.load());
 	result.SetVectorType(VectorType::CONSTANT_VECTOR);
 	ConstantVector::GetData<string_t>(result)[0] = StringVector::AddString(result, text);
 }
@@ -1202,6 +1321,15 @@ static void LoadInternal(ExtensionLoader &loader) {
 	loader.RegisterFunction(ScalarFunction(
 	    "cheapest_path", {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
 	    LogicalType::LIST(LogicalType::BIGINT), CheapestPathB200Function, CheapestPathBind));
+	// shortest_path_count / all_shortest_paths: no reference function is replaced; raw UDFs over the CSR CTE (the
+	// reference's MATCH rewriter rejects ALL SHORTEST)
+	loader.RegisterFunction(ScalarFunction(
+	    "shortest_path_count", {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
+	    LogicalType::BIGINT, ShortestPathCountB200Function, IterativeLengthFunctionData::IterativeLengthBind));
+	loader.RegisterFunction(ScalarFunction(
+	    "all_shortest_paths",
+	    {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
+	    LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT)), AllShortestPathsB200Function, AllShortestPathsBind));
 	ScalarFunction stats("duckpgq_b200_stats", {}, LogicalType::VARCHAR, B200StatsFunction);
 	stats.SetVolatile();
 	loader.RegisterFunction(stats);

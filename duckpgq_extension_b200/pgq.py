@@ -8,6 +8,8 @@ like the reference's own sqllogictests:
     iterativelength(id, v_size, src, dst)                             iterativelength.cpp:34-152
     shortestpath(id, v_size, src, dst)                                shortest_path.cpp:43-217
     cheapest_path(id, v_size, src, dst)                               (no reference function: the cheapest path's list)
+    shortest_path_count(id, v_size, src, dst)                         (no reference function: ALL SHORTEST's count)
+    all_shortest_paths(id, v_size, src, dst, max_paths)               (no reference function: ALL SHORTEST's lists)
     delete_csr(id)                                                    csr_deletion.cpp:10-29
     DuckPGQState.{csr_list, csr_to_delete, get_csr, query_end}        duckpgq_state.hpp:12-39, duckpgq_state.cpp:162-186
 
@@ -424,6 +426,50 @@ class DeviceCSR:
         paths = [flat[offs[i]: offs[i] + lens[i]].tolist() if ov[i] else None for i in range(p)]
         return paths, st.as_dict()
 
+    def shortest_path_count(self, src, dst, src_valid=None, dst_valid=None, options: Optional[Options] = None):
+        """-> (counts int64, valid uint8, stats dict): the number of shortest paths of each row, saturated at
+        INT64_MAX, 0 under NULL (include/duckpgq_b200.h, pgq_shortest_path_count)."""
+        src, dst = _i64(src), _i64(dst)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        dv = None if dst_valid is None else np.ascontiguousarray(dst_valid, dtype=np.uint8)
+        cnt = np.zeros(max(p, 1), dtype=np.int64)
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        st = _native.PgqStats()
+        opts = (options or Options()).c()
+        _check(self._lib.pgq_shortest_path_count(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv), C.byref(opts),
+                                                 _p64(cnt), _pu8(ov), C.byref(st)))
+        return cnt[:p], ov[:p], st.as_dict()
+
+    def all_shortest_paths(self, src, dst, max_paths: int = 0, src_valid=None, dst_valid=None,
+                           options: Optional[Options] = None):
+        """-> (per row: list of [src, e1, v1, ..., dst] lists or None, counts int64, stats dict): the first
+        min(count, max_paths) shortest paths of each row in step order, all of them for max_paths = 0
+        (include/duckpgq_b200.h, pgq_all_shortest_paths)."""
+        src, dst = _i64(src), _i64(dst)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        dv = None if dst_valid is None else np.ascontiguousarray(dst_valid, dtype=np.uint8)
+        cnt = np.zeros(max(p, 1), dtype=np.int64)
+        npaths = np.zeros(max(p, 1), dtype=np.int64)
+        plen = np.zeros(max(p, 1), dtype=np.int64)
+        offs = np.zeros(max(p, 1), dtype=np.int64)
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        elems = C.POINTER(C.c_int64)()
+        total = C.c_int64(0)
+        st = _native.PgqStats()
+        opts = (options or Options()).c()
+        _check(self._lib.pgq_all_shortest_paths(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv), C.byref(opts),
+                                                int(max_paths), _p64(cnt), _p64(npaths), _p64(plen), _p64(offs),
+                                                _pu8(ov), C.byref(elems), C.byref(total), C.byref(st)))
+        try:  # (no rows: no element array)
+            flat = np.ctypeslib.as_array(elems, shape=(total.value,)).copy() if elems else np.zeros(0, np.int64)
+        finally:
+            self._lib.pgq_free(elems)
+        paths = [flat[offs[i]: offs[i] + npaths[i] * plen[i]].reshape(npaths[i], plen[i]).tolist() if ov[i] else None
+                 for i in range(p)]
+        return paths, cnt[:p], st.as_dict()
+
     def free(self):
         if getattr(self, "_h", None):
             self._lib.pgq_csr_free(self._h)
@@ -618,6 +664,31 @@ def shortestpath(state: DuckPGQState, csr_id: int, v_size: int, src, dst, src_va
         raise InvalidInputException(PGQ_ERR_INVALID_ARG, f"v_size {v_size} does not match the CSR ({csr.n} vertices)")
     paths, _ = csr.shortestpath(src, dst, src_valid, options)
     state.csr_to_delete.add(csr_id)  # shortest_path.cpp:206
+    return paths
+
+
+def shortest_path_count(state: DuckPGQState, csr_id: int, v_size: int, src, dst, src_valid=None, dst_valid=None,
+                        options: Optional[Options] = None):
+    """shortest_path_count(INT, BIGINT, BIGINT, BIGINT) -> BIGINT: the number of shortest paths, saturated at
+    INT64_MAX (no reference function; looked up and marked as shortestpath is).  Returns (counts, valid)."""
+    csr = _lookup_for_path(state, csr_id, lengths=False)
+    if int(v_size) != csr.n:
+        raise InvalidInputException(PGQ_ERR_INVALID_ARG, f"v_size {v_size} does not match the CSR ({csr.n} vertices)")
+    counts, valid, _ = csr.shortest_path_count(src, dst, src_valid, dst_valid, options)
+    state.csr_to_delete.add(csr_id)
+    return counts, valid
+
+
+def all_shortest_paths(state: DuckPGQState, csr_id: int, v_size: int, src, dst, max_paths: int = 0, src_valid=None,
+                       dst_valid=None, options: Optional[Options] = None):
+    """all_shortest_paths(INT, BIGINT, BIGINT, BIGINT, BIGINT max_paths) -> LIST(LIST(BIGINT)): per row the first
+    min(count, max_paths) shortest paths (every one for max_paths = 0) or None (no reference function; looked up and
+    marked as shortestpath is)."""
+    csr = _lookup_for_path(state, csr_id, lengths=False)
+    if int(v_size) != csr.n:
+        raise InvalidInputException(PGQ_ERR_INVALID_ARG, f"v_size {v_size} does not match the CSR ({csr.n} vertices)")
+    paths, _, _ = csr.all_shortest_paths(src, dst, max_paths, src_valid, dst_valid, options)
+    state.csr_to_delete.add(csr_id)
     return paths
 
 

@@ -300,6 +300,41 @@ int pgq_cheapest_path(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const i
                       const uint8_t *dst_valid, int64_t *out_offsets, int64_t *out_lengths, uint8_t *out_valid,
                       int64_t **out_elems, int64_t *out_total, pgq_stats *stats);
 
+/* pgq_shortest_path_count / pgq_all_shortest_paths: every shortest path of a row (SQL/PGQ's ALL SHORTEST, which the
+ * reference rejects).  No reference function.  For a row (s, t) with h = the BFS depth of t from s along out-edges:
+ *   - a shortest path is any list [s, e1, v1, ..., eh, t] of h edges along out-edges, in pgq_shortestpath's format
+ *     (vertex rowids; edge rowids from the CSR's edge ids, CSR positions when it was uploaded without ids).  Parallel
+ *     edges give distinct paths (so does an edge rowid that a duplicated source key of pgq_csr_build_keys put into
+ *     several adjacencies).
+ *   - count = the number of such lists = (A^h)[s, t], A the adjacency matrix with edge multiplicities; exact up to
+ *     INT64_MAX, which it saturates at ("at least INT64_MAX").  s == t -> count 1, the one path [s].
+ *   - NULL (out_valid 0, count 0): a NULL source or destination (src_valid / dst_valid, both nullable), or t not
+ *     reachable.  Ids outside [0, n) of a row whose ids are both valid -> PGQ_ERR_RANGE; a missing or unfinalised CSR ->
+ *     pgq_shortestpath's errors; a depth beyond path mode's limit (65533) -> PGQ_ERR_UNSUPPORTED.
+ *   - the order of the paths: walking back from t, a step is (the parent one level closer to s, the edge's position in
+ *     the parent's adjacency as pgq_csr_download returns it), steps compared by the parent's ORIGINAL id first, then by
+ *     the position; paths ordered lexicographically by their steps from t back to s.  Path 0 is pgq_shortestpath's.
+ *   - opts (nullable): lanes, direction, alpha and flags as for pgq_shortestpath (a flag never changes a result);
+ *     shard_count > 1 -> PGQ_ERR_UNSUPPORTED.  The rows run exactly as pgq_shortestpath runs them, a NULL destination
+ *     counting as a NULL source; its BFS counters (batches, levels, edges_traversed, frontier_vertices, push_levels,
+ *     pull_levels, lanes, searches, pruned, search_rows) are pgq_shortestpath's for the same rows when no destination
+ *     is NULL.  kernel_launches and total_ms include the path counts and lists (not the launches inside the step-list
+ *     sort of pgq_all_shortest_paths).
+ * pgq_all_shortest_paths also returns the paths: row i has out_npaths[i] = min(count, max_paths) lists (all of them for
+ * max_paths == 0), the first in the order above, each of out_path_len[i] = 2h + 1 elements, back to back from
+ * (*out_elems)[out_offsets[i]] (rows in row order; a NULL row has none).  *out_elems is allocated by the library:
+ * release with pgq_free().  max_paths < 0 -> PGQ_ERR_INVALID_ARG; max_paths == 0 with a saturated count ->
+ * PGQ_ERR_UNSUPPORTED; an element total that overflows int64 or cannot be allocated -> PGQ_ERR_OOM (checked before it
+ * is allocated).  Ranks stay exact when counts saturate: every rank listed is below INT64_MAX. */
+int pgq_shortest_path_count(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const int64_t *dst,
+                            const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
+                            int64_t *out_count, uint8_t *out_valid, pgq_stats *stats);
+int pgq_all_shortest_paths(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const int64_t *dst,
+                           const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
+                           int64_t max_paths, int64_t *out_count, int64_t *out_npaths, int64_t *out_path_len,
+                           int64_t *out_offsets, uint8_t *out_valid, int64_t **out_elems, int64_t *out_total,
+                           pgq_stats *stats);
+
 /* ---- the other consumers of the CSR ------------------------------------------------------------------------
  * Host pointers in and out.  As in the reference, "v_size" is n + 2: the two entries n and n + 1 behind the
  * vertices have no edges and take part where the reference lets them.  Results are bit-identical to the reference's.
