@@ -16,9 +16,9 @@ CSRC = os.path.join(_PKG, "csrc")
 INCLUDE = os.path.join(ROOT, "include")
 LIB_DIR = os.path.join(_PKG, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libduckpgq_b200.so")
-SOURCES = ["pgq_csr.cu", "pgq_bfs.cu", "pgq_api.cu", "pgq_cheapest.cu", "pgq_allshortest.cu", "pgq_multi.cu",
-           "pgq_analytics.cu"]
-HEADERS = ["pgq_internal.h", "pgq_tile.cuh", "pgq_pull.cuh"]
+SOURCES = ["pgq_csr.cu", "pgq_bfs.cu", "pgq_api.cu", "pgq_cheapest.cu", "pgq_allshortest.cu", "pgq_kshortest.cu",
+           "pgq_multi.cu", "pgq_analytics.cu"]
+HEADERS = ["pgq_internal.h", "pgq_tile.cuh", "pgq_pull.cuh", "pgq_count.cuh"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -119,6 +119,8 @@ SYMBOLS = {
                                           C.POINTER(PgqStats)]),
     "pgq_all_shortest_paths": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, C.c_int64, _P64, _P64, _P64, _P64,
                                          _PU8, C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
+    "pgq_shortest_k_paths": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, C.c_int64, _P64, _P64, _PU8,
+                                       C.POINTER(_P64), C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
     "pgq_local_clustering_coefficient": (C.c_int, [_VP, C.c_int64, _P64, _PU8, C.POINTER(C.c_float), _PU8,
                                                    C.POINTER(PgqStats)]),
     "pgq_pagerank": (C.c_int, [_VP, C.c_int64, _P64, _PU8, C.POINTER(C.c_double), _PU8, _P64, C.POINTER(PgqStats)]),

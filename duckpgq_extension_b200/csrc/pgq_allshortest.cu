@@ -39,29 +39,14 @@
 #include <cstring>
 #include <vector>
 
+#include "pgq_count.cuh"
 #include "pgq_tile.cuh"
 
-#define AS_MAX 0x7fffffffffffffffull
 #define AS_UNSET 0xFFFFu // level of a vertex the lane has not reached
 
 // The batch counters a hook brings back: [0] K, the largest target level of the batch's rows; [1] the call's running
 // element total (saturating); [2] a row with max_paths = 0 saturated its count.
 enum { AS_K = 0, AS_TOTAL = 1, AS_SATURATED = 2 };
-
-__device__ __forceinline__ u64 sat_add(u64 a, u64 b) { // a, b <= INT64_MAX
-	const u64 s = a + b;
-	return s > AS_MAX ? AS_MAX : s;
-}
-
-// *a = sat_add(*a, v); returns the old value
-__device__ __forceinline__ u64 atomic_sat_add(u64 *a, u64 v) {
-	u64 old = *reinterpret_cast<volatile u64 *>(a), assumed;
-	do {
-		assumed = old;
-		old = atomicCAS(a, assumed, sat_add(assumed, v));
-	} while (old != assumed);
-	return old;
-}
 
 // count = lists = list length = 1 for the rows with a valid source and s == t, 0 for the others (the rows on a lane
 // are overwritten by their batch)
@@ -320,8 +305,8 @@ struct AllShortest : PathHook {
 };
 
 // The step lists of the CSR (k_as_step_keys + radix_sort_pairs) into the workspace
-static int build_step_lists(pgq_csr *csr, Workspace *ws, cudaStream_t s, const u64 **keys, const int32_t **pos,
-                            int64_t *launches) {
+int build_step_lists(pgq_csr *csr, Workspace *ws, cudaStream_t s, const u64 **keys, const int32_t **pos,
+                     int64_t *launches) {
 	const int64_t n = csr->n, m = csr->m;
 	const size_t cells = (size_t)std::max<int64_t>(m, 1);
 	uint64_t *ka, *kb;

@@ -142,6 +142,16 @@ enum WsSlot : int {
 	// WS_OUT_OFFSETS).
 	WS_AS_SIGMA = 59, WS_AS_COUNTERS = 60, WS_AS_STEP_KEY_A = 61, WS_AS_STEP_KEY_B = 62, WS_AS_STEP_POS_A = 63,
 	WS_AS_STEP_POS_B = 64, WS_AS_COUNT = 65, WS_AS_NPATHS = 66, WS_AS_PATH_LEN = 67,
+	// shortest_k_paths (pgq_kshortest.cu), which also reads all_shortest_paths' step lists: each lane's row and internal
+	// ids; a batch's backward reach (reach, frontier and next-frontier masks [n][W / 64]); its two rolling count layers
+	// [n_ab][W], each lane's running total, alive flag and counting bit, the call's counters; per row the walks, their
+	// elements, the last walk's length, the first walk and the first element; a storing group's lanes, their sources
+	// and its layers; and the walks' offsets, their elements and the scans' total.
+	WS_KS_LANE_ROW = 68, WS_KS_PSRC = 69, WS_KS_PDST = 70, WS_KS_REACH = 71, WS_KS_FRONT = 72, WS_KS_NEXT = 73,
+	WS_KS_OMEGA_A = 74, WS_KS_OMEGA_B = 75, WS_KS_TOTAL = 76, WS_KS_ALIVE = 77, WS_KS_ACTIVE = 78, WS_KS_COUNTERS = 79,
+	WS_KS_NPATHS = 80, WS_KS_ROW_ELEMS = 81, WS_KS_LAST = 82, WS_KS_FIRST = 83, WS_KS_ELEM_OFF = 84,
+	WS_KS_GROUP_LANE = 85, WS_KS_GROUP_SRC = 86, WS_KS_LAYERS = 87, WS_KS_WALK_OFF = 88, WS_KS_ELEMS = 89,
+	WS_KS_SCAN_TOTAL = 90,
 	WS_SLOTS // (the last block holds the highest numbers)
 };
 
@@ -163,6 +173,10 @@ constexpr int ws_cp[] = {WS_CP_LEVEL, WS_CP_PKEY, WS_CP_FRONTIER, WS_CP_LANE_TGT
                          WS_PATH_TOTAL};
 constexpr int ws_as[] = {WS_AS_SIGMA, WS_AS_COUNTERS, WS_AS_STEP_KEY_A, WS_AS_STEP_KEY_B, WS_AS_STEP_POS_A,
                          WS_AS_STEP_POS_B};
+constexpr int ws_ks[] = {WS_KS_LANE_ROW, WS_KS_PSRC, WS_KS_PDST, WS_KS_REACH, WS_KS_FRONT, WS_KS_NEXT, WS_KS_OMEGA_A,
+                         WS_KS_OMEGA_B, WS_KS_TOTAL, WS_KS_ALIVE, WS_KS_ACTIVE, WS_KS_COUNTERS, WS_KS_NPATHS,
+                         WS_KS_ROW_ELEMS, WS_KS_LAST, WS_KS_FIRST, WS_KS_ELEM_OFF, WS_KS_GROUP_LANE, WS_KS_GROUP_SRC,
+                         WS_KS_LAYERS, WS_KS_WALK_OFF, WS_KS_ELEMS, WS_KS_SCAN_TOTAL};
 constexpr int ws_analytics[] = {WS_LCC_SRC, WS_LCC_OUT, WS_LCC_OUT_VALID, WS_LCC_BIG_ROWS, WS_LCC_BIG_CNT,
                                 WS_LCC_SRC_VALID, WS_LCC_BITMAP, WS_AN_REF_OFF, WS_AN_SCAN, WS_PR_KEY_A, WS_PR_KEY_B,
                                 WS_PR_VAL_A, WS_PR_VAL_B, WS_PR_IN_OFF, WS_PR_SCAN, WS_PR_DFLAG, WS_PR_RANK,
@@ -190,13 +204,15 @@ template <size_t A, size_t... B>
 constexpr bool ws_apart(const int (&a)[A], const int (&...b)[B]) {
 	return (ws_disjoint(a, b) && ...);
 }
-static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_cp, ws_as, ws_analytics, ws_keys,
-                       ws_key_staging),
+static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_cp, ws_as, ws_ks, ws_analytics,
+                       ws_keys, ws_key_staging),
               "only the BFS drivers may write the search masks");
 static_assert(ws_apart(ws_staging, ws_driver, ws_bf), "a path entry point's staged columns live while its driver runs");
 static_assert(ws_apart(ws_cp, ws_staging, ws_bf), "the tight search runs on the distances and columns of its call");
 static_assert(ws_apart(ws_as, ws_staging, ws_driver, ws_radix),
               "path counts and step lists live across the batches of their driver, over the columns of their call");
+static_assert(ws_apart(ws_ks, ws_staging, ws_driver, ws_radix, ws_as),
+              "the walk search lives across its batches and groups, over the columns of its call and the step lists");
 static_assert(WS_OUT_PATH_OFFSETS < WS_SLOTS && WS_OUT_PATH_VALID < WS_SLOTS, "every slot has a buffer");
 static_assert(ws_apart(ws_radix, ws_csr, ws_analytics, ws_keys), "radix_sort_pairs' scratch is apart from its callers'");
 static_assert(ws_apart(ws_key_staging, ws_keys, ws_csr, ws_radix), "a key build's staged columns live while it builds");

@@ -1,0 +1,696 @@
+// pgq_kshortest.cu -- shortest_k_paths on the device CSR: the k shortest walks of a row (SQL/PGQ's SHORTEST k, which
+// the reference parses and rejects).  No reference function.  sm_90a only.
+//
+// A lane is a row: the rows whose ids are both valid take lanes in input order, W per batch, with no source
+// de-duplication, so that a row's answer never depends on the other rows of its batch.  Four phases:
+//   * backward reach.  B(t), the vertices that reach the lane's target t (t included), as a W-bit mask per vertex: a
+//     multi-lane BFS from the batch's targets over the in-CSC (k_ks_reach_level pushes each frontier bit from a vertex
+//     to its in-neighbours, a thread per in-edge; k_ks_reach_update folds the level in), until a level adds no bit.
+//     s outside B(t) makes the row NULL.  It has masks of its own: the BFS drivers' WS_SEEN / WS_VISIT_* keep their
+//     known-zero record.
+//   * counting pass.  w_h(u, l), the number of h-edge walks from the lane's source s to u, kept only for u in B(t):
+//     w_0 is 1 at s (not stored), w_h(u) = the saturating sum of w_{h-1}(v) over the in-edges v -> u, and every vertex
+//     of a level >= 1 has an in-edge, so layers have n_ab rows.  Two rolling layers [n_ab][L].  k_ks_omega pulls over
+//     the in-CSC in chunks of KS_CHUNK edge positions, a warp per chunk and a thread per lane: a vertex whose in-list
+//     lies inside one chunk is summed by one warp and stored, a longer one (an R-MAT hub) is split over the chunks it
+//     spans, each adding its partial sum with atomic_sat_add.  Saturating addition of non-negative values is
+//     associative, so neither the split nor the order changes a count.  A thread skips the rows outside its lane's
+//     B(t) and the lanes that stopped.  k_ks_step then reads each lane's count at t, takes min(count, k - total)
+//     walks of that length and stops the lane after the layer where its total reaches k or where w_h is zero on all
+//     of B(t).  The second test is exact: a non-zero w at a vertex that reaches t means a longer walk to t exists.  It
+//     is what ends the loop; without the restriction to B(t) a self-loop that s reaches but that does not reach t
+//     would keep w alive forever.
+//   * storing pass.  The rows with walks, packed greedily in lane order into groups of at most W rows whose layers
+//     (H + 1) x n_ab x rows x 8 B fit the layer budget (H the group's longest walk), recompute w_1 .. w_H with the
+//     same kernel, every layer kept.  No restriction there: H bounds the loop, and w is the same on B(t) with or
+//     without it (every in-neighbour of a vertex of B(t) is in B(t)), which is all the unranking reads.
+//   * unranking.  k_ks_unrank gives each listed walk a warp.  Walk r of a row finds its length h by a saturating
+//     prefix sum of the row's counts at t over h = 0 .. H and its rank within that length, then walks back from t:
+//     at node u with j steps left it scans u's step list (build_step_lists, shared with all_shortest_paths) with a
+//     saturating prefix sum of w_{j-1}(parent) and takes the first edge whose prefix exceeds the rank, subtracting the
+//     prefix before it.  Ranks stay exact under saturation by all_shortest_paths' argument: every rank is below k.
+//     Element offsets: each row's element base is an exclusive scan of the rows' element counts (pgq_path_offsets),
+//     and the walk adds the elements of the shorter walks of its row and of its rank's predecessors.
+#include <algorithm>
+#include <cstdlib>
+#include <cstring>
+#include <vector>
+
+#include "pgq_count.cuh"
+#include "pgq_tile.cuh"
+
+#define KS_CHUNK 128        // in-CSC positions per warp of k_ks_omega
+#define KS_WALK_MAX 65533   // the longest walk a result may hold (all_shortest_paths' depth limit)
+#define KS_BUDGET ((int64_t)4 << 30)
+
+// The call's counters: [0] a backward level added a bit; [1] lanes still counting; [2] a lane needs a walk longer than
+// KS_WALK_MAX
+enum { KS_CHANGED = 0, KS_ACTIVE = 1, KS_TOO_LONG = 2 };
+
+__device__ __forceinline__ u64 sat_mul_len(u64 c, int64_t len) { // c <= INT64_MAX, len >= 1
+	return c > AS_MAX / (u64)len ? AS_MAX : c * (u64)len;
+}
+
+// the largest row u < n_ab with in_off[u] <= e (rows below n_ab have in-edges, so their offsets rise strictly)
+__device__ __forceinline__ int64_t ks_row_of(const int32_t *__restrict__ in_off, int64_t n_ab, int64_t e) {
+	int64_t lo = 0, hi = n_ab - 1;
+	while (lo < hi) {
+		const int64_t mid = (lo + hi + 1) >> 1;
+		if (in_off[mid] <= e) {
+			lo = mid;
+		} else {
+			hi = mid - 1;
+		}
+	}
+	return lo;
+}
+
+// internal ids of the lanes' sources and targets
+__global__ void k_ks_lanes(int64_t lanes, const int32_t *__restrict__ lane_row, const int64_t *__restrict__ src,
+                           const int64_t *__restrict__ dst, const int32_t *__restrict__ perm, int32_t *psrc,
+                           int32_t *pdst) {
+	for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < lanes; i += (int64_t)gridDim.x * blockDim.x) {
+		const int row = lane_row[i];
+		psrc[i] = perm[src[row]];
+		pdst[i] = perm[dst[row]];
+	}
+}
+
+// level 0 of the backward reach: each lane's target
+__global__ void k_ks_reach_seed(int cnt, int wd, const int32_t *__restrict__ pdst, u64 *reach, u64 *front) {
+	for (int l = blockIdx.x * blockDim.x + threadIdx.x; l < cnt; l += gridDim.x * blockDim.x) {
+		const int64_t cell = (int64_t)pdst[l] * wd + (l >> 6);
+		atomicOr(&reach[cell], 1ull << (l & 63));
+		atomicOr(&front[cell], 1ull << (l & 63));
+	}
+}
+
+// one backward level: every in-edge u -> v of a frontier vertex v passes v's new lanes on to u.  A thread per in-CSC
+// position; a warp finds the row of its first position by bisection and each thread walks on from there.
+__global__ void __launch_bounds__(256) k_ks_reach_level(int64_t m, int64_t n_ab, int wd, const int32_t *__restrict__ in_off,
+                                                        const int32_t *__restrict__ in_adj, const u64 *__restrict__ front,
+                                                        const u64 *__restrict__ reach, u64 *next) {
+	const int lane = threadIdx.x & 31;
+	const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+	for (int64_t base = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 32; base < m; base += nwarps * 32) {
+		int64_t v = ks_row_of(in_off, n_ab, base);
+		const int64_t e = base + lane;
+		if (e >= m) {
+			continue;
+		}
+		while (in_off[v + 1] <= e) {
+			v++;
+		}
+		const int64_t u = in_adj[e];
+		for (int j = 0; j < wd; j++) {
+			const u64 f = front[v * wd + j];
+			if (f) {
+				const u64 nb = f & ~reach[u * wd + j];
+				if (nb) {
+					atomicOr(&next[u * wd + j], nb);
+				}
+			}
+		}
+	}
+}
+
+// folds a backward level in: the new bits become the frontier and join the reach
+__global__ void k_ks_reach_update(int64_t cells, u64 *reach, u64 *front, u64 *next, u64 *ctr) {
+	bool any = false;
+	for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (int64_t)gridDim.x * blockDim.x) {
+		const u64 nw = next[i] & ~reach[i];
+		reach[i] |= nw;
+		front[i] = nw;
+		next[i] = 0;
+		any |= nw != 0;
+	}
+	if (__any_sync(FULL_MASK, any) && (threadIdx.x & 31) == 0) {
+		ctr[KS_CHANGED] = 1;
+	}
+}
+
+// layer 0 of each lane: NULL when s is outside B(t); the walk [s] when s == t; the lane counts on while its total is
+// below k
+__global__ void k_ks_start(int cnt, int wd, int64_t k, const int32_t *__restrict__ lane_row,
+                           const int32_t *__restrict__ psrc, const int32_t *__restrict__ pdst,
+                           const u64 *__restrict__ reach, u64 *total, u64 *act, int64_t *npaths, int64_t *elems,
+                           int64_t *last, u64 *ctr) {
+	for (int l = blockIdx.x * blockDim.x + threadIdx.x; l < cnt; l += gridDim.x * blockDim.x) {
+		const int row = lane_row[l];
+		const int s = psrc[l], t = pdst[l];
+		const bool in_b = (reach[(int64_t)s * wd + (l >> 6)] >> (l & 63)) & 1;
+		const int64_t c0 = s == t ? 1 : 0;
+		total[l] = c0;
+		npaths[row] = c0;
+		elems[row] = c0;
+		last[row] = c0 ? 0 : -1;
+		if (in_b && c0 < k) {
+			atomicOr(&act[l >> 6], 1ull << (l & 63));
+			atomicAdd(&ctr[KS_ACTIVE], 1ull);
+		}
+	}
+}
+
+// Layer h of w over L lanes (see the top).  h == 1 counts the edges from each lane's source (lane_src, nl real lanes);
+// reach / act (nullable) restrict lane l to the rows of B(t_l) while it counts, and alive (nullable) flags each lane
+// with a non-zero w_h.  cur must be zero on entry.
+__global__ void __launch_bounds__(256) k_ks_omega(int h, int64_t m, int64_t n_ab, int L, int nl,
+                                                  const int32_t *__restrict__ in_off, const int32_t *__restrict__ in_adj,
+                                                  const int32_t *__restrict__ lane_src, const u64 *__restrict__ prev,
+                                                  u64 *cur, const u64 *__restrict__ reach, const u64 *__restrict__ act,
+                                                  int wd, uint32_t *alive) {
+	const int lane = threadIdx.x & 31;
+	const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+	const int64_t nchunks = (m + KS_CHUNK - 1) / KS_CHUNK;
+	for (int64_t c = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; c < nchunks; c += nwarps) {
+		const int64_t c0 = c * KS_CHUNK, c1 = min(c0 + KS_CHUNK, m);
+		const int64_t u0 = ks_row_of(in_off, n_ab, c0);
+		for (int g = 0; g < nl; g += 32) {
+			const int l = g + lane;
+			const bool on = l < nl;
+			const int s = on ? lane_src[l] : -1;
+			const bool counting = on && (!act || ((act[l >> 6] >> (l & 63)) & 1));
+			int64_t u = u0, e = c0;
+			while (e < c1) {
+				const int64_t rs = in_off[u], re = in_off[u + 1], end = min(re, c1);
+				const bool keep = counting && (!reach || ((reach[u * wd + (l >> 6)] >> (l & 63)) & 1));
+				if (__any_sync(FULL_MASK, keep)) {
+					u64 sum = 0;
+					for (; e < end; e++) {
+						const int64_t v = in_adj[e];
+						if (keep) {
+							sum = sat_add(sum, h == 1 ? (v == s ? 1ull : 0ull) : (v < n_ab ? prev[v * L + l] : 0ull));
+						}
+					}
+					if (keep && sum) {
+						if (rs >= c0 && re <= c1) {
+							cur[u * L + l] = sum;
+						} else {
+							atomic_sat_add(&cur[u * L + l], sum);
+						}
+						if (alive) {
+							alive[l] = 1;
+						}
+					}
+				}
+				e = end;
+				u++;
+			}
+		}
+	}
+}
+
+// After layer h: each counting lane takes min(count at t, k - total) walks of h edges and stops when its total
+// reaches k or w_h was zero on B(t)
+__global__ void k_ks_step(int h, int cnt, int L, int64_t n_ab, int64_t k, const int32_t *__restrict__ lane_row,
+                          const int32_t *__restrict__ pdst, const u64 *__restrict__ cur, uint32_t *alive, u64 *total,
+                          u64 *act, int64_t *npaths, int64_t *elems, int64_t *last, u64 *ctr) {
+	for (int l = blockIdx.x * blockDim.x + threadIdx.x; l < cnt; l += gridDim.x * blockDim.x) {
+		if (!((act[l >> 6] >> (l & 63)) & 1)) {
+			continue;
+		}
+		const int row = lane_row[l];
+		const int t = pdst[l];
+		const u64 c = t < n_ab ? cur[(int64_t)t * L + l] : 0;
+		const u64 before = total[l];
+		const u64 take = min(c, (u64)k - before);
+		if (take) {
+			total[l] = before + take;
+			npaths[row] = (int64_t)(before + take);
+			elems[row] = (int64_t)sat_add((u64)elems[row], sat_mul_len(take, 2 * (int64_t)h + 1));
+			last[row] = h;
+		}
+		const bool stop = before + take >= (u64)k || !alive[l];
+		alive[l] = 0;
+		if (h > KS_WALK_MAX && (take || !stop)) {
+			ctr[KS_TOO_LONG] = 1;
+		}
+		if (stop) {
+			atomicAnd(&act[l >> 6], ~(1ull << (l & 63)));
+		} else {
+			atomicAdd(&ctr[KS_ACTIVE], 1ull);
+		}
+	}
+}
+
+// the sources of a group's lanes
+__global__ void k_ks_group_src(int ng, const int32_t *__restrict__ glane, const int32_t *__restrict__ psrc,
+                               int32_t *gsrc) {
+	for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < ng; j += gridDim.x * blockDim.x) {
+		gsrc[j] = psrc[glane[j]];
+	}
+}
+
+// The walks of a group's rows: a block per row (grid-stride), a warp per walk (see the top).  layers[h - 1] is w_h of
+// the group, [n_ab][Lg].
+__global__ void __launch_bounds__(256) k_ks_unrank(int ng, int Lg, int64_t n, int64_t n_ab,
+                                                   const int32_t *__restrict__ glane, const int32_t *__restrict__ lane_row,
+                                                   const int32_t *__restrict__ psrc, const int32_t *__restrict__ pdst,
+                                                   const int64_t *__restrict__ src, const int64_t *__restrict__ dst,
+                                                   const u64 *__restrict__ layers, const int32_t *__restrict__ in_off,
+                                                   const u64 *__restrict__ step_key, const int32_t *__restrict__ step_pos,
+                                                   const int32_t *__restrict__ perm, const int64_t *__restrict__ edge_ids,
+                                                   const int64_t *__restrict__ npaths, const int64_t *__restrict__ last,
+                                                   const int64_t *__restrict__ first, const int64_t *__restrict__ elem_off,
+                                                   int64_t *walk_off, int64_t *elems) {
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+	const int64_t layer_cells = n_ab * Lg;
+	for (int j = blockIdx.x; j < ng; j += gridDim.x) {
+		const int ln = glane[j];
+		const int row = lane_row[ln];
+		const int s = psrc[ln], t = pdst[ln];
+		const int H = (int)last[row];
+		const int64_t np = npaths[row];
+		for (int64_t rank = warp; rank < np; rank += nw) {
+			// the walk's length h, and the walks of its row before it of other lengths (count and elements)
+			u64 carry_c = 0, carry_e = 0, before_c = 0, before_e = 0;
+			int h = -1;
+			for (int h0 = 0; h0 <= H && h < 0; h0 += 32) {
+				const int hh = h0 + lane;
+				u64 c = 0;
+				if (hh <= H) {
+					c = hh == 0 ? (s == t ? 1ull : 0ull)
+					            : (t < n_ab ? layers[(int64_t)(hh - 1) * layer_cells + (int64_t)t * Lg + j] : 0ull);
+				}
+				u64 ic = c, ie = c ? sat_mul_len(c, 2 * (int64_t)hh + 1) : 0;
+#pragma unroll
+				for (int d = 1; d < 32; d <<= 1) {
+					const u64 tc = __shfl_up_sync(FULL_MASK, ic, d), te = __shfl_up_sync(FULL_MASK, ie, d);
+					if (lane >= d) {
+						ic = sat_add(ic, tc);
+						ie = sat_add(ie, te);
+					}
+				}
+				const unsigned hit = __ballot_sync(FULL_MASK, sat_add(carry_c, ic) > (u64)rank);
+				if (hit) {
+					const int w = __ffs(hit) - 1;
+					const u64 pc = __shfl_sync(FULL_MASK, ic, w > 0 ? w - 1 : 0);
+					const u64 pe = __shfl_sync(FULL_MASK, ie, w > 0 ? w - 1 : 0);
+					before_c = sat_add(carry_c, w > 0 ? pc : 0);
+					before_e = sat_add(carry_e, w > 0 ? pe : 0);
+					h = h0 + w;
+				} else {
+					carry_c = sat_add(carry_c, __shfl_sync(FULL_MASK, ic, 31));
+					carry_e = sat_add(carry_e, __shfl_sync(FULL_MASK, ie, 31));
+				}
+			}
+			if (h < 0) {
+				break; // (cannot happen: the row's counts at t sum to at least npaths)
+			}
+			u64 r = (u64)rank - before_c;
+			const int64_t len = 2 * (int64_t)h + 1;
+			int64_t *out = elems + elem_off[row] + (int64_t)before_e + (int64_t)r * len;
+			if (lane == 0) {
+				walk_off[first[row] + rank] = out - elems;
+				out[len - 1] = h == 0 ? src[row] : dst[row];
+			}
+			int cur = t;
+			for (int k = h; k >= 1; k--) {
+				const u64 *wl = k >= 2 ? layers + (int64_t)(k - 2) * layer_cells : nullptr;
+				const int e1 = in_off[cur + 1];
+				const u64 key0 = (u64)(uint32_t)cur * (u64)n;
+				int pick_orig = -1, pick_pos = -1;
+				for (int c = in_off[cur]; c < e1 && pick_pos < 0; c += 32) {
+					const int e = c + lane;
+					u64 wv = 0;
+					int orig = 0, pos = 0;
+					if (e < e1) {
+						orig = (int)(step_key[e] - key0);
+						pos = step_pos[e];
+						const int par = perm[orig];
+						wv = k == 1 ? (par == s ? 1ull : 0ull) : (par < n_ab ? wl[(int64_t)par * Lg + j] : 0ull);
+					}
+					u64 incl = wv;
+#pragma unroll
+					for (int d = 1; d < 32; d <<= 1) {
+						const u64 tv = __shfl_up_sync(FULL_MASK, incl, d);
+						if (lane >= d) {
+							incl = sat_add(incl, tv);
+						}
+					}
+					const unsigned hit = __ballot_sync(FULL_MASK, incl > r);
+					if (hit) {
+						const int w = __ffs(hit) - 1;
+						const u64 before = __shfl_sync(FULL_MASK, incl, w > 0 ? w - 1 : 0);
+						r -= w > 0 ? before : 0;
+						pick_orig = __shfl_sync(FULL_MASK, orig, w);
+						pick_pos = __shfl_sync(FULL_MASK, pos, w);
+					} else {
+						r -= __shfl_sync(FULL_MASK, incl, 31);
+					}
+				}
+				if (pick_pos < 0) {
+					break; // (cannot happen: w_k(cur) > r)
+				}
+				if (lane == 0) {
+					out[2 * k - 1] = edge_ids[pick_pos];
+					out[2 * k - 2] = pick_orig;
+				}
+				cur = perm[pick_orig];
+			}
+		}
+	}
+}
+
+static inline u64 sat_add_host(u64 a, u64 b) { // a, b <= INT64_MAX
+	return a > AS_MAX - b ? AS_MAX : a + b;
+}
+
+static inline unsigned ks_grid(int64_t want, int64_t cap) {
+	return (unsigned)std::max<int64_t>(1, std::min<int64_t>(want, cap));
+}
+
+// the layer budget of the storing pass: 4 GiB, or PGQ_B200_KSP_LAYER_BUDGET bytes (tests force regrouping with it)
+static int layer_budget(int64_t *out) {
+	*out = KS_BUDGET;
+	const char *env = getenv("PGQ_B200_KSP_LAYER_BUDGET");
+	if (env && *env) {
+		char *end = nullptr;
+		const long long b = strtoll(env, &end, 10);
+		if (*end || b <= 0) {
+			return pgq_fail(PGQ_ERR_INVALID_ARG, "PGQ_B200_KSP_LAYER_BUDGET must be a positive byte count");
+		}
+		*out = b;
+	}
+	return PGQ_OK;
+}
+
+// the lane width: opts->lanes, or the widest of 512 .. 64 whose two counting layers fit 4 GiB, narrower while half of
+// it would hold every lane
+static int ks_lanes(const pgq_options *opts, int64_t n_ab, int64_t searches) {
+	if (opts && opts->lanes) {
+		return opts->lanes;
+	}
+	int w = 512;
+	while (w > 64 && 2 * std::max<int64_t>(n_ab, 1) * w * (int64_t)sizeof(u64) > KS_BUDGET) {
+		w >>= 1;
+	}
+	while (w > 64 && searches <= w / 2) {
+		w >>= 1;
+	}
+	return w;
+}
+
+extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
+                                    const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
+                                    int64_t k, int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid,
+                                    int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths,
+                                    pgq_stats *stats) {
+	if (!csr) {
+		return pgq_fail(PGQ_ERR_INVALID_ID, "%s", pgq_status_text(PGQ_ERR_INVALID_ID));
+	}
+	if (!out_path_offsets || !out_elems || !out_total_paths) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "null output");
+	}
+	*out_path_offsets = nullptr;
+	*out_elems = nullptr;
+	*out_total_paths = 0;
+	if (p < 0 || (p > 0 && (!src || !dst))) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "null or negative argument");
+	}
+	if (p > 0 && (!out_npaths || !out_first_path || !out_valid)) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "null output");
+	}
+	if (k < 1) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "k must be >= 1");
+	}
+	if (opts && (opts->lanes < 0 || opts->lanes > 512 || opts->lanes % 64)) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "lanes must be 0 or a multiple of 64 up to 512");
+	}
+	if (p >= 0x7fffffffLL) {
+		return pgq_fail(PGQ_ERR_RANGE, "too many pairs in one call");
+	}
+	if (!csr->finalized) {
+		return pgq_fail(PGQ_ERR_NOT_INITIALIZED, "%s", pgq_status_text(PGQ_ERR_NOT_INITIALIZED));
+	}
+	if (opts && opts->shard_count > 1) {
+		return pgq_fail(PGQ_ERR_UNSUPPORTED, "shortest_k_paths has no multi-GPU form");
+	}
+	int64_t budget;
+	PGQ_TRY(layer_budget(&budget));
+	const int64_t n = csr->n, m = csr->m, n_ab = csr->n_ab;
+	// the lanes: the rows whose ids are both valid, in input order
+	std::vector<int32_t> lane_row;
+	for (int64_t i = 0; i < p; i++) {
+		if ((src_valid && !src_valid[i]) || (dst_valid && !dst_valid[i])) {
+			continue;
+		}
+		if (src[i] < 0 || src[i] >= n || dst[i] < 0 || dst[i] >= n) {
+			return pgq_fail(PGQ_ERR_RANGE, "vertex id outside [0, %lld) in row %lld", (long long)n, (long long)i);
+		}
+		lane_row.push_back((int32_t)i);
+	}
+	const int64_t S = (int64_t)lane_row.size();
+	const int W = ks_lanes(opts, n_ab, S);
+	pgq_stats st;
+	memset(&st, 0, sizeof(st));
+	st.lanes = W;
+	st.searches = S;
+	if (p == 0) {
+		*out_path_offsets = (int64_t *)calloc(1, sizeof(int64_t));
+		*out_elems = (int64_t *)malloc(sizeof(int64_t));
+		if (!*out_path_offsets || !*out_elems) {
+			free(*out_path_offsets);
+			free(*out_elems);
+			*out_path_offsets = *out_elems = nullptr;
+			return pgq_fail(PGQ_ERR_OOM, "host allocation failed");
+		}
+		if (stats) {
+			*stats = st;
+		}
+		return PGQ_OK;
+	}
+	PGQ_CUDA(cudaSetDevice(csr->ctx->device));
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	Workspace *ws = g.ws;
+	cudaStream_t s = ws->stream;
+	const int sms = csr->ctx->sm_count;
+	const size_t b8 = (size_t)p * sizeof(int64_t);
+	const int wd = W / 64;
+	const int64_t cells = n * wd;
+	const int64_t *d_src, *d_dst;
+	const int32_t *d_lane_row;
+	int32_t *psrc, *pdst, *gsrc, *glane;
+	u64 *reach, *front, *next, *om_a, *om_b, *total, *act, *ctr;
+	uint32_t *alive;
+	int64_t *npaths, *elems_row, *last, *first, *elem_off;
+	uint8_t *d_valid;
+	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
+	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d_dst));
+	PGQ_TRY(stage_column(ws, WS_KS_LANE_ROW, S ? lane_row.data() : nullptr, (size_t)S * sizeof(int32_t),
+	                     (const void **)&d_lane_row));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_valid));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_PSRC, (size_t)S * sizeof(int32_t), (void **)&psrc));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_PDST, (size_t)S * sizeof(int32_t), (void **)&pdst));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_REACH, (size_t)cells * sizeof(u64), (void **)&reach));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_FRONT, (size_t)cells * sizeof(u64), (void **)&front));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_NEXT, (size_t)cells * sizeof(u64), (void **)&next));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_OMEGA_A, (size_t)n_ab * W * sizeof(u64), (void **)&om_a));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_OMEGA_B, (size_t)n_ab * W * sizeof(u64), (void **)&om_b));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_TOTAL, (size_t)W * sizeof(u64), (void **)&total));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ALIVE, (size_t)W * sizeof(uint32_t), (void **)&alive));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ACTIVE, (size_t)wd * sizeof(u64), (void **)&act));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_COUNTERS, 256, (void **)&ctr));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_NPATHS, b8, (void **)&npaths));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ROW_ELEMS, b8, (void **)&elems_row));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_LAST, b8, (void **)&last));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_FIRST, b8, (void **)&first));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ELEM_OFF, b8, (void **)&elem_off));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_GROUP_SRC, (size_t)W * sizeof(int32_t), (void **)&gsrc));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_GROUP_LANE, (size_t)W * sizeof(int32_t), (void **)&glane));
+	PGQ_CUDA(cudaEventRecord(ws->ev_begin, s));
+	PGQ_CUDA(cudaMemsetAsync(npaths, 0, b8, s));
+	PGQ_CUDA(cudaMemsetAsync(elems_row, 0, b8, s));
+	PGQ_CUDA(cudaMemsetAsync(last, 0xff, b8, s)); // -1: no walk
+	PGQ_CUDA(cudaMemsetAsync(alive, 0, (size_t)W * sizeof(uint32_t), s));
+	if (S > 0) {
+		k_ks_lanes<<<ks_grid((S + 255) / 256, 4096), 256, 0, s>>>(S, d_lane_row, d_src, d_dst, csr->perm, psrc, pdst);
+		PGQ_CUDA(cudaGetLastError());
+		st.kernel_launches++;
+	}
+	const u64 *step_key = nullptr;
+	const int32_t *step_pos = nullptr;
+	PGQ_TRY(build_step_lists(csr, ws, s, &step_key, &step_pos, &st.kernel_launches));
+	const unsigned edge_grid = ks_grid((m + 255) / 256, (int64_t)sms * 16);
+	const unsigned chunk_grid = ks_grid((m + KS_CHUNK * 8 - 1) / (KS_CHUNK * 8), (int64_t)sms * 16);
+	const unsigned cell_grid = ks_grid((cells + 255) / 256, (int64_t)sms * 8);
+	u64 h_ctr[3];
+	// ---- per batch: backward reach, then the counting pass ----
+	for (int64_t b0 = 0; b0 < S; b0 += W) {
+		const int cnt = (int)std::min<int64_t>(W, S - b0);
+		const int L = (int)std::min<int64_t>(W, (cnt + 63) / 64 * 64);
+		const int bwd = L / 64;
+		const int64_t bcells = n * bwd;
+		const unsigned lane_grid = ks_grid((cnt + 255) / 256, 64);
+		st.batches++;
+		PGQ_CUDA(cudaMemsetAsync(reach, 0, (size_t)bcells * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(front, 0, (size_t)bcells * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(next, 0, (size_t)bcells * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(act, 0, (size_t)bwd * sizeof(u64), s));
+		k_ks_reach_seed<<<lane_grid, 256, 0, s>>>(cnt, bwd, pdst + b0, reach, front);
+		PGQ_CUDA(cudaGetLastError());
+		st.kernel_launches++;
+		for (;;) {
+			PGQ_CUDA(cudaMemsetAsync(&ctr[KS_CHANGED], 0, sizeof(u64), s));
+			if (m > 0) {
+				k_ks_reach_level<<<edge_grid, 256, 0, s>>>(m, n_ab, bwd, csr->in.off, csr->in.adj, front, reach, next);
+				st.kernel_launches++;
+			}
+			k_ks_reach_update<<<ks_grid((bcells + 255) / 256, (int64_t)sms * 8), 256, 0, s>>>(bcells, reach, front, next,
+			                                                                                  ctr);
+			PGQ_CUDA(cudaGetLastError());
+			st.kernel_launches++;
+			st.push_levels++;
+			PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(u64), cudaMemcpyDeviceToHost, s));
+			PGQ_CUDA(cudaStreamSynchronize(s));
+			if (!h_ctr[KS_CHANGED]) {
+				break;
+			}
+		}
+		PGQ_CUDA(cudaMemsetAsync(ctr, 0, 3 * sizeof(u64), s));
+		k_ks_start<<<lane_grid, 256, 0, s>>>(cnt, bwd, k, d_lane_row + b0, psrc + b0, pdst + b0, reach, total, act, npaths,
+		                                     elems_row, last, ctr);
+		PGQ_CUDA(cudaGetLastError());
+		st.kernel_launches++;
+		PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaStreamSynchronize(s));
+		u64 *prev = om_a, *cur = om_b;
+		for (int h = 1; h_ctr[KS_ACTIVE] > 0; h++) {
+			PGQ_CUDA(cudaMemsetAsync(cur, 0, (size_t)n_ab * L * sizeof(u64), s));
+			PGQ_CUDA(cudaMemsetAsync(&ctr[KS_ACTIVE], 0, sizeof(u64), s));
+			if (m > 0) {
+				k_ks_omega<<<chunk_grid, 256, 0, s>>>(h, m, n_ab, L, cnt, csr->in.off, csr->in.adj, psrc + b0, prev, cur,
+				                                      reach, act, bwd, alive);
+				st.kernel_launches++;
+			}
+			k_ks_step<<<lane_grid, 256, 0, s>>>(h, cnt, L, n_ab, k, d_lane_row + b0, pdst + b0, cur, alive, total, act,
+			                                    npaths, elems_row, last, ctr);
+			PGQ_CUDA(cudaGetLastError());
+			st.kernel_launches++;
+			st.levels++;
+			PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, s));
+			PGQ_CUDA(cudaStreamSynchronize(s));
+			if (h_ctr[KS_TOO_LONG]) {
+				return pgq_fail(PGQ_ERR_UNSUPPORTED, "a row needs a walk longer than %d edges", KS_WALK_MAX);
+			}
+			std::swap(prev, cur);
+		}
+	}
+	// ---- the rows' walk counts and element counts; their first walk and first element ----
+	std::vector<int64_t> h_np((size_t)p), h_el((size_t)p), h_last((size_t)p);
+	PGQ_CUDA(cudaMemcpyAsync(h_np.data(), npaths, b8, cudaMemcpyDeviceToHost, s));
+	PGQ_CUDA(cudaMemcpyAsync(h_el.data(), elems_row, b8, cudaMemcpyDeviceToHost, s));
+	PGQ_CUDA(cudaMemcpyAsync(h_last.data(), last, b8, cudaMemcpyDeviceToHost, s));
+	PGQ_CUDA(cudaStreamSynchronize(s));
+	u64 walks = 0, elem_total = 0;
+	for (int64_t i = 0; i < p; i++) {
+		walks += (u64)h_np[(size_t)i]; // (each at most k <= INT64_MAX, and p < 2^31 of them)
+		elem_total = sat_add_host(elem_total, (u64)h_el[(size_t)i]);
+	}
+	if (elem_total > (AS_MAX / sizeof(int64_t)) || walks > (AS_MAX / sizeof(int64_t)) - 1) {
+		return pgq_fail(PGQ_ERR_OOM, "the walks of one call hold too many elements (%llu)",
+		                (unsigned long long)elem_total);
+	}
+	int64_t *d_total;
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_SCAN_TOTAL, sizeof(int64_t), (void **)&d_total));
+	pgq_path_offsets(0, 0, p, elem_off, elems_row, d_valid, d_total, s);
+	pgq_path_offsets(0, 0, p, first, npaths, d_valid, d_total, s); // (out_valid = a row has a walk)
+	PGQ_CUDA(cudaGetLastError());
+	st.kernel_launches += 2;
+	int64_t *walk_off, *d_elems;
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_WALK_OFF, (size_t)(walks + 1) * sizeof(int64_t), (void **)&walk_off));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ELEMS, (size_t)elem_total * sizeof(int64_t), (void **)&d_elems));
+	// ---- the storing pass and the unranking, group by group ----
+	std::vector<int32_t> grp;
+	int64_t grp_h = 0;
+	auto layer_bytes = [&](int64_t h, int64_t rows) { return (double)(h + 1) * (double)n_ab * (double)rows * 8.0; };
+	auto run_group = [&]() -> int {
+		const int ng = (int)grp.size();
+		if (ng == 0) {
+			return PGQ_OK;
+		}
+		u64 *layers;
+		PGQ_TRY(pgq_ws_reserve(ws, WS_KS_LAYERS, (size_t)std::max<int64_t>(grp_h, 1) * n_ab * ng * sizeof(u64),
+		                       (void **)&layers));
+		PGQ_CUDA(cudaMemcpyAsync(glane, grp.data(), (size_t)ng * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+		k_ks_group_src<<<ks_grid((ng + 255) / 256, 64), 256, 0, s>>>(ng, glane, psrc, gsrc);
+		PGQ_CUDA(cudaGetLastError());
+		st.kernel_launches++;
+		if (grp_h > 0) {
+			PGQ_CUDA(cudaMemsetAsync(layers, 0, (size_t)grp_h * n_ab * ng * sizeof(u64), s));
+		}
+		for (int64_t h = 1; h <= grp_h && m > 0; h++) {
+			u64 *lcur = layers + (h - 1) * n_ab * ng;
+			const u64 *lprev = h >= 2 ? layers + (h - 2) * n_ab * ng : nullptr;
+			k_ks_omega<<<chunk_grid, 256, 0, s>>>((int)h, m, n_ab, ng, ng, csr->in.off, csr->in.adj, gsrc, lprev, lcur,
+			                                      nullptr, nullptr, 0, nullptr);
+			st.kernel_launches++;
+		}
+		k_ks_unrank<<<ks_grid(ng, (int64_t)sms * 16), 256, 0, s>>>(
+		    ng, ng, n, n_ab, glane, d_lane_row, psrc, pdst, d_src, d_dst, layers, csr->in.off, step_key, step_pos,
+		    csr->perm, csr->edge_ids, npaths, last, first, elem_off, walk_off, d_elems);
+		PGQ_CUDA(cudaGetLastError());
+		st.kernel_launches++;
+		// (the next group reuses the group buffers)
+		PGQ_CUDA(cudaStreamSynchronize(s));
+		grp.clear();
+		grp_h = 0;
+		return PGQ_OK;
+	};
+	for (int64_t ln = 0; ln < S; ln++) {
+		const int64_t row = lane_row[(size_t)ln];
+		if (h_np[(size_t)row] == 0) {
+			continue;
+		}
+		const int64_t h = h_last[(size_t)row];
+		if (layer_bytes(h, 1) > (double)budget) {
+			return pgq_fail(PGQ_ERR_UNSUPPORTED, "the walks of row %lld need %.0f bytes of count layers, over the budget of "
+			                "%lld", (long long)row, layer_bytes(h, 1), (long long)budget);
+		}
+		const int64_t gh = std::max(grp_h, h);
+		if (!grp.empty() && ((int64_t)grp.size() == W || layer_bytes(gh, (int64_t)grp.size() + 1) > (double)budget)) {
+			PGQ_TRY(run_group());
+		}
+		grp.push_back((int32_t)ln);
+		grp_h = std::max(grp_h, h);
+	}
+	PGQ_TRY(run_group());
+	// ---- back to the host ----
+	int64_t *h_off = (int64_t *)malloc((size_t)(walks + 1) * sizeof(int64_t));
+	int64_t *h_elems = (int64_t *)malloc((size_t)std::max<u64>(elem_total, 1) * sizeof(int64_t));
+	if (!h_off || !h_elems) {
+		free(h_off);
+		free(h_elems);
+		return pgq_fail(PGQ_ERR_OOM, "host allocation of %llu walk elements failed", (unsigned long long)elem_total);
+	}
+	cudaError_t e = cudaSuccess;
+	if (walks > 0) e = cudaMemcpyAsync(h_off, walk_off, (size_t)walks * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess && elem_total > 0)
+		e = cudaMemcpyAsync(h_elems, d_elems, (size_t)elem_total * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(out_first_path, first, b8, cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(out_valid, d_valid, (size_t)p, cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaEventRecord(ws->ev_end, s);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+	float ms = 0.f;
+	if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end);
+	g.settled = (e == cudaSuccess);
+	if (e != cudaSuccess) {
+		cudaGetLastError();
+		free(h_off);
+		free(h_elems);
+		return pgq_fail(PGQ_ERR_CUDA, "copying the walks back failed: %s", cudaGetErrorString(e));
+	}
+	h_off[walks] = (int64_t)elem_total;
+	memcpy(out_npaths, h_np.data(), b8);
+	st.total_ms = ms;
+	st.h2d_bytes = 2 * (int64_t)b8 + S * (int64_t)sizeof(int32_t);
+	st.d2h_bytes = 3 * (int64_t)b8 + p + (int64_t)(walks + elem_total) * (int64_t)sizeof(int64_t);
+	*out_path_offsets = h_off;
+	*out_elems = h_elems;
+	*out_total_paths = (int64_t)walks;
+	if (stats) {
+		*stats = st;
+	}
+	return PGQ_OK;
+}

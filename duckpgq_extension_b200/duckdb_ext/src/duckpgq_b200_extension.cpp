@@ -72,6 +72,7 @@ static pgq_ctx *g_ctx = nullptr;
 static std::atomic<int64_t> g_calls_cheapest_path {0};
 static std::atomic<int64_t> g_calls_path_count {0};
 static std::atomic<int64_t> g_calls_all_shortest {0};
+static std::atomic<int64_t> g_calls_shortest_k {0};
 static std::atomic<int64_t> g_calls_lengths {0}, g_calls_paths {0}, g_calls_cheapest {0}, g_pairs {0}, g_uploads {0},
     g_device_builds {0}, g_chunks {0}, g_materialized {0}, g_calls_lcc {0}, g_calls_pagerank {0}, g_calls_wcc {0},
     g_calls_bidirectional {0}, g_calls_w_type {0}, g_calls_reachability {0};
@@ -971,6 +972,75 @@ static void AllShortestPathsB200Function(DataChunk &args, ExpressionState &state
 	duckpgq_state->csr_to_delete.insert(info.csr_id);
 }
 
+// ---- shortest_k_paths (no reference function) ---------------------------------------------------------------
+// The k shortest walks of a row (include/duckpgq_b200.h, pgq_shortest_k_paths), called as a raw UDF over the CSR CTE:
+// the MATCH rewriter stays the reference's, which rejects SHORTEST k (match.cpp:84-86).  The bind is shortestpath's
+// and also wants a constant k >= 1; the CSR lookup is shortestpath's.
+static unique_ptr<FunctionData> ShortestKPathsBind(BindScalarFunctionInput &input) {
+	auto &arguments = input.GetArguments();
+	if (!arguments[4]->IsFoldable()) {
+		throw InvalidInputException("k must be constant.");
+	}
+	auto k = ExpressionExecutor::EvaluateScalar(input.GetClientContext(), *arguments[4]);
+	if (k.IsNull() || k.GetValue<int64_t>() < 1) {
+		throw InvalidInputException("k must be 1 or more.");
+	}
+	return IterativeLengthFunctionData::IterativeLengthBind(input);
+}
+
+static void ShortestKPathsB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
+	auto &info = func_expr.BindInfo()->Cast<IterativeLengthFunctionData>();
+	auto duckpgq_state = GetDuckPGQState(info.context);
+	CSR &csr = ShortestPathCsr(*duckpgq_state, info.csr_id);
+	int64_t v_size = args.data[1].GetValue(0).GetValue<int64_t>();
+	int64_t k = args.data[4].GetValue(0).GetValue<int64_t>(); // (constant: ShortestKPathsBind)
+	PairColumns pairs(args);
+	idx_t count = args.size();
+	auto device_csr = GetB200State(info.context)->ForPathFunction(info.csr_id, csr, v_size);
+	vector<int64_t> npaths(count), first(count);
+	vector<uint8_t> out_valid(count);
+	int64_t *offsets = nullptr, *elems = nullptr;
+	int64_t walks = 0;
+	pgq_options opts = OptionsFromEnv();
+	int st = pgq_shortest_k_paths(device_csr, static_cast<int64_t>(count), pairs.src.data(), pairs.dst.data(),
+	                              pairs.valid.data(), nullptr, &opts, k, npaths.data(), first.data(), out_valid.data(),
+	                              &offsets, &elems, &walks, nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_shortest_k++;
+	g_pairs += static_cast<int64_t>(count);
+	const idx_t total = static_cast<idx_t>(offsets[walks]);
+	result.SetVectorType(VectorType::FLAT_VECTOR);
+	auto result_data = FlatVector::GetDataMutable<list_entry_t>(result);
+	ValidityMask &result_validity = FlatVector::ValidityMutable(result);
+	ListVector::Reserve(result, static_cast<idx_t>(walks));
+	auto &inner = ListVector::GetChildMutable(result);
+	ListVector::Reserve(inner, total);
+	if (total > 0) {
+		auto leaf = FlatVector::GetDataMutable<int64_t>(ListVector::GetChildMutable(inner));
+		memcpy(leaf, elems, total * sizeof(int64_t));
+	}
+	ListVector::SetListSize(inner, total);
+	auto inner_data = FlatVector::GetDataMutable<list_entry_t>(inner);
+	for (int64_t j = 0; j < walks; j++) {
+		inner_data[j].offset = static_cast<idx_t>(offsets[j]);
+		inner_data[j].length = static_cast<idx_t>(offsets[j + 1] - offsets[j]);
+	}
+	pgq_free(offsets);
+	pgq_free(elems);
+	for (idx_t i = 0; i < count; i++) {
+		result_data[i].offset = static_cast<idx_t>(first[i]);
+		result_data[i].length = static_cast<idx_t>(npaths[i]);
+		if (!out_valid[i]) {
+			result_validity.SetInvalid(i);
+		}
+	}
+	ListVector::SetListSize(result, static_cast<idx_t>(walks));
+	duckpgq_state->csr_to_delete.insert(info.csr_id);
+}
+
 // ---- cheapest_path_length -------------------------------------------------------------------------------
 // cheapest_path_length.cpp:138-160: batched Bellman-Ford over the weighted CSR, BIGINT or DOUBLE result as
 // the bind decided (cheapest_path_length_function_data.cpp:26-30).  The bind stays the reference's.
@@ -1215,7 +1285,8 @@ static void B200StatsFunction(DataChunk &args, ExpressionState &state, Vector &r
 	              ",reachability_calls=" + std::to_string(g_calls_reachability.load()) +
 	              ",cheapest_path_calls=" + std::to_string(g_calls_cheapest_path.load()) +
 	              ",shortest_path_count_calls=" + std::to_string(g_calls_path_count.load()) +
-	              ",all_shortest_paths_calls=" + std::to_string(g_calls_all_shortest.load());
+	              ",all_shortest_paths_calls=" + std::to_string(g_calls_all_shortest.load()) +
+	              ",shortest_k_paths_calls=" + std::to_string(g_calls_shortest_k.load());
 	result.SetVectorType(VectorType::CONSTANT_VECTOR);
 	ConstantVector::GetData<string_t>(result)[0] = StringVector::AddString(result, text);
 }
@@ -1330,6 +1401,10 @@ static void LoadInternal(ExtensionLoader &loader) {
 	    "all_shortest_paths",
 	    {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
 	    LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT)), AllShortestPathsB200Function, AllShortestPathsBind));
+	loader.RegisterFunction(ScalarFunction(
+	    "shortest_k_paths",
+	    {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
+	    LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT)), ShortestKPathsB200Function, ShortestKPathsBind));
 	ScalarFunction stats("duckpgq_b200_stats", {}, LogicalType::VARCHAR, B200StatsFunction);
 	stats.SetVolatile();
 	loader.RegisterFunction(stats);

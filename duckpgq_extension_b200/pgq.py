@@ -10,6 +10,7 @@ like the reference's own sqllogictests:
     cheapest_path(id, v_size, src, dst)                               (no reference function: the cheapest path's list)
     shortest_path_count(id, v_size, src, dst)                         (no reference function: ALL SHORTEST's count)
     all_shortest_paths(id, v_size, src, dst, max_paths)               (no reference function: ALL SHORTEST's lists)
+    shortest_k_paths(id, v_size, src, dst, k)                         (no reference function: SHORTEST k's walks)
     delete_csr(id)                                                    csr_deletion.cpp:10-29
     DuckPGQState.{csr_list, csr_to_delete, get_csr, query_end}        duckpgq_state.hpp:12-39, duckpgq_state.cpp:162-186
 
@@ -470,6 +471,34 @@ class DeviceCSR:
                  for i in range(p)]
         return paths, cnt[:p], st.as_dict()
 
+    def shortest_k_paths(self, src, dst, k: int, src_valid=None, dst_valid=None, options: Optional[Options] = None):
+        """-> (per row: list of [src, e1, v1, ..., dst] walks or None, npaths int64, stats dict): the first min(k,
+        total) walks of each row, shortest first, in step order within a length (include/duckpgq_b200.h,
+        pgq_shortest_k_paths)."""
+        src, dst = _i64(src), _i64(dst)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        dv = None if dst_valid is None else np.ascontiguousarray(dst_valid, dtype=np.uint8)
+        npaths = np.zeros(max(p, 1), dtype=np.int64)
+        first = np.zeros(max(p, 1), dtype=np.int64)
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        offs, elems = C.POINTER(C.c_int64)(), C.POINTER(C.c_int64)()
+        total = C.c_int64(0)
+        st = _native.PgqStats()
+        opts = (options or Options()).c()
+        _check(self._lib.pgq_shortest_k_paths(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv), C.byref(opts),
+                                              int(k), _p64(npaths), _p64(first), _pu8(ov), C.byref(offs),
+                                              C.byref(elems), C.byref(total), C.byref(st)))
+        try:
+            woff = np.ctypeslib.as_array(offs, shape=(total.value + 1,)).copy()
+            flat = np.ctypeslib.as_array(elems, shape=(int(woff[-1]),)).copy() if woff[-1] else np.zeros(0, np.int64)
+        finally:
+            self._lib.pgq_free(offs)
+            self._lib.pgq_free(elems)
+        walks = [flat[woff[j]: woff[j + 1]].tolist() for j in range(total.value)]
+        paths = [walks[first[i]: first[i] + npaths[i]] if ov[i] else None for i in range(p)]
+        return paths, npaths[:p], st.as_dict()
+
     def free(self):
         if getattr(self, "_h", None):
             self._lib.pgq_csr_free(self._h)
@@ -688,6 +717,18 @@ def all_shortest_paths(state: DuckPGQState, csr_id: int, v_size: int, src, dst, 
     if int(v_size) != csr.n:
         raise InvalidInputException(PGQ_ERR_INVALID_ARG, f"v_size {v_size} does not match the CSR ({csr.n} vertices)")
     paths, _, _ = csr.all_shortest_paths(src, dst, max_paths, src_valid, dst_valid, options)
+    state.csr_to_delete.add(csr_id)
+    return paths
+
+
+def shortest_k_paths(state: DuckPGQState, csr_id: int, v_size: int, src, dst, k: int, src_valid=None, dst_valid=None,
+                     options: Optional[Options] = None):
+    """shortest_k_paths(INT, BIGINT, BIGINT, BIGINT, BIGINT k) -> LIST(LIST(BIGINT)): per row the first min(k, total)
+    walks, shortest first, or None (no reference function; looked up and marked as shortestpath is)."""
+    csr = _lookup_for_path(state, csr_id, lengths=False)
+    if int(v_size) != csr.n:
+        raise InvalidInputException(PGQ_ERR_INVALID_ARG, f"v_size {v_size} does not match the CSR ({csr.n} vertices)")
+    paths, _, _ = csr.shortest_k_paths(src, dst, k, src_valid, dst_valid, options)
     state.csr_to_delete.add(csr_id)
     return paths
 

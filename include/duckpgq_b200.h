@@ -335,6 +335,50 @@ int pgq_all_shortest_paths(pgq_csr *csr, int64_t n_pairs, const int64_t *src, co
                            int64_t *out_offsets, uint8_t *out_valid, int64_t **out_elems, int64_t *out_total,
                            pgq_stats *stats);
 
+/* pgq_shortest_k_paths: the k shortest walks of a row (SQL/PGQ's SHORTEST k; the reference parses it and rejects it).
+ * No reference function.  SQL/PGQ's default path mode is WALK, and the reference supports no other, so vertices and
+ * edges may repeat.  For a row (s, t) and k >= 1:
+ *   - a walk of h edges is a list [s, e1, v1, ..., eh, t] in pgq_shortestpath's format (vertex rowids; edge rowids from
+ *     the CSR's edge ids, CSR positions when it was uploaded without ids).  Parallel edges give distinct walks.  There
+ *     are (A^h)[s, t] walks of h edges, A the adjacency matrix with edge multiplicities.
+ *   - order: by h ascending; walks of the same h exactly as pgq_all_shortest_paths orders paths (walking back from t, a
+ *     step is (the parent's ORIGINAL id, the edge's position in the parent's adjacency as pgq_csr_download returns
+ *     it), steps compared lexicographically from t back to s).
+ *   - result: the first min(k, total) walks in that order.  A row gets fewer than k walks only when it has fewer than k
+ *     in all, which happens only when no cycle lies on any s -> t walk; then it gets all of them.  s == t: the first
+ *     walk is [s] (h = 0), then the closed walks through s.  For k <= count the result equals
+ *     pgq_all_shortest_paths(max_paths = k); walk 0 is pgq_shortestpath's path.
+ *   - NULL (out_valid 0, no walks): a NULL source or destination (src_valid / dst_valid, both nullable), or t not
+ *     reachable from s.
+ *   - out_npaths[i] walks of row i are the call's walks out_first_path[i] .. + out_npaths[i]; walk j is
+ *     (*out_elems)[(*out_path_offsets)[j] .. (*out_path_offsets)[j + 1]); *out_total_paths walks in all.  Both arrays
+ *     are allocated by the library (also for zero rows): release them with pgq_free().
+ *   - errors: k < 1 -> PGQ_ERR_INVALID_ARG; opts->lanes not 0 or a multiple of 64 up to 512 -> PGQ_ERR_INVALID_ARG; an
+ *     id outside [0, n) in a row whose ids are both valid -> PGQ_ERR_RANGE; a missing or unfinalised CSR ->
+ *     pgq_shortestpath's errors; shard_count > 1 -> PGQ_ERR_UNSUPPORTED; a walk the result needs longer than 65533
+ *     edges -> PGQ_ERR_UNSUPPORTED (this bounds the call, whatever the graph); a row whose count layers alone,
+ *     (H + 1) x n_ab x 8 bytes (H its last walk's length, n_ab the vertices with in-edges), exceed the layer budget
+ *     (4 GiB) -> PGQ_ERR_UNSUPPORTED; an element total that overflows int64 or cannot be allocated -> PGQ_ERR_OOM,
+ *     checked before anything of that size is allocated.
+ *   - counts saturate at INT64_MAX and ranks stay exact anyway: every rank listed is below k.
+ *   - the call: the rows whose ids are both valid take lanes in input order (no de-duplication), W per batch (W =
+ *     opts->lanes, or for 0 the widest of 512, 256, 128, 64 whose two count layers n_ab x W x 8 bytes fit 4 GiB,
+ *     halved while W > 64 and the rows that take lanes are at most W / 2).  A batch finds B(t), the vertices that reach
+ *     its lanes' targets (t included), by a BFS back from the targets, then counts the walks layer by layer: a lane
+ *     stops after the layer h >= 0 where its running total reaches k or where the walk counts are zero on all of B(t)
+ *     (s outside B(t): the row is NULL and its lane stops at layer 0), and a batch runs until all its lanes stop.
+ *     Then the rows with walks are regrouped to recompute and keep their layers within the layer budget, and the walks
+ *     are unranked.  opts->direction, alpha and flags are not used.
+ *   - stats: batches; lanes = W; searches = the rows that took a lane; levels = the sum over batches of the layers
+ *     h >= 1 each computed (its lanes' largest stopping layer); push_levels = the sum over batches of the backward
+ *     BFS's levels (1 + the largest distance to a lane's target from a vertex that reaches it: the last level adds
+ *     nothing); kernel_launches, h2d_bytes, d2h_bytes and total_ms (the whole call).  The other counters are 0. */
+int pgq_shortest_k_paths(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const int64_t *dst,
+                         const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts, int64_t k,
+                         int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid,
+                         int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths,
+                         pgq_stats *stats);
+
 /* ---- the other consumers of the CSR ------------------------------------------------------------------------
  * Host pointers in and out.  As in the reference, "v_size" is n + 2: the two entries n and n + 1 behind the
  * vertices have no edges and take part where the reference lets them.  Results are bit-identical to the reference's.
