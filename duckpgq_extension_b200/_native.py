@@ -17,6 +17,7 @@ INCLUDE = os.path.join(ROOT, "include")
 LIB_DIR = os.path.join(_PKG, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libduckpgq_b200.so")
 SOURCES = ["pgq_csr.cu", "pgq_bfs.cu", "pgq_api.cu", "pgq_cheapest.cu", "pgq_allshortest.cu", "pgq_kshortest.cu",
+           "pgq_kpaths_modes.cu",
            "pgq_multi.cu", "pgq_analytics.cu"]
 HEADERS = ["pgq_internal.h", "pgq_tile.cuh", "pgq_pull.cuh", "pgq_count.cuh"]
 
@@ -121,6 +122,8 @@ SYMBOLS = {
                                          _PU8, C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
     "pgq_shortest_k_paths": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, C.c_int64, _P64, _P64, _PU8,
                                        C.POINTER(_P64), C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
+    "pgq_shortest_k_paths_mode": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, C.c_int64, C.c_int32, _P64,
+                                            _P64, _PU8, C.POINTER(_P64), C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
     "pgq_local_clustering_coefficient": (C.c_int, [_VP, C.c_int64, _P64, _PU8, C.POINTER(C.c_float), _PU8,
                                                    C.POINTER(PgqStats)]),
     "pgq_pagerank": (C.c_int, [_VP, C.c_int64, _P64, _PU8, C.POINTER(C.c_double), _PU8, _P64, C.POINTER(PgqStats)]),

@@ -26,3 +26,9 @@ __device__ __forceinline__ u64 atomic_sat_add(u64 *a, u64 v) {
 // the parent's ORIGINAL id, then the edge's position in the parent's adjacency -- sit at [in_off[u], in_off[u + 1]).
 int build_step_lists(pgq_csr *csr, Workspace *ws, cudaStream_t s, const u64 **keys, const int32_t **pos,
                      int64_t *launches);
+
+// shortest_k_paths' argument checks, shared by every path mode: the outputs are cleared first, then null and negative
+// arguments, k < 1, lanes, the pair count, an unfinalised CSR and shard_count, in that order
+int ks_check_call(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, const pgq_options *opts, int64_t k,
+                  const int64_t *out_npaths, const int64_t *out_first_path, const uint8_t *out_valid,
+                  int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths);

@@ -152,6 +152,14 @@ enum WsSlot : int {
 	WS_KS_NPATHS = 80, WS_KS_ROW_ELEMS = 81, WS_KS_LAST = 82, WS_KS_FIRST = 83, WS_KS_ELEM_OFF = 84,
 	WS_KS_GROUP_LANE = 85, WS_KS_GROUP_SRC = 86, WS_KS_LAYERS = 87, WS_KS_WALK_OFF = 88, WS_KS_ELEMS = 89,
 	WS_KS_SCAN_TOTAL = 90,
+	// shortest_k_paths' path modes (pgq_kpaths_modes.cu), which also read the step lists: the rows' internal ids; a
+	// round's spur searches, their ban lists and seed flags; a batch's lane -> spur map, seen / frontier / next masks
+	// [n][W / 64], levels [n][W] uint16, done and grew masks, spur lengths and offsets, counters, TRAIL's ban bitmap over
+	// out-CSR positions and its (position, lane) table; the spurs' steps and elements.
+	WS_KM_IDS = 91, WS_KM_PIDS = 92, WS_KM_SPURS = 93, WS_KM_LISTS = 94, WS_KM_HAS_SEED = 95, WS_KM_LANE_SPUR = 96,
+	WS_KM_SEEN = 97, WS_KM_FRONT = 98, WS_KM_NEXT = 99, WS_KM_LEVEL = 100, WS_KM_DONE = 101, WS_KM_GREW = 102,
+	WS_KM_HLEN = 103, WS_KM_LANE_OFF = 104, WS_KM_COUNTERS = 105, WS_KM_BAN_BITS = 106, WS_KM_BAN_KEYS = 107,
+	WS_KM_STEPS = 108, WS_KM_STEP_ELEMS = 109,
 	WS_SLOTS // (the last block holds the highest numbers)
 };
 
@@ -177,6 +185,10 @@ constexpr int ws_ks[] = {WS_KS_LANE_ROW, WS_KS_PSRC, WS_KS_PDST, WS_KS_REACH, WS
                          WS_KS_OMEGA_B, WS_KS_TOTAL, WS_KS_ALIVE, WS_KS_ACTIVE, WS_KS_COUNTERS, WS_KS_NPATHS,
                          WS_KS_ROW_ELEMS, WS_KS_LAST, WS_KS_FIRST, WS_KS_ELEM_OFF, WS_KS_GROUP_LANE, WS_KS_GROUP_SRC,
                          WS_KS_LAYERS, WS_KS_WALK_OFF, WS_KS_ELEMS, WS_KS_SCAN_TOTAL};
+constexpr int ws_km[] = {WS_KM_IDS, WS_KM_PIDS, WS_KM_SPURS, WS_KM_LISTS, WS_KM_HAS_SEED, WS_KM_LANE_SPUR,
+                         WS_KM_SEEN, WS_KM_FRONT, WS_KM_NEXT, WS_KM_LEVEL, WS_KM_DONE, WS_KM_GREW, WS_KM_HLEN,
+                         WS_KM_LANE_OFF, WS_KM_COUNTERS, WS_KM_BAN_BITS, WS_KM_BAN_KEYS, WS_KM_STEPS,
+                         WS_KM_STEP_ELEMS};
 constexpr int ws_analytics[] = {WS_LCC_SRC, WS_LCC_OUT, WS_LCC_OUT_VALID, WS_LCC_BIG_ROWS, WS_LCC_BIG_CNT,
                                 WS_LCC_SRC_VALID, WS_LCC_BITMAP, WS_AN_REF_OFF, WS_AN_SCAN, WS_PR_KEY_A, WS_PR_KEY_B,
                                 WS_PR_VAL_A, WS_PR_VAL_B, WS_PR_IN_OFF, WS_PR_SCAN, WS_PR_DFLAG, WS_PR_RANK,
@@ -204,8 +216,8 @@ template <size_t A, size_t... B>
 constexpr bool ws_apart(const int (&a)[A], const int (&...b)[B]) {
 	return (ws_disjoint(a, b) && ...);
 }
-static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_cp, ws_as, ws_ks, ws_analytics,
-                       ws_keys, ws_key_staging),
+static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_cp, ws_as, ws_ks, ws_km,
+                       ws_analytics, ws_keys, ws_key_staging),
               "only the BFS drivers may write the search masks");
 static_assert(ws_apart(ws_staging, ws_driver, ws_bf), "a path entry point's staged columns live while its driver runs");
 static_assert(ws_apart(ws_cp, ws_staging, ws_bf), "the tight search runs on the distances and columns of its call");
@@ -213,6 +225,8 @@ static_assert(ws_apart(ws_as, ws_staging, ws_driver, ws_radix),
               "path counts and step lists live across the batches of their driver, over the columns of their call");
 static_assert(ws_apart(ws_ks, ws_staging, ws_driver, ws_radix, ws_as),
               "the walk search lives across its batches and groups, over the columns of its call and the step lists");
+static_assert(ws_apart(ws_km, ws_staging, ws_driver, ws_radix, ws_as, ws_ks),
+              "the spur searches live across their rounds, over the step lists; WALK's own slots stay apart");
 static_assert(WS_OUT_PATH_OFFSETS < WS_SLOTS && WS_OUT_PATH_VALID < WS_SLOTS, "every slot has a buffer");
 static_assert(ws_apart(ws_radix, ws_csr, ws_analytics, ws_keys), "radix_sort_pairs' scratch is apart from its callers'");
 static_assert(ws_apart(ws_key_staging, ws_keys, ws_csr, ws_radix), "a key build's staged columns live while it builds");

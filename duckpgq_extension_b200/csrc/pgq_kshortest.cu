@@ -391,11 +391,9 @@ static int ks_lanes(const pgq_options *opts, int64_t n_ab, int64_t searches) {
 	return w;
 }
 
-extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
-                                    const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
-                                    int64_t k, int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid,
-                                    int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths,
-                                    pgq_stats *stats) {
+int ks_check_call(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, const pgq_options *opts, int64_t k,
+                  const int64_t *out_npaths, const int64_t *out_first_path, const uint8_t *out_valid,
+                  int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths) {
 	if (!csr) {
 		return pgq_fail(PGQ_ERR_INVALID_ID, "%s", pgq_status_text(PGQ_ERR_INVALID_ID));
 	}
@@ -426,6 +424,16 @@ extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src,
 	if (opts && opts->shard_count > 1) {
 		return pgq_fail(PGQ_ERR_UNSUPPORTED, "shortest_k_paths has no multi-GPU form");
 	}
+	return PGQ_OK;
+}
+
+extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
+                                    const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
+                                    int64_t k, int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid,
+                                    int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths,
+                                    pgq_stats *stats) {
+	PGQ_TRY(ks_check_call(csr, p, src, dst, opts, k, out_npaths, out_first_path, out_valid, out_path_offsets, out_elems,
+	                      out_total_paths));
 	int64_t budget;
 	PGQ_TRY(layer_budget(&budget));
 	const int64_t n = csr->n, m = csr->m, n_ab = csr->n_ab;

@@ -37,6 +37,7 @@
 
 #include "duckdb/catalog/catalog_entry/scalar_function_catalog_entry.hpp"
 #include "duckdb/catalog/catalog_entry/table_function_catalog_entry.hpp"
+#include "duckdb/common/string_util.hpp"
 #include "duckdb/common/vector/flat_vector.hpp"
 #include "duckdb/common/vector/list_vector.hpp"
 #include "duckdb/execution/expression_executor.hpp"
@@ -73,6 +74,7 @@ static std::atomic<int64_t> g_calls_cheapest_path {0};
 static std::atomic<int64_t> g_calls_path_count {0};
 static std::atomic<int64_t> g_calls_all_shortest {0};
 static std::atomic<int64_t> g_calls_shortest_k {0};
+static std::atomic<int64_t> g_calls_shortest_k_mode {0};
 static std::atomic<int64_t> g_calls_lengths {0}, g_calls_paths {0}, g_calls_cheapest {0}, g_pairs {0}, g_uploads {0},
     g_device_builds {0}, g_chunks {0}, g_materialized {0}, g_calls_lcc {0}, g_calls_pagerank {0}, g_calls_wcc {0},
     g_calls_bidirectional {0}, g_calls_w_type {0}, g_calls_reachability {0};
@@ -988,7 +990,32 @@ static unique_ptr<FunctionData> ShortestKPathsBind(BindScalarFunctionInput &inpu
 	return IterativeLengthFunctionData::IterativeLengthBind(input);
 }
 
-static void ShortestKPathsB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+// SQL/PGQ's path mode by name, any case (PGQPathMode's WALK, TRAIL, ACYCLIC, SIMPLE), or -1
+static int32_t PathModeId(const string &name) {
+	const string up = StringUtil::Upper(name);
+	return up == "WALK" ? PGQ_PATH_WALK
+	       : up == "TRAIL" ? PGQ_PATH_TRAIL
+	       : up == "ACYCLIC" ? PGQ_PATH_ACYCLIC
+	       : up == "SIMPLE" ? PGQ_PATH_SIMPLE
+	                        : -1;
+}
+
+// shortest_k_paths(INTEGER, BIGINT, BIGINT, BIGINT, BIGINT k, VARCHAR mode): the 5-argument bind, and a constant mode
+// that names a path mode
+static unique_ptr<FunctionData> ShortestKPathsModeBind(BindScalarFunctionInput &input) {
+	auto &arguments = input.GetArguments();
+	if (!arguments[5]->IsFoldable()) {
+		throw InvalidInputException("the path mode must be constant.");
+	}
+	auto mode = ExpressionExecutor::EvaluateScalar(input.GetClientContext(), *arguments[5]);
+	if (mode.IsNull() || PathModeId(mode.GetValue<string>()) < 0) {
+		throw InvalidInputException("the path mode must be WALK, TRAIL, ACYCLIC or SIMPLE.");
+	}
+	return ShortestKPathsBind(input);
+}
+
+// Both overloads: the rows' lists of pgq_shortest_k_paths_mode (WALK is pgq_shortest_k_paths itself)
+static void ShortestKPathsRows(DataChunk &args, ExpressionState &state, Vector &result, int32_t mode) {
 	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
 	auto &info = func_expr.BindInfo()->Cast<IterativeLengthFunctionData>();
 	auto duckpgq_state = GetDuckPGQState(info.context);
@@ -1003,13 +1030,12 @@ static void ShortestKPathsB200Function(DataChunk &args, ExpressionState &state, 
 	int64_t *offsets = nullptr, *elems = nullptr;
 	int64_t walks = 0;
 	pgq_options opts = OptionsFromEnv();
-	int st = pgq_shortest_k_paths(device_csr, static_cast<int64_t>(count), pairs.src.data(), pairs.dst.data(),
-	                              pairs.valid.data(), nullptr, &opts, k, npaths.data(), first.data(), out_valid.data(),
-	                              &offsets, &elems, &walks, nullptr);
+	int st = pgq_shortest_k_paths_mode(device_csr, static_cast<int64_t>(count), pairs.src.data(), pairs.dst.data(),
+	                                   pairs.valid.data(), nullptr, &opts, k, mode, npaths.data(), first.data(),
+	                                   out_valid.data(), &offsets, &elems, &walks, nullptr);
 	if (st != PGQ_OK) {
 		ThrowStatus(st);
 	}
-	g_calls_shortest_k++;
 	g_pairs += static_cast<int64_t>(count);
 	const idx_t total = static_cast<idx_t>(offsets[walks]);
 	result.SetVectorType(VectorType::FLAT_VECTOR);
@@ -1039,6 +1065,17 @@ static void ShortestKPathsB200Function(DataChunk &args, ExpressionState &state, 
 	}
 	ListVector::SetListSize(result, static_cast<idx_t>(walks));
 	duckpgq_state->csr_to_delete.insert(info.csr_id);
+}
+
+static void ShortestKPathsB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	ShortestKPathsRows(args, state, result, PGQ_PATH_WALK);
+	g_calls_shortest_k++;
+}
+
+static void ShortestKPathsModeB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	// (constant and valid: ShortestKPathsModeBind)
+	ShortestKPathsRows(args, state, result, PathModeId(args.data[5].GetValue(0).GetValue<string>()));
+	g_calls_shortest_k_mode++;
 }
 
 // ---- cheapest_path_length -------------------------------------------------------------------------------
@@ -1286,7 +1323,8 @@ static void B200StatsFunction(DataChunk &args, ExpressionState &state, Vector &r
 	              ",cheapest_path_calls=" + std::to_string(g_calls_cheapest_path.load()) +
 	              ",shortest_path_count_calls=" + std::to_string(g_calls_path_count.load()) +
 	              ",all_shortest_paths_calls=" + std::to_string(g_calls_all_shortest.load()) +
-	              ",shortest_k_paths_calls=" + std::to_string(g_calls_shortest_k.load());
+	              ",shortest_k_paths_calls=" + std::to_string(g_calls_shortest_k.load()) +
+	              ",shortest_k_paths_mode_calls=" + std::to_string(g_calls_shortest_k_mode.load());
 	result.SetVectorType(VectorType::CONSTANT_VECTOR);
 	ConstantVector::GetData<string_t>(result)[0] = StringVector::AddString(result, text);
 }
@@ -1401,10 +1439,16 @@ static void LoadInternal(ExtensionLoader &loader) {
 	    "all_shortest_paths",
 	    {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
 	    LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT)), AllShortestPathsB200Function, AllShortestPathsBind));
-	loader.RegisterFunction(ScalarFunction(
-	    "shortest_k_paths",
+	// shortest_k_paths: the walks (5 arguments) and SQL/PGQ's path modes (a 6th, VARCHAR mode)
+	ScalarFunctionSet shortest_k {Identifier("shortest_k_paths")};
+	shortest_k.AddFunction(ScalarFunction(
 	    {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
 	    LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT)), ShortestKPathsB200Function, ShortestKPathsBind));
+	shortest_k.AddFunction(ScalarFunction({LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT,
+	                                       LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::VARCHAR},
+	                                      LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT)),
+	                                      ShortestKPathsModeB200Function, ShortestKPathsModeBind));
+	loader.RegisterFunction(shortest_k);
 	ScalarFunction stats("duckpgq_b200_stats", {}, LogicalType::VARCHAR, B200StatsFunction);
 	stats.SetVolatile();
 	loader.RegisterFunction(stats);

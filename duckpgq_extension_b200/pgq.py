@@ -30,6 +30,15 @@ from . import _native
 PGQ_OK = 0
 PGQ_ERR_INVALID_ARG, PGQ_ERR_CUDA, PGQ_ERR_OOM, PGQ_ERR_CONSTRAINT = 1, 2, 3, 4
 PGQ_ERR_RANGE, PGQ_ERR_INVALID_ID, PGQ_ERR_NOT_INITIALIZED, PGQ_ERR_UNSUPPORTED = 5, 6, 7, 8
+PGQ_PATH_WALK, PGQ_PATH_TRAIL, PGQ_PATH_ACYCLIC, PGQ_PATH_SIMPLE = 0, 1, 2, 3  # pgq_path_mode
+
+
+def path_mode_id(mode: str) -> int:
+    """SQL/PGQ's path mode by name, any case -> PGQ_PATH_*; another name raises InvalidInputException."""
+    ids = {"WALK": PGQ_PATH_WALK, "TRAIL": PGQ_PATH_TRAIL, "ACYCLIC": PGQ_PATH_ACYCLIC, "SIMPLE": PGQ_PATH_SIMPLE}
+    if not isinstance(mode, str) or mode.upper() not in ids:
+        raise InvalidInputException(PGQ_ERR_INVALID_ARG, f"path mode must be WALK, TRAIL, ACYCLIC or SIMPLE, not {mode!r}")
+    return ids[mode.upper()]
 
 
 class PgqError(RuntimeError):
@@ -471,10 +480,12 @@ class DeviceCSR:
                  for i in range(p)]
         return paths, cnt[:p], st.as_dict()
 
-    def shortest_k_paths(self, src, dst, k: int, src_valid=None, dst_valid=None, options: Optional[Options] = None):
-        """-> (per row: list of [src, e1, v1, ..., dst] walks or None, npaths int64, stats dict): the first min(k,
-        total) walks of each row, shortest first, in step order within a length (include/duckpgq_b200.h,
-        pgq_shortest_k_paths)."""
+    def shortest_k_paths(self, src, dst, k: int, src_valid=None, dst_valid=None, options: Optional[Options] = None,
+                         mode: str = "WALK"):
+        """-> (per row: list of [src, e1, v1, ..., dst] paths or None, npaths int64, stats dict): the first min(k,
+        total) paths of each row in the path mode ("WALK", "TRAIL", "ACYCLIC" or "SIMPLE", any case), shortest first,
+        in step order within a length (include/duckpgq_b200.h, pgq_shortest_k_paths / pgq_shortest_k_paths_mode)."""
+        path_mode = path_mode_id(mode)
         src, dst = _i64(src), _i64(dst)
         p = src.shape[0]
         sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
@@ -486,9 +497,9 @@ class DeviceCSR:
         total = C.c_int64(0)
         st = _native.PgqStats()
         opts = (options or Options()).c()
-        _check(self._lib.pgq_shortest_k_paths(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv), C.byref(opts),
-                                              int(k), _p64(npaths), _p64(first), _pu8(ov), C.byref(offs),
-                                              C.byref(elems), C.byref(total), C.byref(st)))
+        _check(self._lib.pgq_shortest_k_paths_mode(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv), C.byref(opts),
+                                                   int(k), path_mode, _p64(npaths), _p64(first), _pu8(ov),
+                                                   C.byref(offs), C.byref(elems), C.byref(total), C.byref(st)))
         try:
             woff = np.ctypeslib.as_array(offs, shape=(total.value + 1,)).copy()
             flat = np.ctypeslib.as_array(elems, shape=(int(woff[-1]),)).copy() if woff[-1] else np.zeros(0, np.int64)
@@ -722,13 +733,15 @@ def all_shortest_paths(state: DuckPGQState, csr_id: int, v_size: int, src, dst, 
 
 
 def shortest_k_paths(state: DuckPGQState, csr_id: int, v_size: int, src, dst, k: int, src_valid=None, dst_valid=None,
-                     options: Optional[Options] = None):
-    """shortest_k_paths(INT, BIGINT, BIGINT, BIGINT, BIGINT k) -> LIST(LIST(BIGINT)): per row the first min(k, total)
-    walks, shortest first, or None (no reference function; looked up and marked as shortestpath is)."""
+                     options: Optional[Options] = None, mode: str = "WALK"):
+    """shortest_k_paths(INT, BIGINT, BIGINT, BIGINT, BIGINT k[, VARCHAR mode]) -> LIST(LIST(BIGINT)): per row the first
+    min(k, total) paths of the path mode, shortest first, or None (no reference function; looked up and marked as
+    shortestpath is)."""
+    path_mode_id(mode)
     csr = _lookup_for_path(state, csr_id, lengths=False)
     if int(v_size) != csr.n:
         raise InvalidInputException(PGQ_ERR_INVALID_ARG, f"v_size {v_size} does not match the CSR ({csr.n} vertices)")
-    paths, _, _ = csr.shortest_k_paths(src, dst, k, src_valid, dst_valid, options)
+    paths, _, _ = csr.shortest_k_paths(src, dst, k, src_valid, dst_valid, options, mode)
     state.csr_to_delete.add(csr_id)
     return paths
 

@@ -379,6 +379,50 @@ int pgq_shortest_k_paths(pgq_csr *csr, int64_t n_pairs, const int64_t *src, cons
                          int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths,
                          pgq_stats *stats);
 
+/* SQL/PGQ's path modes (PGQPathMode's WALK, TRAIL, ACYCLIC, SIMPLE) */
+typedef enum { PGQ_PATH_WALK = 0, PGQ_PATH_TRAIL = 1, PGQ_PATH_ACYCLIC = 2, PGQ_PATH_SIMPLE = 3 } pgq_path_mode;
+
+/* pgq_shortest_k_paths_mode: SHORTEST k with a path mode (the reference rejects every mode but WALK).  PGQ_PATH_WALK
+ * is pgq_shortest_k_paths itself, bit for bit; any value outside pgq_path_mode -> PGQ_ERR_INVALID_ARG.  For a row
+ * (s, t) and k >= 1:
+ *   - format and order are pgq_shortest_k_paths': a path is [s, e1, v1, ..., eh, t], paths by h, then by their steps
+ *     (the parent's ORIGINAL id, the edge's position in the parent's adjacency) from t back to s.  The result is the
+ *     first min(k, total) paths the mode admits in that order, i.e. pgq_shortest_k_paths' walk sequence filtered to
+ *     the mode, first k; the total is always finite.
+ *   - ACYCLIC: no vertex repeats.  SIMPLE: no vertex repeats except that the first may equal the last (for s != t
+ *     exactly ACYCLIC).  TRAIL: no edge repeats, an edge being an adjacency entry (parent, position): parallel edges
+ *     are distinct, and on an undirected CSR the two directions of an undirected edge are two entries, so a trail may
+ *     go u -> v -> u.  A trail may pass through t and come back to it.
+ *   - s == t: ACYCLIC gives [s] alone; SIMPLE gives [s], then the simple cycles through s (a self-loop on s is one);
+ *     TRAIL gives [s], then the closed trails through s.
+ *   - k = 1 gives pgq_shortestpath's path ([s] when s == t).  When a row has at least k shortest paths, the result is
+ *     pgq_all_shortest_paths(max_paths = k) in every mode (except SIMPLE and TRAIL at s == t).
+ *   - outputs, NULL rows (out_valid 0: a NULL id, or no path), lanes, PGQ_ERR_RANGE, a missing or unfinalised CSR,
+ *     shard_count > 1 and the element-total check (PGQ_ERR_OOM before anything of that size is allocated) are
+ *     pgq_shortest_k_paths'.  PGQ_ERR_UNSUPPORTED when a spur search reaches a vertex 65534 edges from its spur node
+ *     before its target, or when a row accepts a path longer than 65533 edges.
+ *   - the call (DESIGN.md §3): Yen's algorithm with Lawler's rule.  Round 0 runs one search per row with s != t, from
+ *     s with no bans (s == t: path 0 is [s] with no search).  Each later round takes, for every row still short of k
+ *     paths, the path P it accepted last (L edges, found at spur index dev) and runs a spur search from P[j] for
+ *     ACYCLIC, and SIMPLE with s != t, at dev <= j < L; SIMPLE with s == t at j = 0 when P = [s], else dev <= j < L;
+ *     TRAIL at dev <= j <= L.  The search is a BFS from u = P[j] whose first edge avoids edge j of every accepted path
+ *     that shares P's first j steps; ACYCLIC and SIMPLE ban P[0 .. j] (t exempt for SIMPLE at s == t), TRAIL bans P's
+ *     first j edges at every level.  Its path back from t takes the first admissible step in step order.  The new
+ *     candidates join the row's pool unless already known, and each row then accepts its pool's least path; a row
+ *     stops with k paths or an empty pool.  A round's searches take lanes in (row, j) order, W per batch, batches
+ *     never mixing rounds; a search whose spur node has no admissible first edge takes no lane.  W = opts->lanes, or
+ *     for 0 the widest of 512 .. 64 whose level array n x W x 2 bytes fits 4 GiB, halved while W > 64 and the round's
+ *     searches are at most W / 2.  opts->direction, alpha and flags are not used.
+ *   - stats: batches (spur batches over all rounds); lanes (the widest W of the call's rounds, round 0 included);
+ *     searches (spur searches that took a lane); levels (the sum over batches of the forward expansions run: a batch
+ *     expands while a lane that has not reached its target has a non-empty frontier); kernel_launches, h2d_bytes,
+ *     d2h_bytes, total_ms as in pgq_shortest_k_paths.  The other counters are 0. */
+int pgq_shortest_k_paths_mode(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const int64_t *dst,
+                              const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts, int64_t k,
+                              int32_t path_mode, int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid,
+                              int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths,
+                              pgq_stats *stats);
+
 /* ---- the other consumers of the CSR ------------------------------------------------------------------------
  * Host pointers in and out.  As in the reference, "v_size" is n + 2: the two entries n and n + 1 behind the
  * vertices have no edges and take part where the reference lets them.  Results are bit-identical to the reference's.
