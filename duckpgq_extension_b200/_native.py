@@ -124,6 +124,11 @@ SYMBOLS = {
                                        C.POINTER(_P64), C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
     "pgq_shortest_k_paths_mode": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, C.c_int64, C.c_int32, _P64,
                                             _P64, _PU8, C.POINTER(_P64), C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
+    "pgq_shortest_k_groups": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, C.c_int64, C.c_int32, C.c_int64,
+                                        _P64, _P64, _P64, _PU8, _P64, _P64, _PU8, C.POINTER(_P64), C.POINTER(_P64),
+                                        _P64, C.POINTER(PgqStats)]),
+    "pgq_shortest_k_groups_count": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, C.c_int64, _P64, _P64, _P64,
+                                              _PU8, C.POINTER(PgqStats)]),
     "pgq_local_clustering_coefficient": (C.c_int, [_VP, C.c_int64, _P64, _PU8, C.POINTER(C.c_float), _PU8,
                                                    C.POINTER(PgqStats)]),
     "pgq_pagerank": (C.c_int, [_VP, C.c_int64, _P64, _PU8, C.POINTER(C.c_double), _PU8, _P64, C.POINTER(PgqStats)]),

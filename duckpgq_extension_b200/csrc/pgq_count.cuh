@@ -32,3 +32,10 @@ int build_step_lists(pgq_csr *csr, Workspace *ws, cudaStream_t s, const u64 **ke
 int ks_check_call(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, const pgq_options *opts, int64_t k,
                   const int64_t *out_npaths, const int64_t *out_first_path, const uint8_t *out_valid,
                   int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths);
+
+// shortest_k_groups in WALK mode (pgq_kshortest.cu), over arguments pgq_shortest_k_groups has checked
+int kg_walk(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, const uint8_t *src_valid,
+            const uint8_t *dst_valid, const pgq_options *opts, int64_t k, int64_t max_paths, int64_t *out_count,
+            int64_t *out_ngroups, int64_t *out_last_len, uint8_t *out_complete, int64_t *out_npaths,
+            int64_t *out_first_path, uint8_t *out_valid, int64_t **out_path_offsets, int64_t **out_elems,
+            int64_t *out_total_paths, pgq_stats *stats);

@@ -160,6 +160,8 @@ enum WsSlot : int {
 	WS_KM_SEEN = 97, WS_KM_FRONT = 98, WS_KM_NEXT = 99, WS_KM_LEVEL = 100, WS_KM_DONE = 101, WS_KM_GREW = 102,
 	WS_KM_HLEN = 103, WS_KM_LANE_OFF = 104, WS_KM_COUNTERS = 105, WS_KM_BAN_BITS = 106, WS_KM_BAN_KEYS = 107,
 	WS_KM_STEPS = 108, WS_KM_STEP_ELEMS = 109,
+	// shortest_k_groups in WALK mode, on top of shortest_k_paths' slots: each lane's length groups found past h = 0
+	WS_KG_GROUPS = 110,
 	WS_SLOTS // (the last block holds the highest numbers)
 };
 
@@ -189,6 +191,7 @@ constexpr int ws_km[] = {WS_KM_IDS, WS_KM_PIDS, WS_KM_SPURS, WS_KM_LISTS, WS_KM_
                          WS_KM_SEEN, WS_KM_FRONT, WS_KM_NEXT, WS_KM_LEVEL, WS_KM_DONE, WS_KM_GREW, WS_KM_HLEN,
                          WS_KM_LANE_OFF, WS_KM_COUNTERS, WS_KM_BAN_BITS, WS_KM_BAN_KEYS, WS_KM_STEPS,
                          WS_KM_STEP_ELEMS};
+constexpr int ws_kg[] = {WS_KG_GROUPS};
 constexpr int ws_analytics[] = {WS_LCC_SRC, WS_LCC_OUT, WS_LCC_OUT_VALID, WS_LCC_BIG_ROWS, WS_LCC_BIG_CNT,
                                 WS_LCC_SRC_VALID, WS_LCC_BITMAP, WS_AN_REF_OFF, WS_AN_SCAN, WS_PR_KEY_A, WS_PR_KEY_B,
                                 WS_PR_VAL_A, WS_PR_VAL_B, WS_PR_IN_OFF, WS_PR_SCAN, WS_PR_DFLAG, WS_PR_RANK,
@@ -216,7 +219,7 @@ template <size_t A, size_t... B>
 constexpr bool ws_apart(const int (&a)[A], const int (&...b)[B]) {
 	return (ws_disjoint(a, b) && ...);
 }
-static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_cp, ws_as, ws_ks, ws_km,
+static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_cp, ws_as, ws_ks, ws_km, ws_kg,
                        ws_analytics, ws_keys, ws_key_staging),
               "only the BFS drivers may write the search masks");
 static_assert(ws_apart(ws_staging, ws_driver, ws_bf), "a path entry point's staged columns live while its driver runs");
@@ -227,6 +230,8 @@ static_assert(ws_apart(ws_ks, ws_staging, ws_driver, ws_radix, ws_as),
               "the walk search lives across its batches and groups, over the columns of its call and the step lists");
 static_assert(ws_apart(ws_km, ws_staging, ws_driver, ws_radix, ws_as, ws_ks),
               "the spur searches live across their rounds, over the step lists; WALK's own slots stay apart");
+static_assert(ws_apart(ws_kg, ws_staging, ws_driver, ws_radix, ws_as, ws_ks),
+              "the length groups live across the walk search's batches, beside its own slots");
 static_assert(WS_OUT_PATH_OFFSETS < WS_SLOTS && WS_OUT_PATH_VALID < WS_SLOTS, "every slot has a buffer");
 static_assert(ws_apart(ws_radix, ws_csr, ws_analytics, ws_keys), "radix_sort_pairs' scratch is apart from its callers'");
 static_assert(ws_apart(ws_key_staging, ws_keys, ws_csr, ws_radix), "a key build's staged columns live while it builds");

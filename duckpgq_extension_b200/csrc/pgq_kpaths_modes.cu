@@ -24,6 +24,8 @@
 //     Lawler's rule (spurs only at j >= dev) with D gives each candidate once; DESIGN.md §3 has the argument,
 //     including why TRAIL also spurs at j = len(P), past t.
 // The BFS drivers' WS_SEEN / WS_VISIT_* are not touched: the searches have masks of their own (WS_KM_*).
+// shortest_k_groups in these modes runs the same rounds (km_run) with another stop test before a row accepts its pool's
+// least path: an empty pool, k groups and a longer least path, or max_paths paths listed (DESIGN.md §3).
 #include <algorithm>
 #include <cstring>
 #include <map>
@@ -352,6 +354,16 @@ struct KmRow {
 	std::vector<KmPath> acc;
 	std::map<std::vector<int64_t>, KmPath> pool;
 	std::set<std::vector<int64_t>> known;
+	int64_t groups = 0;   // shortest_k_groups: the distinct lengths of acc
+	bool complete = true; // shortest_k_groups: acc holds every path of the row's first k groups
+};
+
+// What a shortest_k_groups call asks of the rounds on top of shortest_k_paths_mode's outputs: k counts length groups,
+// max_paths cuts the lists, and the per-row group results (host arrays of p; count nullable)
+struct KmGroups {
+	int64_t max_paths;
+	int64_t *count, *ngroups, *last_len;
+	uint8_t *complete;
 };
 
 // a spur of the round on the host side: its row and j
@@ -381,20 +393,12 @@ static int km_lanes(const pgq_options *opts, int cap, int64_t searches) {
 	return w;
 }
 
-extern "C" int pgq_shortest_k_paths_mode(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
-                                         const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
-                                         int64_t k, int32_t path_mode, int64_t *out_npaths, int64_t *out_first_path,
-                                         uint8_t *out_valid, int64_t **out_path_offsets, int64_t **out_elems,
-                                         int64_t *out_total_paths, pgq_stats *stats) {
-	if (path_mode == PGQ_PATH_WALK) {
-		return pgq_shortest_k_paths(csr, p, src, dst, src_valid, dst_valid, opts, k, out_npaths, out_first_path,
-		                            out_valid, out_path_offsets, out_elems, out_total_paths, stats);
-	}
-	if (path_mode != PGQ_PATH_TRAIL && path_mode != PGQ_PATH_ACYCLIC && path_mode != PGQ_PATH_SIMPLE) {
-		return pgq_fail(PGQ_ERR_INVALID_ARG, "unknown path mode %d", (int)path_mode);
-	}
-	PGQ_TRY(ks_check_call(csr, p, src, dst, opts, k, out_npaths, out_first_path, out_valid, out_path_offsets, out_elems,
-	                      out_total_paths));
+// shortest_k_paths_mode (kg null) and shortest_k_groups in the TRAIL, ACYCLIC and SIMPLE modes: the rounds of the top.
+// The arguments are checked.
+static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, const uint8_t *src_valid,
+                  const uint8_t *dst_valid, const pgq_options *opts, int64_t k, int32_t path_mode, const KmGroups *kg,
+                  int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid, int64_t **out_path_offsets,
+                  int64_t **out_elems, int64_t *out_total_paths, pgq_stats *stats) {
 	const bool trail = path_mode == PGQ_PATH_TRAIL;
 	const int64_t n = csr->n, m = csr->m;
 	std::vector<int64_t> ids; // the rows whose ids are both valid: sources, then targets
@@ -491,6 +495,7 @@ extern "C" int pgq_shortest_k_paths_mode(pgq_csr *csr, int64_t p, const int64_t 
 			q.el.push_back(src[r.row]);
 			r.known.insert(q.key());
 			r.acc.push_back(std::move(q));
+			r.groups = 1;
 			r.live = k > 1;
 		}
 	}
@@ -716,13 +721,27 @@ extern "C" int pgq_shortest_k_paths_mode(pgq_csr *csr, int64_t p, const int64_t 
 				continue;
 			}
 			auto it = r.pool.begin();
+			if (kg) { // the least path is the row's next: past its k-th group the row is complete, at max_paths cut
+				if (r.groups == k && it->second.h() > r.acc.back().h()) {
+					r.live = false;
+					continue;
+				}
+				if (kg->max_paths && (int64_t)r.acc.size() == kg->max_paths) {
+					r.live = false;
+					r.complete = false;
+					continue;
+				}
+			}
 			if (it->second.h() > KM_PATH_MAX) {
 				return pgq_fail(PGQ_ERR_UNSUPPORTED, "row %lld needs a path longer than %d edges", (long long)r.row,
 				                KM_PATH_MAX);
 			}
+			if (r.acc.empty() || it->second.h() > r.acc.back().h()) {
+				r.groups++;
+			}
 			r.acc.push_back(std::move(it->second));
 			r.pool.erase(it);
-			r.live = (int64_t)r.acc.size() < k;
+			r.live = kg || (int64_t)r.acc.size() < k; // (a row of groups spurs off every path it accepts)
 			any |= r.live;
 		}
 		if (!any) {
@@ -758,6 +777,24 @@ extern "C" int pgq_shortest_k_paths_mode(pgq_csr *csr, int64_t p, const int64_t 
 		out_npaths[r.row] = (int64_t)r.acc.size();
 		out_valid[r.row] = !r.acc.empty();
 	}
+	if (kg) { // NULL rows: no paths, no groups, complete
+		for (int64_t i = 0; i < p; i++) {
+			if (kg->count) {
+				kg->count[i] = 0;
+			}
+			kg->ngroups[i] = 0;
+			kg->last_len[i] = -1;
+			kg->complete[i] = 1;
+		}
+		for (const KmRow &r : rows) {
+			if (kg->count) {
+				kg->count[r.row] = r.complete ? (int64_t)r.acc.size() : -1;
+			}
+			kg->ngroups[r.row] = r.groups;
+			kg->last_len[r.row] = r.acc.empty() ? -1 : r.acc.back().h();
+			kg->complete[r.row] = r.complete;
+		}
+	}
 	int64_t np = 0, ne = 0;
 	size_t ri = 0;
 	for (int64_t i = 0; i < p; i++) {
@@ -780,4 +817,51 @@ extern "C" int pgq_shortest_k_paths_mode(pgq_csr *csr, int64_t p, const int64_t 
 		*stats = st;
 	}
 	return PGQ_OK;
+}
+
+extern "C" int pgq_shortest_k_paths_mode(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
+                                         const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
+                                         int64_t k, int32_t path_mode, int64_t *out_npaths, int64_t *out_first_path,
+                                         uint8_t *out_valid, int64_t **out_path_offsets, int64_t **out_elems,
+                                         int64_t *out_total_paths, pgq_stats *stats) {
+	if (path_mode == PGQ_PATH_WALK) {
+		return pgq_shortest_k_paths(csr, p, src, dst, src_valid, dst_valid, opts, k, out_npaths, out_first_path,
+		                            out_valid, out_path_offsets, out_elems, out_total_paths, stats);
+	}
+	if (path_mode != PGQ_PATH_TRAIL && path_mode != PGQ_PATH_ACYCLIC && path_mode != PGQ_PATH_SIMPLE) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "unknown path mode %d", (int)path_mode);
+	}
+	PGQ_TRY(ks_check_call(csr, p, src, dst, opts, k, out_npaths, out_first_path, out_valid, out_path_offsets, out_elems,
+	                      out_total_paths));
+	return km_run(csr, p, src, dst, src_valid, dst_valid, opts, k, path_mode, nullptr, out_npaths, out_first_path,
+	              out_valid, out_path_offsets, out_elems, out_total_paths, stats);
+}
+
+extern "C" int pgq_shortest_k_groups(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
+                                     const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
+                                     int64_t k, int32_t path_mode, int64_t max_paths, int64_t *out_count,
+                                     int64_t *out_ngroups, int64_t *out_last_len, uint8_t *out_complete,
+                                     int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid,
+                                     int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths,
+                                     pgq_stats *stats) {
+	if (path_mode != PGQ_PATH_WALK && path_mode != PGQ_PATH_TRAIL && path_mode != PGQ_PATH_ACYCLIC &&
+	    path_mode != PGQ_PATH_SIMPLE) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "unknown path mode %d", (int)path_mode);
+	}
+	PGQ_TRY(ks_check_call(csr, p, src, dst, opts, k, out_npaths, out_first_path, out_valid, out_path_offsets, out_elems,
+	                      out_total_paths));
+	if (p > 0 && (!out_ngroups || !out_last_len || !out_complete)) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "null output");
+	}
+	if (max_paths < 0) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "max_paths must be >= 0");
+	}
+	if (path_mode == PGQ_PATH_WALK) {
+		return kg_walk(csr, p, src, dst, src_valid, dst_valid, opts, k, max_paths, out_count, out_ngroups, out_last_len,
+		               out_complete, out_npaths, out_first_path, out_valid, out_path_offsets, out_elems,
+		               out_total_paths, stats);
+	}
+	const KmGroups kg = {max_paths, out_count, out_ngroups, out_last_len, out_complete};
+	return km_run(csr, p, src, dst, src_valid, dst_valid, opts, k, path_mode, &kg, out_npaths, out_first_path,
+	              out_valid, out_path_offsets, out_elems, out_total_paths, stats);
 }

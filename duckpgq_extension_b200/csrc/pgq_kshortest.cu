@@ -31,6 +31,8 @@
 //     prefix before it.  Ranks stay exact under saturation by all_shortest_paths' argument: every rank is below k.
 //     Element offsets: each row's element base is an exclusive scan of the rows' element counts (pgq_path_offsets),
 //     and the walk adds the elements of the shorter walks of its row and of its rank's predecessors.
+// shortest_k_groups in WALK mode runs the same four phases (ks_run) with k_kg_step in place of k_ks_step: k counts
+// length groups, max_paths cuts the lists, and each row's rank bound is its listed count (DESIGN.md §3).
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -223,6 +225,46 @@ __global__ void k_ks_step(int h, int cnt, int L, int64_t n_ab, int64_t k, const 
 		const bool stop = before + take >= (u64)k || !alive[l];
 		alive[l] = 0;
 		if (h > KS_WALK_MAX && (take || !stop)) {
+			ctr[KS_TOO_LONG] = 1;
+		}
+		if (stop) {
+			atomicAnd(&act[l >> 6], ~(1ull << (l & 63)));
+		} else {
+			atomicAdd(&ctr[KS_ACTIVE], 1ull);
+		}
+	}
+}
+
+// After layer h, for shortest_k_groups: a counting lane whose count c at t is non-zero finds length group h (lg counts
+// the groups past h = 0, which s == t is), adds c to its saturating total and lists min(c, the room under max_paths)
+// walks of h edges (all c for max_paths = 0); it stops after its k-th group or when w_h was zero on B(t)
+__global__ void k_kg_step(int h, int cnt, int L, int64_t n_ab, int64_t k, int64_t max_paths,
+                          const int32_t *__restrict__ lane_row, const int32_t *__restrict__ psrc,
+                          const int32_t *__restrict__ pdst, const u64 *__restrict__ cur, uint32_t *alive, u64 *total,
+                          int64_t *lg, u64 *act, int64_t *npaths, int64_t *elems, int64_t *last, u64 *ctr) {
+	for (int l = blockIdx.x * blockDim.x + threadIdx.x; l < cnt; l += gridDim.x * blockDim.x) {
+		if (!((act[l >> 6] >> (l & 63)) & 1)) {
+			continue;
+		}
+		const int row = lane_row[l];
+		const int t = pdst[l];
+		const u64 c = t < n_ab ? cur[(int64_t)t * L + l] : 0;
+		int64_t groups = lg[l] + (psrc[l] == t ? 1 : 0);
+		if (c) {
+			groups++;
+			lg[l]++;
+			total[l] = sat_add(total[l], c);
+			last[row] = h;
+			const u64 listed = (u64)npaths[row];
+			const u64 take = max_paths ? min(c, (u64)max_paths - listed) : c;
+			if (take) {
+				npaths[row] = (int64_t)sat_add(listed, take);
+				elems[row] = (int64_t)sat_add((u64)elems[row], sat_mul_len(take, 2 * (int64_t)h + 1));
+			}
+		}
+		const bool stop = groups >= k || !alive[l];
+		alive[l] = 0;
+		if (h > KS_WALK_MAX && (c || !stop)) {
 			ctr[KS_TOO_LONG] = 1;
 		}
 		if (stop) {
@@ -427,13 +469,21 @@ int ks_check_call(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 	return PGQ_OK;
 }
 
-extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
-                                    const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
-                                    int64_t k, int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid,
-                                    int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths,
-                                    pgq_stats *stats) {
-	PGQ_TRY(ks_check_call(csr, p, src, dst, opts, k, out_npaths, out_first_path, out_valid, out_path_offsets, out_elems,
-	                      out_total_paths));
+// What a shortest_k_groups call asks of the walk driver on top of shortest_k_paths' outputs: k counts length groups,
+// max_paths cuts the lists, and the per-row group results (host arrays of p; count nullable).  count_only stops after
+// the counting pass, with out_valid = the row has a walk.
+struct KgCall {
+	int64_t max_paths;
+	bool count_only;
+	int64_t *count, *ngroups, *last_len;
+	uint8_t *complete;
+};
+
+// shortest_k_paths (kg null) and WALK's shortest_k_groups: the four phases of the top.  The arguments are checked.
+static int ks_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, const uint8_t *src_valid,
+                  const uint8_t *dst_valid, const pgq_options *opts, int64_t k, const KgCall *kg, int64_t *out_npaths,
+                  int64_t *out_first_path, uint8_t *out_valid, int64_t **out_path_offsets, int64_t **out_elems,
+                  int64_t *out_total_paths, pgq_stats *stats) {
 	int64_t budget;
 	PGQ_TRY(layer_budget(&budget));
 	const int64_t n = csr->n, m = csr->m, n_ab = csr->n_ab;
@@ -454,6 +504,12 @@ extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src,
 	memset(&st, 0, sizeof(st));
 	st.lanes = W;
 	st.searches = S;
+	if (p == 0 && kg && kg->count_only) {
+		if (stats) {
+			*stats = st;
+		}
+		return PGQ_OK;
+	}
 	if (p == 0) {
 		*out_path_offsets = (int64_t *)calloc(1, sizeof(int64_t));
 		*out_elems = (int64_t *)malloc(sizeof(int64_t));
@@ -507,6 +563,14 @@ extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src,
 	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ELEM_OFF, b8, (void **)&elem_off));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_GROUP_SRC, (size_t)W * sizeof(int32_t), (void **)&gsrc));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_GROUP_LANE, (size_t)W * sizeof(int32_t), (void **)&glane));
+	int64_t *lg = nullptr;
+	std::vector<u64> h_total; // shortest_k_groups: each lane's walk count N and its groups past h = 0
+	std::vector<int64_t> h_lg;
+	if (kg) {
+		PGQ_TRY(pgq_ws_reserve(ws, WS_KG_GROUPS, (size_t)W * sizeof(int64_t), (void **)&lg));
+		h_total.resize((size_t)S);
+		h_lg.resize((size_t)S);
+	}
 	PGQ_CUDA(cudaEventRecord(ws->ev_begin, s));
 	PGQ_CUDA(cudaMemsetAsync(npaths, 0, b8, s));
 	PGQ_CUDA(cudaMemsetAsync(elems_row, 0, b8, s));
@@ -519,7 +583,9 @@ extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src,
 	}
 	const u64 *step_key = nullptr;
 	const int32_t *step_pos = nullptr;
-	PGQ_TRY(build_step_lists(csr, ws, s, &step_key, &step_pos, &st.kernel_launches));
+	if (!(kg && kg->count_only)) {
+		PGQ_TRY(build_step_lists(csr, ws, s, &step_key, &step_pos, &st.kernel_launches));
+	}
 	const unsigned edge_grid = ks_grid((m + 255) / 256, (int64_t)sms * 16);
 	const unsigned chunk_grid = ks_grid((m + KS_CHUNK * 8 - 1) / (KS_CHUNK * 8), (int64_t)sms * 16);
 	const unsigned cell_grid = ks_grid((cells + 255) / 256, (int64_t)sms * 8);
@@ -536,6 +602,9 @@ extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src,
 		PGQ_CUDA(cudaMemsetAsync(front, 0, (size_t)bcells * sizeof(u64), s));
 		PGQ_CUDA(cudaMemsetAsync(next, 0, (size_t)bcells * sizeof(u64), s));
 		PGQ_CUDA(cudaMemsetAsync(act, 0, (size_t)bwd * sizeof(u64), s));
+		if (kg) {
+			PGQ_CUDA(cudaMemsetAsync(lg, 0, (size_t)cnt * sizeof(int64_t), s));
+		}
 		k_ks_reach_seed<<<lane_grid, 256, 0, s>>>(cnt, bwd, pdst + b0, reach, front);
 		PGQ_CUDA(cudaGetLastError());
 		st.kernel_launches++;
@@ -572,8 +641,13 @@ extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src,
 				                                      reach, act, bwd, alive);
 				st.kernel_launches++;
 			}
-			k_ks_step<<<lane_grid, 256, 0, s>>>(h, cnt, L, n_ab, k, d_lane_row + b0, pdst + b0, cur, alive, total, act,
-			                                    npaths, elems_row, last, ctr);
+			if (kg) {
+				k_kg_step<<<lane_grid, 256, 0, s>>>(h, cnt, L, n_ab, k, kg->max_paths, d_lane_row + b0, psrc + b0, pdst + b0,
+				                                    cur, alive, total, lg, act, npaths, elems_row, last, ctr);
+			} else {
+				k_ks_step<<<lane_grid, 256, 0, s>>>(h, cnt, L, n_ab, k, d_lane_row + b0, pdst + b0, cur, alive, total, act,
+				                                    npaths, elems_row, last, ctr);
+			}
 			PGQ_CUDA(cudaGetLastError());
 			st.kernel_launches++;
 			st.levels++;
@@ -584,6 +658,11 @@ extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src,
 			}
 			std::swap(prev, cur);
 		}
+		if (kg) {
+			PGQ_CUDA(cudaMemcpyAsync(h_total.data() + b0, total, (size_t)cnt * sizeof(u64), cudaMemcpyDeviceToHost, s));
+			PGQ_CUDA(cudaMemcpyAsync(h_lg.data() + b0, lg, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+			st.d2h_bytes += cnt * (int64_t)(sizeof(u64) + sizeof(int64_t));
+		}
 	}
 	// ---- the rows' walk counts and element counts; their first walk and first element ----
 	std::vector<int64_t> h_np((size_t)p), h_el((size_t)p), h_last((size_t)p);
@@ -591,9 +670,51 @@ extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src,
 	PGQ_CUDA(cudaMemcpyAsync(h_el.data(), elems_row, b8, cudaMemcpyDeviceToHost, s));
 	PGQ_CUDA(cudaMemcpyAsync(h_last.data(), last, b8, cudaMemcpyDeviceToHost, s));
 	PGQ_CUDA(cudaStreamSynchronize(s));
+	if (kg) { // the rows' groups: NULL rows have none and are complete
+		std::vector<int64_t> h_count((size_t)p, 0);
+		for (int64_t i = 0; i < p; i++) {
+			kg->ngroups[i] = 0;
+			kg->last_len[i] = -1;
+		}
+		for (int64_t ln = 0; ln < S; ln++) {
+			const int64_t row = lane_row[(size_t)ln];
+			h_count[(size_t)row] = (int64_t)h_total[(size_t)ln];
+			if (h_total[(size_t)ln]) {
+				kg->ngroups[row] = h_lg[(size_t)ln] + (src[row] == dst[row] ? 1 : 0);
+				kg->last_len[row] = h_last[(size_t)row];
+			}
+		}
+		if (kg->count) {
+			memcpy(kg->count, h_count.data(), b8);
+		}
+		if (kg->count_only) {
+			PGQ_CUDA(cudaEventRecord(ws->ev_end, s));
+			PGQ_CUDA(cudaStreamSynchronize(s));
+			g.settled = true;
+			float ms = 0.f;
+			PGQ_CUDA(cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end));
+			for (int64_t i = 0; i < p; i++) {
+				out_valid[i] = h_count[(size_t)i] > 0;
+			}
+			st.total_ms = ms;
+			st.h2d_bytes += 2 * (int64_t)b8 + S * (int64_t)sizeof(int32_t);
+			st.d2h_bytes += 3 * (int64_t)b8;
+			if (stats) {
+				*stats = st;
+			}
+			return PGQ_OK;
+		}
+		for (int64_t i = 0; i < p; i++) {
+			if (kg->max_paths == 0 && (u64)h_count[(size_t)i] == AS_MAX) {
+				return pgq_fail(PGQ_ERR_UNSUPPORTED, "row %lld has at least INT64_MAX walks: list them with max_paths > 0",
+				                (long long)i);
+			}
+			kg->complete[i] = h_np[(size_t)i] == h_count[(size_t)i];
+		}
+	}
 	u64 walks = 0, elem_total = 0;
 	for (int64_t i = 0; i < p; i++) {
-		walks += (u64)h_np[(size_t)i]; // (each at most k <= INT64_MAX, and p < 2^31 of them)
+		walks = sat_add_host(walks, (u64)h_np[(size_t)i]);
 		elem_total = sat_add_host(elem_total, (u64)h_el[(size_t)i]);
 	}
 	if (elem_total > (AS_MAX / sizeof(int64_t)) || walks > (AS_MAX / sizeof(int64_t)) - 1) {
@@ -692,8 +813,8 @@ extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src,
 	h_off[walks] = (int64_t)elem_total;
 	memcpy(out_npaths, h_np.data(), b8);
 	st.total_ms = ms;
-	st.h2d_bytes = 2 * (int64_t)b8 + S * (int64_t)sizeof(int32_t);
-	st.d2h_bytes = 3 * (int64_t)b8 + p + (int64_t)(walks + elem_total) * (int64_t)sizeof(int64_t);
+	st.h2d_bytes += 2 * (int64_t)b8 + S * (int64_t)sizeof(int32_t);
+	st.d2h_bytes += 3 * (int64_t)b8 + p + (int64_t)(walks + elem_total) * (int64_t)sizeof(int64_t);
 	*out_path_offsets = h_off;
 	*out_elems = h_elems;
 	*out_total_paths = (int64_t)walks;
@@ -701,4 +822,41 @@ extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src,
 		*stats = st;
 	}
 	return PGQ_OK;
+}
+
+extern "C" int pgq_shortest_k_paths(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
+                                    const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
+                                    int64_t k, int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid,
+                                    int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths,
+                                    pgq_stats *stats) {
+	PGQ_TRY(ks_check_call(csr, p, src, dst, opts, k, out_npaths, out_first_path, out_valid, out_path_offsets, out_elems,
+	                      out_total_paths));
+	return ks_run(csr, p, src, dst, src_valid, dst_valid, opts, k, nullptr, out_npaths, out_first_path, out_valid,
+	              out_path_offsets, out_elems, out_total_paths, stats);
+}
+
+// shortest_k_groups' WALK (pgq_kpaths_modes.cu checks the call and sends WALK here)
+int kg_walk(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, const uint8_t *src_valid,
+            const uint8_t *dst_valid, const pgq_options *opts, int64_t k, int64_t max_paths, int64_t *out_count,
+            int64_t *out_ngroups, int64_t *out_last_len, uint8_t *out_complete, int64_t *out_npaths,
+            int64_t *out_first_path, uint8_t *out_valid, int64_t **out_path_offsets, int64_t **out_elems,
+            int64_t *out_total_paths, pgq_stats *stats) {
+	const KgCall kg = {max_paths, false, out_count, out_ngroups, out_last_len, out_complete};
+	return ks_run(csr, p, src, dst, src_valid, dst_valid, opts, k, &kg, out_npaths, out_first_path, out_valid,
+	              out_path_offsets, out_elems, out_total_paths, stats);
+}
+
+extern "C" int pgq_shortest_k_groups_count(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
+                                           const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts,
+                                           int64_t k, int64_t *out_count, int64_t *out_ngroups, int64_t *out_last_len,
+                                           uint8_t *out_valid, pgq_stats *stats) {
+	int64_t *no_offsets, *no_elems, no_total;
+	PGQ_TRY(ks_check_call(csr, p, src, dst, opts, k, out_count, out_ngroups, out_valid, &no_offsets, &no_elems,
+	                      &no_total));
+	if (p > 0 && !out_last_len) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "null output");
+	}
+	const KgCall kg = {0, true, out_count, out_ngroups, out_last_len, nullptr};
+	return ks_run(csr, p, src, dst, src_valid, dst_valid, opts, k, &kg, nullptr, nullptr, out_valid, nullptr, nullptr,
+	              nullptr, stats);
 }

@@ -75,6 +75,8 @@ static std::atomic<int64_t> g_calls_path_count {0};
 static std::atomic<int64_t> g_calls_all_shortest {0};
 static std::atomic<int64_t> g_calls_shortest_k {0};
 static std::atomic<int64_t> g_calls_shortest_k_mode {0};
+static std::atomic<int64_t> g_calls_shortest_k_groups {0};
+static std::atomic<int64_t> g_calls_shortest_k_groups_count {0};
 static std::atomic<int64_t> g_calls_lengths {0}, g_calls_paths {0}, g_calls_cheapest {0}, g_pairs {0}, g_uploads {0},
     g_device_builds {0}, g_chunks {0}, g_materialized {0}, g_calls_lcc {0}, g_calls_pagerank {0}, g_calls_wcc {0},
     g_calls_bidirectional {0}, g_calls_w_type {0}, g_calls_reachability {0};
@@ -1014,6 +1016,38 @@ static unique_ptr<FunctionData> ShortestKPathsModeBind(BindScalarFunctionInput &
 	return ShortestKPathsBind(input);
 }
 
+// The rows' path lists of pgq_shortest_k_paths_mode / pgq_shortest_k_groups as LIST(LIST(BIGINT)): row i holds paths
+// first[i] .. first[i] + npaths[i] - 1, path j is elems[offsets[j] .. offsets[j + 1]), and a row with valid[i] = 0 is
+// NULL.  The caller frees offsets and elems.
+static void SetPathLists(Vector &result, idx_t count, const int64_t *offsets, const int64_t *elems, int64_t paths,
+                         const vector<int64_t> &first, const vector<int64_t> &npaths, const vector<uint8_t> &valid) {
+	const idx_t total = static_cast<idx_t>(offsets[paths]);
+	result.SetVectorType(VectorType::FLAT_VECTOR);
+	auto result_data = FlatVector::GetDataMutable<list_entry_t>(result);
+	ValidityMask &result_validity = FlatVector::ValidityMutable(result);
+	ListVector::Reserve(result, static_cast<idx_t>(paths));
+	auto &inner = ListVector::GetChildMutable(result);
+	ListVector::Reserve(inner, total);
+	if (total > 0) {
+		auto leaf = FlatVector::GetDataMutable<int64_t>(ListVector::GetChildMutable(inner));
+		memcpy(leaf, elems, total * sizeof(int64_t));
+	}
+	ListVector::SetListSize(inner, total);
+	auto inner_data = FlatVector::GetDataMutable<list_entry_t>(inner);
+	for (int64_t j = 0; j < paths; j++) {
+		inner_data[j].offset = static_cast<idx_t>(offsets[j]);
+		inner_data[j].length = static_cast<idx_t>(offsets[j + 1] - offsets[j]);
+	}
+	for (idx_t i = 0; i < count; i++) {
+		result_data[i].offset = static_cast<idx_t>(first[i]);
+		result_data[i].length = static_cast<idx_t>(npaths[i]);
+		if (!valid[i]) {
+			result_validity.SetInvalid(i);
+		}
+	}
+	ListVector::SetListSize(result, static_cast<idx_t>(paths));
+}
+
 // Both overloads: the rows' lists of pgq_shortest_k_paths_mode (WALK is pgq_shortest_k_paths itself)
 static void ShortestKPathsRows(DataChunk &args, ExpressionState &state, Vector &result, int32_t mode) {
 	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
@@ -1037,33 +1071,9 @@ static void ShortestKPathsRows(DataChunk &args, ExpressionState &state, Vector &
 		ThrowStatus(st);
 	}
 	g_pairs += static_cast<int64_t>(count);
-	const idx_t total = static_cast<idx_t>(offsets[walks]);
-	result.SetVectorType(VectorType::FLAT_VECTOR);
-	auto result_data = FlatVector::GetDataMutable<list_entry_t>(result);
-	ValidityMask &result_validity = FlatVector::ValidityMutable(result);
-	ListVector::Reserve(result, static_cast<idx_t>(walks));
-	auto &inner = ListVector::GetChildMutable(result);
-	ListVector::Reserve(inner, total);
-	if (total > 0) {
-		auto leaf = FlatVector::GetDataMutable<int64_t>(ListVector::GetChildMutable(inner));
-		memcpy(leaf, elems, total * sizeof(int64_t));
-	}
-	ListVector::SetListSize(inner, total);
-	auto inner_data = FlatVector::GetDataMutable<list_entry_t>(inner);
-	for (int64_t j = 0; j < walks; j++) {
-		inner_data[j].offset = static_cast<idx_t>(offsets[j]);
-		inner_data[j].length = static_cast<idx_t>(offsets[j + 1] - offsets[j]);
-	}
+	SetPathLists(result, count, offsets, elems, walks, first, npaths, out_valid);
 	pgq_free(offsets);
 	pgq_free(elems);
-	for (idx_t i = 0; i < count; i++) {
-		result_data[i].offset = static_cast<idx_t>(first[i]);
-		result_data[i].length = static_cast<idx_t>(npaths[i]);
-		if (!out_valid[i]) {
-			result_validity.SetInvalid(i);
-		}
-	}
-	ListVector::SetListSize(result, static_cast<idx_t>(walks));
 	duckpgq_state->csr_to_delete.insert(info.csr_id);
 }
 
@@ -1076,6 +1086,100 @@ static void ShortestKPathsModeB200Function(DataChunk &args, ExpressionState &sta
 	// (constant and valid: ShortestKPathsModeBind)
 	ShortestKPathsRows(args, state, result, PathModeId(args.data[5].GetValue(0).GetValue<string>()));
 	g_calls_shortest_k_mode++;
+}
+
+// ---- shortest_k_groups (no reference function) --------------------------------------------------------------
+// Every path of the k shortest lengths of a row (include/duckpgq_b200.h, pgq_shortest_k_groups), SQL/PGQ's SHORTEST k
+// GROUP, called as a raw UDF over the CSR CTE like shortest_k_paths.
+// shortest_k_groups(INTEGER, BIGINT, BIGINT, BIGINT, BIGINT k, BIGINT max_paths[, VARCHAR mode]): shortest_k_paths'
+// checks of k and the mode, and a constant max_paths >= 0
+static unique_ptr<FunctionData> ShortestKGroupsBind(BindScalarFunctionInput &input) {
+	auto &arguments = input.GetArguments();
+	if (!arguments[5]->IsFoldable()) {
+		throw InvalidInputException("max_paths must be constant.");
+	}
+	auto max_paths = ExpressionExecutor::EvaluateScalar(input.GetClientContext(), *arguments[5]);
+	if (max_paths.IsNull() || max_paths.GetValue<int64_t>() < 0) {
+		throw InvalidInputException("max_paths must be 0 (every path) or more.");
+	}
+	if (arguments.size() > 6) {
+		if (!arguments[6]->IsFoldable()) {
+			throw InvalidInputException("the path mode must be constant.");
+		}
+		auto mode = ExpressionExecutor::EvaluateScalar(input.GetClientContext(), *arguments[6]);
+		if (mode.IsNull() || PathModeId(mode.GetValue<string>()) < 0) {
+			throw InvalidInputException("the path mode must be WALK, TRAIL, ACYCLIC or SIMPLE.");
+		}
+	}
+	return ShortestKPathsBind(input);
+}
+
+static void ShortestKGroupsB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
+	auto &info = func_expr.BindInfo()->Cast<IterativeLengthFunctionData>();
+	auto duckpgq_state = GetDuckPGQState(info.context);
+	CSR &csr = ShortestPathCsr(*duckpgq_state, info.csr_id);
+	int64_t v_size = args.data[1].GetValue(0).GetValue<int64_t>();
+	// (constant and valid: ShortestKGroupsBind)
+	int64_t k = args.data[4].GetValue(0).GetValue<int64_t>();
+	int64_t max_paths = args.data[5].GetValue(0).GetValue<int64_t>();
+	int32_t mode = args.ColumnCount() > 6 ? PathModeId(args.data[6].GetValue(0).GetValue<string>()) : PGQ_PATH_WALK;
+	PairColumns pairs(args);
+	idx_t count = args.size();
+	auto device_csr = GetB200State(info.context)->ForPathFunction(info.csr_id, csr, v_size);
+	vector<int64_t> ngroups(count), last_len(count), npaths(count), first(count);
+	vector<uint8_t> complete(count), out_valid(count);
+	int64_t *offsets = nullptr, *elems = nullptr;
+	int64_t paths = 0;
+	pgq_options opts = OptionsFromEnv();
+	int st = pgq_shortest_k_groups(device_csr, static_cast<int64_t>(count), pairs.src.data(), pairs.dst.data(),
+	                               pairs.valid.data(), nullptr, &opts, k, mode, max_paths, nullptr, ngroups.data(),
+	                               last_len.data(), complete.data(), npaths.data(), first.data(), out_valid.data(),
+	                               &offsets, &elems, &paths, nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_shortest_k_groups++;
+	g_pairs += static_cast<int64_t>(count);
+	SetPathLists(result, count, offsets, elems, paths, first, npaths, out_valid);
+	pgq_free(offsets);
+	pgq_free(elems);
+	duckpgq_state->csr_to_delete.insert(info.csr_id);
+}
+
+// shortest_k_groups_count(INTEGER, BIGINT, BIGINT, BIGINT, BIGINT k) -> BIGINT: WALK's N, saturated at INT64_MAX, NULL
+// for a row without a walk
+static void ShortestKGroupsCountB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
+	auto &info = func_expr.BindInfo()->Cast<IterativeLengthFunctionData>();
+	auto duckpgq_state = GetDuckPGQState(info.context);
+	CSR &csr = ShortestPathCsr(*duckpgq_state, info.csr_id);
+	int64_t v_size = args.data[1].GetValue(0).GetValue<int64_t>();
+	int64_t k = args.data[4].GetValue(0).GetValue<int64_t>(); // (constant: ShortestKPathsBind)
+	PairColumns pairs(args);
+	idx_t count = args.size();
+	auto device_csr = GetB200State(info.context)->ForPathFunction(info.csr_id, csr, v_size);
+	vector<int64_t> out_count(count), ngroups(count), last_len(count);
+	vector<uint8_t> out_valid(count);
+	pgq_options opts = OptionsFromEnv();
+	int st = pgq_shortest_k_groups_count(device_csr, static_cast<int64_t>(count), pairs.src.data(), pairs.dst.data(),
+	                                     pairs.valid.data(), nullptr, &opts, k, out_count.data(), ngroups.data(),
+	                                     last_len.data(), out_valid.data(), nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_shortest_k_groups_count++;
+	g_pairs += static_cast<int64_t>(count);
+	result.SetVectorType(VectorType::FLAT_VECTOR);
+	auto result_data = FlatVector::GetDataMutable<int64_t>(result);
+	ValidityMask &result_validity = FlatVector::ValidityMutable(result);
+	for (idx_t i = 0; i < count; i++) {
+		result_data[i] = out_count[i];
+		if (!out_valid[i]) {
+			result_validity.SetInvalid(i);
+		}
+	}
+	duckpgq_state->csr_to_delete.insert(info.csr_id);
 }
 
 // ---- cheapest_path_length -------------------------------------------------------------------------------
@@ -1324,7 +1428,9 @@ static void B200StatsFunction(DataChunk &args, ExpressionState &state, Vector &r
 	              ",shortest_path_count_calls=" + std::to_string(g_calls_path_count.load()) +
 	              ",all_shortest_paths_calls=" + std::to_string(g_calls_all_shortest.load()) +
 	              ",shortest_k_paths_calls=" + std::to_string(g_calls_shortest_k.load()) +
-	              ",shortest_k_paths_mode_calls=" + std::to_string(g_calls_shortest_k_mode.load());
+	              ",shortest_k_paths_mode_calls=" + std::to_string(g_calls_shortest_k_mode.load()) +
+	              ",shortest_k_groups_calls=" + std::to_string(g_calls_shortest_k_groups.load()) +
+	              ",shortest_k_groups_count_calls=" + std::to_string(g_calls_shortest_k_groups_count.load());
 	result.SetVectorType(VectorType::CONSTANT_VECTOR);
 	ConstantVector::GetData<string_t>(result)[0] = StringVector::AddString(result, text);
 }
@@ -1449,6 +1555,21 @@ static void LoadInternal(ExtensionLoader &loader) {
 	                                      LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT)),
 	                                      ShortestKPathsModeB200Function, ShortestKPathsModeBind));
 	loader.RegisterFunction(shortest_k);
+	// shortest_k_groups: SHORTEST k GROUP's paths (6 arguments: WALK; a 7th, VARCHAR mode) and WALK's count
+	const auto lists = LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT));
+	ScalarFunctionSet shortest_k_groups {Identifier("shortest_k_groups")};
+	shortest_k_groups.AddFunction(ScalarFunction({LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT,
+	                                              LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
+	                                             lists, ShortestKGroupsB200Function, ShortestKGroupsBind));
+	shortest_k_groups.AddFunction(ScalarFunction({LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT,
+	                                              LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT,
+	                                              LogicalType::VARCHAR},
+	                                             lists, ShortestKGroupsB200Function, ShortestKGroupsBind));
+	loader.RegisterFunction(shortest_k_groups);
+	loader.RegisterFunction(ScalarFunction("shortest_k_groups_count",
+	                                       {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT,
+	                                        LogicalType::BIGINT, LogicalType::BIGINT},
+	                                       LogicalType::BIGINT, ShortestKGroupsCountB200Function, ShortestKPathsBind));
 	ScalarFunction stats("duckpgq_b200_stats", {}, LogicalType::VARCHAR, B200StatsFunction);
 	stats.SetVolatile();
 	loader.RegisterFunction(stats);

@@ -11,6 +11,7 @@ like the reference's own sqllogictests:
     shortest_path_count(id, v_size, src, dst)                         (no reference function: ALL SHORTEST's count)
     all_shortest_paths(id, v_size, src, dst, max_paths)               (no reference function: ALL SHORTEST's lists)
     shortest_k_paths(id, v_size, src, dst, k)                         (no reference function: SHORTEST k's walks)
+    shortest_k_groups(id, v_size, src, dst, k, max_paths)             (no reference function: SHORTEST k GROUP's paths)
     delete_csr(id)                                                    csr_deletion.cpp:10-29
     DuckPGQState.{csr_list, csr_to_delete, get_csr, query_end}        duckpgq_state.hpp:12-39, duckpgq_state.cpp:162-186
 
@@ -510,6 +511,57 @@ class DeviceCSR:
         paths = [walks[first[i]: first[i] + npaths[i]] if ov[i] else None for i in range(p)]
         return paths, npaths[:p], st.as_dict()
 
+    def shortest_k_groups(self, src, dst, k: int, max_paths: int = 0, src_valid=None, dst_valid=None,
+                          options: Optional[Options] = None, mode: str = "WALK"):
+        """-> (per row: list of [src, e1, v1, ..., dst] paths or None, counts int64, ngroups int64, last_len int64,
+        complete uint8, stats dict): every path of the k shortest lengths of each row in the path mode, in
+        shortest_k_paths' order, the first max_paths of them for max_paths > 0.  counts is N, the number of such paths
+        (-1 when a mode's row was cut by max_paths); last_len is the last group's length, -1 for none
+        (include/duckpgq_b200.h, pgq_shortest_k_groups)."""
+        path_mode = path_mode_id(mode)
+        src, dst = _i64(src), _i64(dst)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        dv = None if dst_valid is None else np.ascontiguousarray(dst_valid, dtype=np.uint8)
+        cnt, ngroups, last_len, npaths, first = (np.zeros(max(p, 1), dtype=np.int64) for _ in range(5))
+        complete = np.zeros(max(p, 1), dtype=np.uint8)
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        offs, elems = C.POINTER(C.c_int64)(), C.POINTER(C.c_int64)()
+        total = C.c_int64(0)
+        st = _native.PgqStats()
+        opts = (options or Options()).c()
+        _check(self._lib.pgq_shortest_k_groups(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv), C.byref(opts),
+                                               int(k), path_mode, int(max_paths), _p64(cnt), _p64(ngroups),
+                                               _p64(last_len), _pu8(complete), _p64(npaths), _p64(first), _pu8(ov),
+                                               C.byref(offs), C.byref(elems), C.byref(total), C.byref(st)))
+        try:
+            woff = np.ctypeslib.as_array(offs, shape=(total.value + 1,)).copy()
+            flat = np.ctypeslib.as_array(elems, shape=(int(woff[-1]),)).copy() if woff[-1] else np.zeros(0, np.int64)
+        finally:
+            self._lib.pgq_free(offs)
+            self._lib.pgq_free(elems)
+        walks = [flat[woff[j]: woff[j + 1]].tolist() for j in range(total.value)]
+        paths = [walks[first[i]: first[i] + npaths[i]] if ov[i] else None for i in range(p)]
+        return paths, cnt[:p], ngroups[:p], last_len[:p], complete[:p], st.as_dict()
+
+    def shortest_k_groups_count(self, src, dst, k: int, src_valid=None, dst_valid=None,
+                                options: Optional[Options] = None):
+        """-> (counts int64, ngroups int64, last_len int64, valid uint8, stats dict): WALK's N, saturated at INT64_MAX,
+        with the groups found and the last group's length, from the counting pass alone
+        (include/duckpgq_b200.h, pgq_shortest_k_groups_count)."""
+        src, dst = _i64(src), _i64(dst)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        dv = None if dst_valid is None else np.ascontiguousarray(dst_valid, dtype=np.uint8)
+        cnt, ngroups, last_len = (np.zeros(max(p, 1), dtype=np.int64) for _ in range(3))
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        st = _native.PgqStats()
+        opts = (options or Options()).c()
+        _check(self._lib.pgq_shortest_k_groups_count(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv),
+                                                     C.byref(opts), int(k), _p64(cnt), _p64(ngroups), _p64(last_len),
+                                                     _pu8(ov), C.byref(st)))
+        return cnt[:p], ngroups[:p], last_len[:p], ov[:p], st.as_dict()
+
     def free(self):
         if getattr(self, "_h", None):
             self._lib.pgq_csr_free(self._h)
@@ -744,6 +796,34 @@ def shortest_k_paths(state: DuckPGQState, csr_id: int, v_size: int, src, dst, k:
     paths, _, _ = csr.shortest_k_paths(src, dst, k, src_valid, dst_valid, options, mode)
     state.csr_to_delete.add(csr_id)
     return paths
+
+
+def shortest_k_groups(state: DuckPGQState, csr_id: int, v_size: int, src, dst, k: int, max_paths: int = 0,
+                      src_valid=None, dst_valid=None, options: Optional[Options] = None, mode: str = "WALK"):
+    """shortest_k_groups(INT, BIGINT, BIGINT, BIGINT, BIGINT k, BIGINT max_paths[, VARCHAR mode]) ->
+    LIST(LIST(BIGINT)): per row every path of the path mode whose length is among the row's k shortest, shortest first
+    (the first max_paths of them for max_paths > 0), or None (no reference function; looked up and marked as
+    shortestpath is)."""
+    path_mode_id(mode)
+    csr = _lookup_for_path(state, csr_id, lengths=False)
+    if int(v_size) != csr.n:
+        raise InvalidInputException(PGQ_ERR_INVALID_ARG, f"v_size {v_size} does not match the CSR ({csr.n} vertices)")
+    paths = csr.shortest_k_groups(src, dst, k, max_paths, src_valid, dst_valid, options, mode)[0]
+    state.csr_to_delete.add(csr_id)
+    return paths
+
+
+def shortest_k_groups_count(state: DuckPGQState, csr_id: int, v_size: int, src, dst, k: int, src_valid=None,
+                            dst_valid=None, options: Optional[Options] = None):
+    """shortest_k_groups_count(INT, BIGINT, BIGINT, BIGINT, BIGINT k) -> BIGINT: the number of walks whose length is
+    among the row's k shortest, saturated at INT64_MAX (no reference function; looked up and marked as shortestpath
+    is).  Returns (counts, valid)."""
+    csr = _lookup_for_path(state, csr_id, lengths=False)
+    if int(v_size) != csr.n:
+        raise InvalidInputException(PGQ_ERR_INVALID_ARG, f"v_size {v_size} does not match the CSR ({csr.n} vertices)")
+    counts, _, _, valid, _ = csr.shortest_k_groups_count(src, dst, k, src_valid, dst_valid, options)
+    state.csr_to_delete.add(csr_id)
+    return counts, valid
 
 
 _NOT_INITIALIZED_TEXT = {  # the binds' texts: local_clustering_coefficient.cpp:22, pagerank.cpp:23,

@@ -423,6 +423,57 @@ int pgq_shortest_k_paths_mode(pgq_csr *csr, int64_t n_pairs, const int64_t *src,
                               int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths,
                               pgq_stats *stats);
 
+/* pgq_shortest_k_groups: the paths of the k shortest lengths of a row (SQL/PGQ's SHORTEST k GROUP; the reference
+ * carries the selector in its AST and rejects it).  No reference function.  For a row (s, t), a path mode M (a
+ * pgq_path_mode; another value -> PGQ_ERR_INVALID_ARG) and k >= 1:
+ *   - the length groups of the row are the lengths h at which M admits at least one s -> t path, h_1 < h_2 < ....  The
+ *     result is every M-path whose length is among h_1 .. h_k.  A row has fewer than k groups only when its lengths
+ *     run out (for WALK only when no cycle lies on any s -> t walk).
+ *   - equivalence: the result is the first N paths of pgq_shortest_k_paths_mode's sequence, N = the number of M-paths
+ *     of length <= h_k (the sequence is sorted by length, and a length with no M-path contributes nothing).  Format
+ *     and order are that function's: [s, e1, v1, ..., eh, t], by h, then by step order from t back to s.
+ *   - max_paths: a row lists min(N, max_paths) paths, all N for max_paths = 0.  max_paths < 0 -> PGQ_ERR_INVALID_ARG;
+ *     WALK with max_paths = 0 and a saturated N -> PGQ_ERR_UNSUPPORTED (pgq_all_shortest_paths' rule).
+ *   - per row, besides out_npaths, out_first_path and out_valid (pgq_shortest_k_paths' lists): out_ngroups = the
+ *     groups found (at most k); out_last_len = h of the last group found (-1: none); out_complete = 1 when the listed
+ *     paths are all N.  When max_paths cuts a row in TRAIL, ACYCLIC or SIMPLE mode, out_ngroups and out_last_len
+ *     describe only the groups of the paths listed.  out_count (nullable) = N: for WALK exact and saturated at
+ *     INT64_MAX, from the walk counts; for the other modes exact when out_complete, else -1 (counting trails or simple
+ *     paths is #P-hard: the call does not enumerate past max_paths).  A NULL row has count 0, no groups, last_len -1
+ *     and out_complete 1.
+ *   - s == t: group 1 is h = 0, [s]; WALK goes on with the closed walks through s, SIMPLE with the simple cycles
+ *     through s, TRAIL with the closed trails through s; ACYCLIC has [s] only.
+ *   - k = 1 gives pgq_all_shortest_paths(max_paths) for s != t in every mode (shortest walks are acyclic); for WALK
+ *     out_count then equals pgq_shortest_path_count.
+ *   - NULL rows, PGQ_ERR_RANGE, a missing or unfinalised CSR, lanes, shard_count > 1 -> PGQ_ERR_UNSUPPORTED, the
+ *     65533-edge limit (a group past it -> PGQ_ERR_UNSUPPORTED), the layer budget ((h_k + 1) x n_ab x 8 bytes per row)
+ *     and the element-total check (PGQ_ERR_OOM before anything of that size is allocated) are
+ *     pgq_shortest_k_paths[_mode]'s.
+ *   - the call (DESIGN.md §3).  WALK runs pgq_shortest_k_paths' four phases; only the counting pass's stop rule
+ *     differs: after layer h >= 1 a lane whose count at t is non-zero adds a group, and it stops after its k-th group
+ *     or after a layer whose counts are zero on all of B(t).  The storing pass and the unranking then run over the
+ *     listed paths (a row's rank bound is its listed count).  The other modes run pgq_shortest_k_paths_mode's rounds;
+ *     only a row's stop test differs: before it accepts its pool's least path, a row stops when the pool is empty, or
+ *     when it has k groups and the least path is longer than h_k (complete), or when it already lists max_paths
+ *     paths (max_paths > 0; complete exactly when the pool's least path is not part of the result).  A row that
+ *     accepts a path goes on to the next round, which spurs off it (s == t: [s] is accepted without a search, and the
+ *     row stops there when k = 1).
+ *   - stats: pgq_shortest_k_paths' for WALK, pgq_shortest_k_paths_mode's for the other modes, over the rounds and
+ *     layers this call runs. */
+int pgq_shortest_k_groups(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const int64_t *dst,
+                          const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts, int64_t k,
+                          int32_t path_mode, int64_t max_paths, int64_t *out_count, int64_t *out_ngroups,
+                          int64_t *out_last_len, uint8_t *out_complete, int64_t *out_npaths, int64_t *out_first_path,
+                          uint8_t *out_valid, int64_t **out_path_offsets, int64_t **out_elems,
+                          int64_t *out_total_paths, pgq_stats *stats);
+/* pgq_shortest_k_groups_count: WALK only, the counting pass and nothing after it.  out_count, out_ngroups and
+ * out_last_len as pgq_shortest_k_groups' for WALK; out_valid = the row has a walk (N > 0).  Its errors and stats are
+ * pgq_shortest_k_groups' up to the end of the counting pass (stats: kernel_launches, bytes and total_ms of this call). */
+int pgq_shortest_k_groups_count(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const int64_t *dst,
+                                const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts, int64_t k,
+                                int64_t *out_count, int64_t *out_ngroups, int64_t *out_last_len, uint8_t *out_valid,
+                                pgq_stats *stats);
+
 /* ---- the other consumers of the CSR ------------------------------------------------------------------------
  * Host pointers in and out.  As in the reference, "v_size" is n + 2: the two entries n and n + 1 behind the
  * vertices have no edges and take part where the reference lets them.  Results are bit-identical to the reference's.
