@@ -13,7 +13,8 @@
  *   - the paths are enumerated by a depth-first search back from t that tries, at a node of depth k, its in-edges from
  *     vertices of depth k - 1 in step order (the parent's id, then the edge's position in the parent's adjacency) and
  *     stops after max_paths complete paths (0 = all of them).  The device unranks instead; the two meet only in the
- *     order both are defined by.
+ *     order both are defined by.  A row whose elements would pass INT64_MAX bytes is refused (ORC_ERR_ALLOC) before
+ *     its enumeration starts, as the device refuses the call (PGQ_ERR_OOM).
  */
 #include <stdint.h>
 #include <stdlib.h>
@@ -234,6 +235,11 @@ int orc_all_shortest_paths(int64_t n, const int64_t *v, const int64_t *e, const 
 				last = src[i];
 			}
 			const int64_t h = a.dist[dst[i]], len = 2 * h + 1;
+			const int64_t np = max_paths > 0 && max_paths < out_count[i] ? max_paths : out_count[i];
+			if (np > INT64_MAX / (int64_t)sizeof(int64_t) / len) {
+				rc = ORC_ERR_ALLOC; /* the row's elements do not fit in memory: refuse before enumerating */
+				goto done;
+			}
 			a.limit = max_paths;
 			a.emitted = 0;
 			rc = enumerate(&a, dst[i], h, len);

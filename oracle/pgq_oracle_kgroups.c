@@ -10,7 +10,9 @@
  *   - WALK: B(t) by a sequential BFS back from t; the layers w_h(u) = the number of h-edge walks s -> u on B(t),
  *     saturated at INT64_MAX, every layer kept; a row stops after its k-th length group or after a layer that is zero
  *     on all of B(t).  The walks of each group length are enumerated by a depth-first search back from t in step
- *     order, until max_paths are listed.  The stats simulate the batches at the lane width.
+ *     order, until max_paths are listed; a row whose elements would pass INT64_MAX bytes is refused (ORC_ERR_ALLOC)
+ *     before its enumeration starts, as the device refuses the call (PGQ_ERR_OOM).  The stats simulate the batches at
+ *     the lane width.
  *   - TRAIL, ACYCLIC, SIMPLE: Yen's algorithm with Lawler's rule, a plain BFS per spur search and a sorted array as the
  *     pool; before it accepts its pool's least path a row stops when the pool is empty, when it has k groups and the
  *     least path is longer than its last group's length, or when it lists max_paths paths already (then complete
@@ -254,6 +256,13 @@ static int walk_row(orc_kg *a, int64_t s, int64_t t, int64_t k, int64_t max_path
 	}
 	if (max_paths == 0 && r->count == INT64_MAX) {
 		return ORC_ERR_UNSUPPORTED;
+	}
+	for (int64_t h = 0, np = 0; h <= r->last; h++) { /* refuse a row whose elements do not fit in memory */
+		const int64_t c = a->layer[h][t], room = max_paths ? max_paths - np : c, want = c < room ? c : room;
+		if (want > INT64_MAX / (int64_t)sizeof(int64_t) / (2 * h + 1)) {
+			return ORC_ERR_ALLOC;
+		}
+		np += want;
 	}
 	for (int64_t h = 0; h <= r->last; h++) {
 		const int64_t c = a->layer[h][t];
