@@ -116,6 +116,9 @@ SYMBOLS = {
     "pgq_cheapest_path_length": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, _PU8, C.POINTER(PgqStats)]),
     "pgq_cheapest_path": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _P64, _P64, _PU8, C.POINTER(_P64), _P64,
                                     C.POINTER(PgqStats)]),
+    "pgq_cheapest_path_count": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _P64, _PU8, C.POINTER(PgqStats)]),
+    "pgq_all_cheapest_paths": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, C.c_int64, _P64, _P64, _P64, _PU8,
+                                         C.POINTER(_P64), C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
     "pgq_shortest_path_count": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, _P64, _PU8,
                                           C.POINTER(PgqStats)]),
     "pgq_all_shortest_paths": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, C.c_int64, _P64, _P64, _P64, _P64,

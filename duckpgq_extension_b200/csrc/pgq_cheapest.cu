@@ -30,9 +30,20 @@
 // cheapest_path_length cost bit for bit, and the path has the fewest edges among the cheapest.  d(s) != 0 only through
 // the sentinel arithmetic of a weight of -inf (or, for BIGINT, below about -max/2) on an edge into s, or a DOUBLE cycle
 // through a -inf edge: the path follows the same rule, but its sum is not promised to be the cost.
+//
+// cheapest_path_count / all_cheapest_paths (SQL/PGQ's ALL CHEAPEST) run the same sweeps and then, per batch, the walk
+// engine of shortest_k_paths (pgq_count.cuh, pgq_kshortest.cu's top) over the tight edges of each lane: a BFS back from
+// t over the tight in-edges gives B(t) (s outside it: NULL), and the tight walks from s inside B(t) are counted layer
+// by layer.  A lane stops after the layer h where the counts are zero on B(t) (exact), where its total saturates, or
+// once h >= |B(t)| with counts still alive: such a walk of |B(t)| edges inside B(t) repeats a vertex, so a tight cycle
+// lies on an s -> t route and the count is infinite (INT64_MAX); a list of max_paths > 0 walks counts on until it has
+// them.  Then the listed walks are stored and unranked as in shortest_k_paths, their offsets continuing batch to batch.
 #include <algorithm>
+#include <cstdlib>
 #include <cstring>
+#include <vector>
 
+#include "pgq_count.cuh"
 #include "pgq_tile.cuh"
 
 #define BF_INF_I64 (0x7fffffffffffffffLL / 2)
@@ -614,4 +625,561 @@ extern "C" int pgq_cheapest_path(pgq_csr *csr, int64_t p, const int64_t *src, co
 		*stats = st;
 	}
 	return PGQ_OK;
+}
+
+// ---- cheapest_path_count / all_cheapest_paths: the walk engine over the tight edges of a batch (see the top) ---------
+// The call's counters: [0] a backward level added a bit (k_ks_reach_update); [1] lanes still counting; [2] a lane still
+// counts after layer KS_WALK_MAX
+enum { AC_CHANGED = 0, AC_ACTIVE = 1, AC_TOO_LONG = 2 };
+
+// The tight edges of a batch as the walk kernels' edge filter (pgq_count.cuh).  The kernels walk the step lists, whose
+// entry e carries the out-CSR position pos[e] of its edge, and so its weight; kernel lane l is lane lane_map[l] of the
+// batch (l itself without a map).  The rule is k_tight_level's: d(from) + w == d(to) in the weight type's arithmetic.
+template <bool F64>
+struct TightEdges {
+	const u64 *dist;
+	int L;
+	const int64_t *w_bits;
+	const int32_t *pos;
+	const int32_t *lane_map;
+	__device__ __forceinline__ bool edge(int64_t e, int64_t from, int64_t to, int l) const {
+		const int bl = lane_map ? lane_map[l] : l;
+		const u64 dv = dist[from * L + bl], du = dist[to * L + bl];
+		const int64_t w = w_bits[pos[e]];
+		if (F64) {
+			return key_f64(dv) + __longlong_as_double(w) == key_f64(du);
+		}
+		return dv + (u64)w == du;
+	}
+	__device__ __forceinline__ u64 lanes(int64_t e, int64_t from, int64_t to, int j, u64 cand) const {
+		u64 out = 0;
+		while (cand) {
+			const int b = __ffsll((long long)cand) - 1;
+			cand &= cand - 1;
+			if (edge(e, from, to, j * 64 + b)) {
+				out |= 1ull << b;
+			}
+		}
+		return out;
+	}
+};
+
+// par[e] = the internal id of the parent of step-list entry e: the in-lists the tight kernels walk in place of in_adj,
+// so that entry e's out-CSR position is step_pos[e].  A warp per in-list.
+__global__ void __launch_bounds__(256) k_ac_step_par(int64_t n, int64_t n_ab, const int32_t *__restrict__ in_off,
+                                                     const u64 *__restrict__ step_key, const int32_t *__restrict__ perm,
+                                                     int32_t *par) {
+	const int lane = threadIdx.x & 31;
+	const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+	for (int64_t u = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; u < n_ab; u += nwarps) {
+		const u64 key0 = (u64)u * (u64)n;
+		for (int e = in_off[u] + lane; e < in_off[u + 1]; e += 32) {
+			par[e] = perm[(int)(step_key[e] - key0)];
+		}
+	}
+}
+
+// Each lane of the batch: its row, its internal ids, and whether it is open -- both ids valid and s == t or a cost at t
+// (k_tight_seed's rule).  An open lane seeds its target into the backward reach.  One thread per lane.
+template <bool F64>
+__global__ void k_ac_lanes(int b0, int cnt, int L, int wd, const int64_t *__restrict__ src, const int64_t *__restrict__ dst,
+                           const uint8_t *__restrict__ src_valid, const uint8_t *__restrict__ dst_valid,
+                           const int32_t *__restrict__ perm, int64_t n, const u64 *__restrict__ dist, int32_t *psrc,
+                           int32_t *pdst, int32_t *lane_row, uint32_t *open, u64 *reach, u64 *front) {
+	const int l = blockIdx.x * blockDim.x + threadIdx.x;
+	if (l >= cnt) {
+		return;
+	}
+	const int64_t row = b0 + l;
+	const int64_t s = src[row], t = dst[row];
+	int ps = 0, pt = 0;
+	bool op = false;
+	if ((!src_valid || src_valid[row]) && (!dst_valid || dst_valid[row]) && s >= 0 && s < n && t >= 0 && t < n) {
+		ps = perm[s];
+		pt = perm[t];
+		const u64 k = dist[(int64_t)pt * L + l];
+		op = s == t || (F64 ? key_f64(k) != 1.7976931348623157e308 / 2 : (long long)k != BF_INF_I64);
+	}
+	lane_row[l] = (int32_t)row;
+	psrc[l] = ps;
+	pdst[l] = pt;
+	open[l] = op;
+	if (op) {
+		const int64_t cell = (int64_t)pt * wd + (l >> 6);
+		atomicOr(&reach[cell], 1ull << (l & 63));
+		atomicOr(&front[cell], 1ull << (l & 63));
+	}
+}
+
+// |B_tight(t)| of each lane: a thread per lane, a block per slice of the vertices
+__global__ void k_ac_bsize(int64_t n, int wd, const u64 *__restrict__ reach, unsigned long long *bsize) {
+	const int l = threadIdx.x;
+	unsigned long long c = 0;
+	for (int64_t v = blockIdx.x; v < n; v += gridDim.x) {
+		c += (reach[v * wd + (l >> 6)] >> (l & 63)) & 1;
+	}
+	if (c) {
+		atomicAdd(&bsize[l], c);
+	}
+}
+
+// Layer 0 of each lane: NULL unless the lane is open and s lies in B_tight(t); then the lane counts, with [s] as its walk
+// of 0 edges when s == t
+__global__ void k_ac_start(int cnt, int wd, bool list, const int32_t *__restrict__ lane_row,
+                           const int32_t *__restrict__ psrc, const int32_t *__restrict__ pdst,
+                           const uint32_t *__restrict__ open, const u64 *__restrict__ reach, u64 *total, uint32_t *inf,
+                           u64 *act, int64_t *count, int64_t *npaths, int64_t *elems, int64_t *last, u64 *ctr) {
+	for (int l = blockIdx.x * blockDim.x + threadIdx.x; l < cnt; l += gridDim.x * blockDim.x) {
+		const int row = lane_row[l];
+		const int s = psrc[l], t = pdst[l];
+		const bool in_b = open[l] && ((reach[(int64_t)s * wd + (l >> 6)] >> (l & 63)) & 1);
+		const int64_t c0 = in_b && s == t ? 1 : 0;
+		total[l] = c0;
+		inf[l] = 0;
+		count[row] = c0;
+		npaths[row] = list ? c0 : 0;
+		elems[row] = list ? c0 : 0;
+		last[row] = c0 ? 0 : -1;
+		if (in_b) {
+			atomicOr(&act[l >> 6], 1ull << (l & 63));
+			atomicAdd(&ctr[AC_ACTIVE], 1ull);
+		}
+	}
+}
+
+// After layer h: each counting lane adds its count c at t to its saturating total and lists min(c, the room under
+// max_paths) walks of h edges (all c for max_paths = 0; none for a count).  It stops after the layer where w_h was zero
+// on B_tight(t) (the count is exact), where its total saturates, or once w_h is alive at h >= |B_tight(t)| (the count is
+// infinite: DESIGN.md section 3) -- at once when it lists nothing more or max_paths = 0, else when it has max_paths walks.
+__global__ void k_ac_step(int h, int cnt, int L, int64_t n_ab, bool list, int64_t max_paths,
+                          const int32_t *__restrict__ lane_row, const int32_t *__restrict__ pdst,
+                          const u64 *__restrict__ cur, const unsigned long long *__restrict__ bsize, uint32_t *alive,
+                          u64 *total, uint32_t *inf, u64 *act, int64_t *count, int64_t *npaths, int64_t *elems,
+                          int64_t *last, u64 *ctr) {
+	for (int l = blockIdx.x * blockDim.x + threadIdx.x; l < cnt; l += gridDim.x * blockDim.x) {
+		if (!((act[l >> 6] >> (l & 63)) & 1)) {
+			continue;
+		}
+		const int row = lane_row[l];
+		const int t = pdst[l];
+		const u64 c = t < n_ab ? cur[(int64_t)t * L + l] : 0;
+		const u64 tot = sat_add(total[l], c);
+		total[l] = tot;
+		const u64 listed = (u64)npaths[row];
+		const u64 take = !list ? 0 : max_paths ? min(c, (u64)max_paths - listed) : c;
+		if (take) {
+			npaths[row] = (int64_t)sat_add(listed, take);
+			elems[row] = (int64_t)sat_add((u64)elems[row], sat_mul_len(take, 2 * (int64_t)h + 1));
+			last[row] = h;
+		}
+		const bool live = alive[l] != 0;
+		alive[l] = 0;
+		const bool infinite = inf[l] || (live && (u64)h >= (u64)bsize[l]);
+		inf[l] = infinite;
+		count[row] = infinite ? (int64_t)AS_MAX : (int64_t)tot;
+		const bool stop = !live || tot == AS_MAX || (infinite && (!list || max_paths == 0 || listed + take >= (u64)max_paths));
+		if (h >= KS_WALK_MAX && !stop) {
+			ctr[AC_TOO_LONG] = 1;
+		}
+		if (stop) {
+			atomicAnd(&act[l >> 6], ~(1ull << (l & 63)));
+		} else {
+			atomicAdd(&ctr[AC_ACTIVE], 1ull);
+		}
+	}
+}
+
+static inline unsigned ac_grid(int64_t want, int64_t cap) {
+	return (unsigned)std::max<int64_t>(1, std::min<int64_t>(want, cap));
+}
+
+static inline u64 ac_sat_add(u64 a, u64 b) { // a, b <= INT64_MAX
+	return a > AS_MAX - b ? AS_MAX : a + b;
+}
+
+// What both calls keep across the batches: the per-row results on the device ([p]) and, for the lists, the walks so far
+struct AcCall {
+	bool list;
+	int64_t max_paths, budget;
+	const u64 *step_key;
+	const int32_t *step_pos, *step_par;
+	int64_t *count, *npaths, *elems_row, *last, *first, *elem_off;
+	uint8_t *valid;
+	u64 walks, elem_total; // listed so far
+};
+
+// The tight walk search of every batch, behind its sweeps (run_bf's AfterSweeps): the tight backward reach, the counting
+// pass, and for the lists the storing pass and the unranking, whose offsets continue the previous batch's.
+template <bool F64>
+struct TightWalks {
+	pgq_csr *csr;
+	Workspace *ws;
+	const int64_t *d_src, *d_dst;
+	const uint8_t *d_sv, *d_dv;
+	pgq_stats *st;
+	AcCall *call;
+	int operator()(int b0, int cnt, int L, const u64 *dist) const {
+		cudaStream_t s = ws->stream;
+		const int64_t n = csr->n, m = csr->m, n_ab = csr->n_ab;
+		const int sms = csr->ctx->sm_count;
+		const int wd = (L + 63) / 64;
+		const int64_t cells = std::max<int64_t>(n, 1) * wd;
+		const size_t layer = (size_t)std::max<int64_t>(n_ab, 1) * L * sizeof(u64);
+		int32_t *psrc, *pdst, *lane_row;
+		uint32_t *open, *alive, *inf;
+		u64 *reach, *front, *next, *om_a, *om_b, *total, *act, *ctr;
+		unsigned long long *bsize;
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_PSRC, (size_t)L * sizeof(int32_t), (void **)&psrc));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_PDST, (size_t)L * sizeof(int32_t), (void **)&pdst));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_LANE_ROW, (size_t)L * sizeof(int32_t), (void **)&lane_row));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_OPEN, (size_t)L * sizeof(uint32_t), (void **)&open));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_REACH, (size_t)cells * sizeof(u64), (void **)&reach));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_FRONT, (size_t)cells * sizeof(u64), (void **)&front));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_NEXT, (size_t)cells * sizeof(u64), (void **)&next));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_BSIZE, (size_t)L * sizeof(u64), (void **)&bsize));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_OMEGA_A, layer, (void **)&om_a));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_OMEGA_B, layer, (void **)&om_b));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_TOTAL, (size_t)L * sizeof(u64), (void **)&total));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_ALIVE, (size_t)L * sizeof(uint32_t), (void **)&alive));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_INF, (size_t)L * sizeof(uint32_t), (void **)&inf));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_ACTIVE, (size_t)wd * sizeof(u64), (void **)&act));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_COUNTERS, 256, (void **)&ctr));
+		PGQ_CUDA(cudaMemsetAsync(reach, 0, (size_t)cells * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(front, 0, (size_t)cells * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(next, 0, (size_t)cells * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(bsize, 0, (size_t)L * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(alive, 0, (size_t)L * sizeof(uint32_t), s));
+		PGQ_CUDA(cudaMemsetAsync(act, 0, (size_t)wd * sizeof(u64), s));
+		const TightEdges<F64> tight {dist, L, csr->w_bits, call->step_pos, nullptr};
+		k_ac_lanes<F64><<<(cnt + 127) / 128, 128, 0, s>>>(b0, cnt, L, wd, d_src, d_dst, d_sv, d_dv, csr->perm, n, dist, psrc,
+		                                                 pdst, lane_row, open, reach, front);
+		PGQ_CUDA(cudaGetLastError());
+		st->kernel_launches++;
+		// ---- the tight backward reach ----
+		u64 h_ctr[3];
+		const unsigned edge_grid = ac_grid((m + 255) / 256, (int64_t)sms * 16);
+		for (;;) {
+			PGQ_CUDA(cudaMemsetAsync(&ctr[AC_CHANGED], 0, sizeof(u64), s));
+			if (m > 0) {
+				k_ks_reach_level<<<edge_grid, 256, 0, s>>>(m, n_ab, wd, csr->in.off, call->step_par, front, reach, next, tight);
+				st->kernel_launches++;
+			}
+			k_ks_reach_update<<<ac_grid((cells + 255) / 256, (int64_t)sms * 8), 256, 0, s>>>(cells, reach, front, next, ctr);
+			PGQ_CUDA(cudaGetLastError());
+			st->kernel_launches++;
+			st->push_levels++;
+			PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(u64), cudaMemcpyDeviceToHost, s));
+			PGQ_CUDA(cudaStreamSynchronize(s));
+			if (!h_ctr[AC_CHANGED]) {
+				break;
+			}
+		}
+		k_ac_bsize<<<ac_grid(n, (int64_t)sms * 8), L, 0, s>>>(n, wd, reach, bsize);
+		PGQ_CUDA(cudaMemsetAsync(ctr, 0, 3 * sizeof(u64), s));
+		k_ac_start<<<(cnt + 255) / 256, 256, 0, s>>>(cnt, wd, call->list, lane_row, psrc, pdst, open, reach, total, inf, act,
+		                                             call->count, call->npaths, call->elems_row, call->last, ctr);
+		PGQ_CUDA(cudaGetLastError());
+		st->kernel_launches += 2;
+		PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaStreamSynchronize(s));
+		// ---- the counting pass ----
+		const unsigned chunk_grid = ac_grid((m + KS_CHUNK * 8 - 1) / (KS_CHUNK * 8), (int64_t)sms * 16);
+		u64 *prev = om_a, *cur = om_b;
+		for (int h = 1; h_ctr[AC_ACTIVE] > 0; h++) {
+			PGQ_CUDA(cudaMemsetAsync(cur, 0, layer, s));
+			PGQ_CUDA(cudaMemsetAsync(&ctr[AC_ACTIVE], 0, sizeof(u64), s));
+			if (m > 0) {
+				k_ks_omega<<<chunk_grid, 256, 0, s>>>(h, m, n_ab, L, cnt, csr->in.off, call->step_par, psrc, prev, cur, reach,
+				                                      act, wd, alive, tight);
+				st->kernel_launches++;
+			}
+			k_ac_step<<<(cnt + 255) / 256, 256, 0, s>>>(h, cnt, L, n_ab, call->list, call->max_paths, lane_row, pdst, cur,
+			                                            bsize, alive, total, inf, act, call->count, call->npaths,
+			                                            call->elems_row, call->last, ctr);
+			PGQ_CUDA(cudaGetLastError());
+			st->kernel_launches++;
+			st->pull_levels++;
+			PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, s));
+			PGQ_CUDA(cudaStreamSynchronize(s));
+			if (h_ctr[AC_TOO_LONG]) {
+				return pgq_fail(PGQ_ERR_UNSUPPORTED, "a row still counts cheapest paths after %d edges", KS_WALK_MAX);
+			}
+			std::swap(prev, cur);
+		}
+		if (!call->list) {
+			return PGQ_OK;
+		}
+		// ---- the batch's walks and elements: checked, then placed behind the previous batches' ----
+		std::vector<int64_t> h_count((size_t)cnt), h_np((size_t)cnt), h_el((size_t)cnt), h_last((size_t)cnt);
+		PGQ_CUDA(cudaMemcpyAsync(h_count.data(), call->count + b0, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaMemcpyAsync(h_np.data(), call->npaths + b0, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaMemcpyAsync(h_el.data(), call->elems_row + b0, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaMemcpyAsync(h_last.data(), call->last + b0, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaStreamSynchronize(s));
+		st->d2h_bytes += 4 * cnt * (int64_t)sizeof(int64_t);
+		u64 walks = call->walks, elem_total = call->elem_total;
+		for (int l = 0; l < cnt; l++) {
+			if (call->max_paths == 0 && (u64)h_count[(size_t)l] == AS_MAX) {
+				return pgq_fail(PGQ_ERR_UNSUPPORTED, "row %lld has INT64_MAX or infinitely many cheapest paths: list them with "
+				                "max_paths > 0", (long long)(b0 + l));
+			}
+			walks = ac_sat_add(walks, (u64)h_np[(size_t)l]);
+			elem_total = ac_sat_add(elem_total, (u64)h_el[(size_t)l]);
+		}
+		if (elem_total > (AS_MAX / sizeof(int64_t)) || walks > (AS_MAX / sizeof(int64_t)) - 1) {
+			return pgq_fail(PGQ_ERR_OOM, "the cheapest paths of one call hold too many elements (%llu)",
+			                (unsigned long long)elem_total);
+		}
+		int64_t *d_scan, *walk_off, *d_elems;
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_SCAN_TOTAL, sizeof(int64_t), (void **)&d_scan));
+		pgq_path_offsets((int64_t)call->elem_total, b0, (int64_t)b0 + cnt, call->elem_off, call->elems_row, call->valid,
+		                 d_scan, s);
+		pgq_path_offsets((int64_t)call->walks, b0, (int64_t)b0 + cnt, call->first, call->npaths, call->valid, d_scan, s);
+		PGQ_CUDA(cudaGetLastError());
+		st->kernel_launches += 2;
+		PGQ_TRY(pgq_ws_grow(ws, WS_AC_WALK_OFF, (size_t)(walks + 1) * sizeof(int64_t), (size_t)call->walks * sizeof(int64_t),
+		                    s, (void **)&walk_off));
+		PGQ_TRY(pgq_ws_grow(ws, WS_AC_ELEMS, (size_t)elem_total * sizeof(int64_t),
+		                    (size_t)call->elem_total * sizeof(int64_t), s, (void **)&d_elems));
+		call->walks = walks;
+		call->elem_total = elem_total;
+		// ---- the storing pass and the unranking, group by group (ks_run's grouping under the layer budget) ----
+		int32_t *glane, *gsrc;
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_GROUP_LANE, (size_t)L * sizeof(int32_t), (void **)&glane));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_GROUP_SRC, (size_t)L * sizeof(int32_t), (void **)&gsrc));
+		std::vector<int32_t> grp;
+		int64_t grp_h = 0;
+		auto layer_bytes = [&](int64_t h, int64_t rows) { return (double)(h + 1) * (double)n_ab * (double)rows * 8.0; };
+		auto run_group = [&]() -> int {
+			const int ng = (int)grp.size();
+			if (ng == 0) {
+				return PGQ_OK;
+			}
+			u64 *layers;
+			PGQ_TRY(pgq_ws_reserve(ws, WS_AC_LAYERS, (size_t)std::max<int64_t>(grp_h, 1) * n_ab * ng * sizeof(u64),
+			                       (void **)&layers));
+			PGQ_CUDA(cudaMemcpyAsync(glane, grp.data(), (size_t)ng * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+			k_ks_group_src<<<ac_grid((ng + 255) / 256, 64), 256, 0, s>>>(ng, glane, psrc, gsrc);
+			PGQ_CUDA(cudaGetLastError());
+			st->kernel_launches++;
+			st->h2d_bytes += ng * (int64_t)sizeof(int32_t);
+			if (grp_h > 0) {
+				PGQ_CUDA(cudaMemsetAsync(layers, 0, (size_t)grp_h * n_ab * ng * sizeof(u64), s));
+			}
+			const TightEdges<F64> gtight {dist, L, csr->w_bits, call->step_pos, glane};
+			for (int64_t h = 1; h <= grp_h && m > 0; h++) {
+				u64 *lcur = layers + (h - 1) * n_ab * ng;
+				const u64 *lprev = h >= 2 ? layers + (h - 2) * n_ab * ng : nullptr;
+				k_ks_omega<<<chunk_grid, 256, 0, s>>>((int)h, m, n_ab, ng, ng, csr->in.off, call->step_par, gsrc, lprev, lcur,
+				                                      nullptr, nullptr, 0, nullptr, gtight);
+				st->kernel_launches++;
+			}
+			k_ks_unrank<<<ac_grid(ng, (int64_t)sms * 16), 256, 0, s>>>(
+			    ng, ng, n, n_ab, glane, lane_row, psrc, pdst, d_src, d_dst, layers, csr->in.off, call->step_key,
+			    call->step_pos, csr->perm, csr->edge_ids, call->npaths, call->last, call->first, call->elem_off, walk_off,
+			    d_elems, gtight);
+			PGQ_CUDA(cudaGetLastError());
+			st->kernel_launches++;
+			// (the next group reuses the group buffers)
+			PGQ_CUDA(cudaStreamSynchronize(s));
+			grp.clear();
+			grp_h = 0;
+			return PGQ_OK;
+		};
+		for (int l = 0; l < cnt; l++) {
+			if (h_np[(size_t)l] == 0) {
+				continue;
+			}
+			const int64_t h = h_last[(size_t)l];
+			if (layer_bytes(h, 1) > (double)call->budget) {
+				return pgq_fail(PGQ_ERR_UNSUPPORTED, "the cheapest paths of row %lld need %.0f bytes of count layers, over the "
+				                "budget of %lld", (long long)(b0 + l), layer_bytes(h, 1), (long long)call->budget);
+			}
+			const int64_t gh = std::max(grp_h, h);
+			if (!grp.empty() && layer_bytes(gh, (int64_t)grp.size() + 1) > (double)call->budget) {
+				PGQ_TRY(run_group());
+			}
+			grp.push_back(l);
+			grp_h = std::max(grp_h, h);
+		}
+		return run_group();
+	}
+};
+
+// Both calls: the arguments are checked; list = false is cheapest_path_count (the list outputs unused)
+static int ac_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, const uint8_t *src_valid,
+                  const uint8_t *dst_valid, bool list, int64_t max_paths, int64_t *out_count, int64_t *out_npaths,
+                  int64_t *out_first_path, uint8_t *out_valid, int64_t **out_path_offsets, int64_t **out_elems,
+                  int64_t *out_total_paths, pgq_stats *stats) {
+	pgq_stats st;
+	memset(&st, 0, sizeof(st));
+	if (p == 0) {
+		if (list) {
+			*out_path_offsets = (int64_t *)calloc(1, sizeof(int64_t));
+			*out_elems = (int64_t *)malloc(sizeof(int64_t));
+			if (!*out_path_offsets || !*out_elems) {
+				free(*out_path_offsets);
+				free(*out_elems);
+				*out_path_offsets = *out_elems = nullptr;
+				return pgq_fail(PGQ_ERR_OOM, "host allocation failed");
+			}
+		}
+		if (stats) {
+			*stats = st;
+		}
+		return PGQ_OK;
+	}
+	AcCall call;
+	memset(&call, 0, sizeof(call));
+	call.list = list;
+	call.max_paths = max_paths;
+	PGQ_TRY(layer_budget(&call.budget));
+	PGQ_CUDA(cudaSetDevice(csr->ctx->device));
+	WsGuard g(csr->ctx);
+	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
+	Workspace *ws = g.ws;
+	cudaStream_t s = ws->stream;
+	const int64_t n = csr->n, n_ab = csr->n_ab;
+	int64_t *d_src, *d_dst, *d_cost;
+	uint8_t *d_sv, *d_dv, *d_cv;
+	const size_t b8 = (size_t)p * sizeof(int64_t);
+	PGQ_CUDA(cudaEventRecord(ws->ev_begin, s));
+	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
+	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d_dst));
+	PGQ_TRY(stage_column(ws, WS_IN_VALID, src_valid, (size_t)p, (const void **)&d_sv));
+	PGQ_TRY(stage_column(ws, WS_IN_DST_VALID, dst_valid, (size_t)p, (const void **)&d_dv));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LEN, b8, (void **)&d_cost)); // the sweeps' costs
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_cv));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_PATH_VALID, (size_t)p, (void **)&call.valid));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_COUNT, b8, (void **)&call.count));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_NPATHS, b8, (void **)&call.npaths));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_ROW_ELEMS, b8, (void **)&call.elems_row));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_LAST, b8, (void **)&call.last));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_FIRST, b8, (void **)&call.first));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_ELEM_OFF, b8, (void **)&call.elem_off));
+	st.h2d_bytes = 2 * (int64_t)b8 + (src_valid ? p : 0) + (dst_valid ? p : 0);
+	// the step lists, and each entry's parent: the tight kernels' in-lists
+	int32_t *step_par;
+	PGQ_TRY(build_step_lists(csr, ws, s, &call.step_key, &call.step_pos, &st.kernel_launches));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_STEP_PAR, (size_t)std::max<int64_t>(csr->m, 1) * sizeof(int32_t), (void **)&step_par));
+	if (csr->m > 0) {
+		k_ac_step_par<<<ac_grid((n_ab + 7) / 8, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(n, n_ab, csr->in.off,
+		                                                                                     call.step_key, csr->perm,
+		                                                                                     step_par);
+		PGQ_CUDA(cudaGetLastError());
+		st.kernel_launches++;
+	}
+	call.step_par = step_par;
+	if (csr->weight_type == 2) {
+		const TightWalks<true> walks {csr, ws, d_src, d_dst, d_sv, d_dv, &st, &call};
+		PGQ_TRY(run_bf<true>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_cost, d_cv, &st, walks));
+	} else {
+		const TightWalks<false> walks {csr, ws, d_src, d_dst, d_sv, d_dv, &st, &call};
+		PGQ_TRY(run_bf<false>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_cost, d_cv, &st, walks));
+	}
+	cudaError_t e = cudaMemcpyAsync(out_count, call.count, b8, cudaMemcpyDeviceToHost, s);
+	st.d2h_bytes += (int64_t)b8 + p;
+	if (!list) {
+		if (e == cudaSuccess) e = cudaEventRecord(ws->ev_end, s);
+		if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+		float ms = 0.f;
+		if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end);
+		g.settled = (e == cudaSuccess);
+		if (e != cudaSuccess) {
+			cudaGetLastError();
+			return pgq_fail(PGQ_ERR_CUDA, "copying the cheapest path counts back failed: %s", cudaGetErrorString(e));
+		}
+		for (int64_t i = 0; i < p; i++) {
+			out_valid[i] = out_count[i] > 0;
+		}
+		st.total_ms = ms;
+		if (stats) {
+			*stats = st;
+		}
+		return PGQ_OK;
+	}
+	const u64 walks = call.walks, elem_total = call.elem_total;
+	int64_t *h_off = (int64_t *)malloc((size_t)(walks + 1) * sizeof(int64_t));
+	int64_t *h_elems = (int64_t *)malloc((size_t)std::max<u64>(elem_total, 1) * sizeof(int64_t));
+	if (!h_off || !h_elems) {
+		free(h_off);
+		free(h_elems);
+		return pgq_fail(PGQ_ERR_OOM, "host allocation of %llu path elements failed", (unsigned long long)elem_total);
+	}
+	if (e == cudaSuccess && walks > 0)
+		e = cudaMemcpyAsync(h_off, ws->buf[WS_AC_WALK_OFF], (size_t)walks * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess && elem_total > 0)
+		e = cudaMemcpyAsync(h_elems, ws->buf[WS_AC_ELEMS], (size_t)elem_total * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(out_npaths, call.npaths, b8, cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(out_first_path, call.first, b8, cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(out_valid, call.valid, (size_t)p, cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaEventRecord(ws->ev_end, s);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+	float ms = 0.f;
+	if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end);
+	g.settled = (e == cudaSuccess);
+	if (e != cudaSuccess) {
+		cudaGetLastError();
+		free(h_off);
+		free(h_elems);
+		return pgq_fail(PGQ_ERR_CUDA, "copying the cheapest paths back failed: %s", cudaGetErrorString(e));
+	}
+	h_off[walks] = (int64_t)elem_total;
+	st.total_ms = ms;
+	st.d2h_bytes += 2 * (int64_t)b8 + (int64_t)(walks + elem_total) * (int64_t)sizeof(int64_t);
+	*out_path_offsets = h_off;
+	*out_elems = h_elems;
+	*out_total_paths = (int64_t)walks;
+	if (stats) {
+		*stats = st;
+	}
+	return PGQ_OK;
+}
+
+// pgq_cheapest_path's argument checks, and max_paths
+static int ac_check_call(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, int64_t max_paths,
+                         const int64_t *out_count, const uint8_t *out_valid) {
+	if (!csr) {
+		return pgq_fail(PGQ_ERR_INVALID_ID, "%s", pgq_status_text(PGQ_ERR_INVALID_ID));
+	}
+	if (p < 0 || (p > 0 && (!src || !dst || !out_count || !out_valid))) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "null or negative argument");
+	}
+	if (max_paths < 0) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "max_paths must be >= 0");
+	}
+	if (!csr->finalized || !csr->w_bits || csr->weight_type == 0) {
+		return pgq_fail(PGQ_ERR_NOT_INITIALIZED, "Need to initialize CSR before doing cheapest path");
+	}
+	if (p >= 0x7fffffffLL) {
+		return pgq_fail(PGQ_ERR_RANGE, "too many pairs in one call");
+	}
+	return PGQ_OK;
+}
+
+extern "C" int pgq_cheapest_path_count(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
+                                       const uint8_t *src_valid, const uint8_t *dst_valid, int64_t *out_count,
+                                       uint8_t *out_valid, pgq_stats *stats) {
+	PGQ_TRY(ac_check_call(csr, p, src, dst, 0, out_count, out_valid));
+	return ac_run(csr, p, src, dst, src_valid, dst_valid, false, 0, out_count, nullptr, nullptr, out_valid, nullptr,
+	              nullptr, nullptr, stats);
+}
+
+extern "C" int pgq_all_cheapest_paths(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
+                                      const uint8_t *src_valid, const uint8_t *dst_valid, int64_t max_paths,
+                                      int64_t *out_count, int64_t *out_npaths, int64_t *out_first_path,
+                                      uint8_t *out_valid, int64_t **out_path_offsets, int64_t **out_elems,
+                                      int64_t *out_total_paths, pgq_stats *stats) {
+	if (!out_path_offsets || !out_elems || !out_total_paths) {
+		return pgq_fail(csr ? PGQ_ERR_INVALID_ARG : PGQ_ERR_INVALID_ID, "null output");
+	}
+	*out_path_offsets = nullptr;
+	*out_elems = nullptr;
+	*out_total_paths = 0;
+	PGQ_TRY(ac_check_call(csr, p, src, dst, max_paths, out_count, out_valid));
+	if (p > 0 && (!out_npaths || !out_first_path)) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "null output");
+	}
+	return ac_run(csr, p, src, dst, src_valid, dst_valid, true, max_paths, out_count, out_npaths, out_first_path,
+	              out_valid, out_path_offsets, out_elems, out_total_paths, stats);
 }

@@ -162,6 +162,17 @@ enum WsSlot : int {
 	WS_KM_STEPS = 108, WS_KM_STEP_ELEMS = 109,
 	// shortest_k_groups in WALK mode, on top of shortest_k_paths' slots: each lane's length groups found past h = 0
 	WS_KG_GROUPS = 110,
+	// cheapest_path_count / all_cheapest_paths (pgq_cheapest.cu), behind the Bellman-Ford sweeps and over the step lists:
+	// each step-list entry's parent as an internal id; per lane of a sweep batch its internal ids, row and open flag; the
+	// tight backward reach (reach, frontier and next-frontier masks [n][L / 64]) and |B_tight(t)|; the two rolling count
+	// layers [n_ab][L], each lane's running total, alive and infinite flags and counting bit, the counters; per row the
+	// count, the walks listed, their elements, the last one's length, the first walk and the first element; a storing
+	// group's lanes, their sources and its layers; the walks' offsets and elements, and the scans' total.
+	WS_AC_STEP_PAR = 111, WS_AC_PSRC = 112, WS_AC_PDST = 113, WS_AC_LANE_ROW = 114, WS_AC_OPEN = 115, WS_AC_REACH = 116,
+	WS_AC_FRONT = 117, WS_AC_NEXT = 118, WS_AC_BSIZE = 119, WS_AC_OMEGA_A = 120, WS_AC_OMEGA_B = 121, WS_AC_TOTAL = 122,
+	WS_AC_ALIVE = 123, WS_AC_INF = 124, WS_AC_ACTIVE = 125, WS_AC_COUNTERS = 126, WS_AC_COUNT = 127, WS_AC_NPATHS = 128,
+	WS_AC_ROW_ELEMS = 129, WS_AC_LAST = 130, WS_AC_FIRST = 131, WS_AC_ELEM_OFF = 132, WS_AC_GROUP_LANE = 133,
+	WS_AC_GROUP_SRC = 134, WS_AC_LAYERS = 135, WS_AC_WALK_OFF = 136, WS_AC_ELEMS = 137, WS_AC_SCAN_TOTAL = 138,
 	WS_SLOTS // (the last block holds the highest numbers)
 };
 
@@ -192,6 +203,11 @@ constexpr int ws_km[] = {WS_KM_IDS, WS_KM_PIDS, WS_KM_SPURS, WS_KM_LISTS, WS_KM_
                          WS_KM_LANE_OFF, WS_KM_COUNTERS, WS_KM_BAN_BITS, WS_KM_BAN_KEYS, WS_KM_STEPS,
                          WS_KM_STEP_ELEMS};
 constexpr int ws_kg[] = {WS_KG_GROUPS};
+constexpr int ws_ac[] = {WS_AC_STEP_PAR, WS_AC_PSRC, WS_AC_PDST, WS_AC_LANE_ROW, WS_AC_OPEN, WS_AC_REACH, WS_AC_FRONT,
+                         WS_AC_NEXT, WS_AC_BSIZE, WS_AC_OMEGA_A, WS_AC_OMEGA_B, WS_AC_TOTAL, WS_AC_ALIVE, WS_AC_INF,
+                         WS_AC_ACTIVE, WS_AC_COUNTERS, WS_AC_COUNT, WS_AC_NPATHS, WS_AC_ROW_ELEMS, WS_AC_LAST,
+                         WS_AC_FIRST, WS_AC_ELEM_OFF, WS_AC_GROUP_LANE, WS_AC_GROUP_SRC, WS_AC_LAYERS, WS_AC_WALK_OFF,
+                         WS_AC_ELEMS, WS_AC_SCAN_TOTAL};
 constexpr int ws_analytics[] = {WS_LCC_SRC, WS_LCC_OUT, WS_LCC_OUT_VALID, WS_LCC_BIG_ROWS, WS_LCC_BIG_CNT,
                                 WS_LCC_SRC_VALID, WS_LCC_BITMAP, WS_AN_REF_OFF, WS_AN_SCAN, WS_PR_KEY_A, WS_PR_KEY_B,
                                 WS_PR_VAL_A, WS_PR_VAL_B, WS_PR_IN_OFF, WS_PR_SCAN, WS_PR_DFLAG, WS_PR_RANK,
@@ -220,7 +236,7 @@ constexpr bool ws_apart(const int (&a)[A], const int (&...b)[B]) {
 	return (ws_disjoint(a, b) && ...);
 }
 static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_cp, ws_as, ws_ks, ws_km, ws_kg,
-                       ws_analytics, ws_keys, ws_key_staging),
+                       ws_ac, ws_analytics, ws_keys, ws_key_staging),
               "only the BFS drivers may write the search masks");
 static_assert(ws_apart(ws_staging, ws_driver, ws_bf), "a path entry point's staged columns live while its driver runs");
 static_assert(ws_apart(ws_cp, ws_staging, ws_bf), "the tight search runs on the distances and columns of its call");
@@ -232,6 +248,9 @@ static_assert(ws_apart(ws_km, ws_staging, ws_driver, ws_radix, ws_as, ws_ks),
               "the spur searches live across their rounds, over the step lists; WALK's own slots stay apart");
 static_assert(ws_apart(ws_kg, ws_staging, ws_driver, ws_radix, ws_as, ws_ks),
               "the length groups live across the walk search's batches, beside its own slots");
+static_assert(ws_apart(ws_ac, ws_staging, ws_bf, ws_as, ws_ks, ws_kg, ws_cp, ws_radix),
+              "the tight walk search lives across the sweep batches, over their distances, the columns of its call and the "
+              "step lists; the walk search's own slots stay apart");
 static_assert(WS_OUT_PATH_OFFSETS < WS_SLOTS && WS_OUT_PATH_VALID < WS_SLOTS, "every slot has a buffer");
 static_assert(ws_apart(ws_radix, ws_csr, ws_analytics, ws_keys), "radix_sort_pairs' scratch is apart from its callers'");
 static_assert(ws_apart(ws_key_staging, ws_keys, ws_csr, ws_radix), "a key build's staged columns live while it builds");

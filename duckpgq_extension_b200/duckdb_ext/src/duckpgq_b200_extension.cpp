@@ -72,6 +72,8 @@ static std::mutex g_ctx_lock;
 static pgq_ctx *g_ctx = nullptr;
 static std::atomic<int64_t> g_calls_cheapest_path {0};
 static std::atomic<int64_t> g_calls_path_count {0};
+static std::atomic<int64_t> g_calls_cheapest_count {0};
+static std::atomic<int64_t> g_calls_all_cheapest {0};
 static std::atomic<int64_t> g_calls_all_shortest {0};
 static std::atomic<int64_t> g_calls_shortest_k {0};
 static std::atomic<int64_t> g_calls_shortest_k_mode {0};
@@ -1309,6 +1311,120 @@ static void CheapestPathB200Function(DataChunk &args, ExpressionState &state, Ve
 	duckpgq_state->csr_to_delete.insert(info.csr_id);
 }
 
+// ---- cheapest_path_count / all_cheapest_paths (no reference function) ------------------------------------------
+// Every cheapest path of a row (include/duckpgq_b200.h, pgq_cheapest_path_count / pgq_all_cheapest_paths).  The binds
+// are cheapest_path's (constant id, GetCSR, the mark for deletion, the weights check) with their own result types;
+// all_cheapest_paths' max_paths is a constant >= 0.
+static unique_ptr<FunctionData> CheapestPathCountBind(BindScalarFunctionInput &input) {
+	auto data = CheapestPathBind(input);
+	input.GetBoundFunction().SetReturnType(LogicalType::BIGINT);
+	return data;
+}
+
+static unique_ptr<FunctionData> AllCheapestPathsBind(BindScalarFunctionInput &input) {
+	auto &arguments = input.GetArguments();
+	if (!arguments[4]->IsFoldable()) {
+		throw InvalidInputException("max_paths must be constant.");
+	}
+	auto max_paths = ExpressionExecutor::EvaluateScalar(input.GetClientContext(), *arguments[4]);
+	if (max_paths.IsNull() || max_paths.GetValue<int64_t>() < 0) {
+		throw InvalidInputException("max_paths must be 0 (every path) or more.");
+	}
+	auto data = CheapestPathBind(input);
+	input.GetBoundFunction().SetReturnType(LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT)));
+	return data;
+}
+
+// The weighted device CSR of a cheapest-path call and its rows' ids and validity (cheapest_path's lookup)
+static pgq_csr *CheapestCsr(ClientContext &context, int32_t csr_id, const char *what) {
+	auto duckpgq_state = GetDuckPGQState(context);
+	(void)duckpgq_state->GetCSR(csr_id); // "CSR not found with ID", duckpgq_state.cpp:180-186
+	auto entry = GetB200State(context)->Find(csr_id);
+	int wt = 0;
+	if (!entry || !entry->error.empty() || pgq_csr_finalize(entry->csr) != PGQ_OK ||
+	    pgq_csr_weight_type(entry->csr, &wt) != PGQ_OK || wt == 0) {
+		throw InvalidInputException("duckpgq_b200: %s needs a weighted CSR built through create_csr_edge", what);
+	}
+	return entry->csr;
+}
+
+struct CheapestPairs {
+	vector<int64_t> src, dst;
+	vector<uint8_t> src_valid, dst_valid;
+	explicit CheapestPairs(DataChunk &args) {
+		idx_t count = args.size();
+		UnifiedVectorFormat vsrc, vdst;
+		args.data[2].ToUnifiedFormat(vsrc);
+		args.data[3].ToUnifiedFormat(vdst);
+		auto src_data = reinterpret_cast<const int64_t *>(vsrc.data);
+		auto dst_data = reinterpret_cast<const int64_t *>(vdst.data);
+		src.resize(count);
+		dst.resize(count);
+		src_valid.resize(count);
+		dst_valid.resize(count);
+		for (idx_t i = 0; i < count; i++) {
+			auto sp = vsrc.sel->get_index(i), dp = vdst.sel->get_index(i);
+			src_valid[i] = vsrc.validity.RowIsValid(sp);
+			dst_valid[i] = vdst.validity.RowIsValid(dp);
+			src[i] = src_valid[i] ? src_data[sp] : 0;
+			dst[i] = dst_valid[i] ? dst_data[dp] : 0;
+		}
+	}
+};
+
+static void CheapestPathCountB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
+	auto &info = func_expr.BindInfo()->Cast<CheapestPathLengthFunctionData>();
+	pgq_csr *device_csr = CheapestCsr(info.context, info.csr_id, "cheapest_path_count");
+	idx_t count = args.size();
+	CheapestPairs pairs(args);
+	vector<int64_t> out_count(count);
+	vector<uint8_t> out_valid(count);
+	int st = pgq_cheapest_path_count(device_csr, static_cast<int64_t>(count), pairs.src.data(), pairs.dst.data(),
+	                                 pairs.src_valid.data(), pairs.dst_valid.data(), out_count.data(), out_valid.data(),
+	                                 nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_cheapest_count++;
+	g_pairs += static_cast<int64_t>(count);
+	result.SetVectorType(VectorType::FLAT_VECTOR);
+	auto result_data = FlatVector::GetDataMutable<int64_t>(result);
+	ValidityMask &result_validity = FlatVector::ValidityMutable(result);
+	for (idx_t i = 0; i < count; i++) {
+		result_data[i] = out_count[i];
+		if (!out_valid[i]) {
+			result_validity.SetInvalid(i);
+		}
+	}
+	GetDuckPGQState(info.context)->csr_to_delete.insert(info.csr_id);
+}
+
+static void AllCheapestPathsB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
+	auto &info = func_expr.BindInfo()->Cast<CheapestPathLengthFunctionData>();
+	pgq_csr *device_csr = CheapestCsr(info.context, info.csr_id, "all_cheapest_paths");
+	int64_t max_paths = args.data[4].GetValue(0).GetValue<int64_t>(); // (constant: AllCheapestPathsBind)
+	idx_t count = args.size();
+	CheapestPairs pairs(args);
+	vector<int64_t> out_count(count), npaths(count), first(count);
+	vector<uint8_t> out_valid(count);
+	int64_t *offsets = nullptr, *elems = nullptr;
+	int64_t paths = 0;
+	int st = pgq_all_cheapest_paths(device_csr, static_cast<int64_t>(count), pairs.src.data(), pairs.dst.data(),
+	                                pairs.src_valid.data(), pairs.dst_valid.data(), max_paths, out_count.data(),
+	                                npaths.data(), first.data(), out_valid.data(), &offsets, &elems, &paths, nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_all_cheapest++;
+	g_pairs += static_cast<int64_t>(count);
+	SetPathLists(result, count, offsets, elems, paths, first, npaths, out_valid);
+	pgq_free(offsets);
+	pgq_free(elems);
+	GetDuckPGQState(info.context)->csr_to_delete.insert(info.csr_id);
+}
+
 // ---- local_clustering_coefficient / pagerank / weakly_connected_component ---------------------------------------
 // Registered through WrapScalar, so the signatures and binds are the reference's; the reference callback is not
 // called.  The device CSR is found like a path function's (the device build, or an upload of the host CSR).
@@ -1430,7 +1546,9 @@ static void B200StatsFunction(DataChunk &args, ExpressionState &state, Vector &r
 	              ",shortest_k_paths_calls=" + std::to_string(g_calls_shortest_k.load()) +
 	              ",shortest_k_paths_mode_calls=" + std::to_string(g_calls_shortest_k_mode.load()) +
 	              ",shortest_k_groups_calls=" + std::to_string(g_calls_shortest_k_groups.load()) +
-	              ",shortest_k_groups_count_calls=" + std::to_string(g_calls_shortest_k_groups_count.load());
+	              ",shortest_k_groups_count_calls=" + std::to_string(g_calls_shortest_k_groups_count.load()) +
+	              ",cheapest_path_count_calls=" + std::to_string(g_calls_cheapest_count.load()) +
+	              ",all_cheapest_paths_calls=" + std::to_string(g_calls_all_cheapest.load());
 	result.SetVectorType(VectorType::CONSTANT_VECTOR);
 	ConstantVector::GetData<string_t>(result)[0] = StringVector::AddString(result, text);
 }
@@ -1536,6 +1654,14 @@ static void LoadInternal(ExtensionLoader &loader) {
 	loader.RegisterFunction(ScalarFunction(
 	    "cheapest_path", {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
 	    LogicalType::LIST(LogicalType::BIGINT), CheapestPathB200Function, CheapestPathBind));
+	// cheapest_path_count / all_cheapest_paths: ALL CHEAPEST's count and lists, raw UDFs like cheapest_path
+	loader.RegisterFunction(ScalarFunction(
+	    "cheapest_path_count", {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
+	    LogicalType::BIGINT, CheapestPathCountB200Function, CheapestPathCountBind));
+	loader.RegisterFunction(ScalarFunction(
+	    "all_cheapest_paths",
+	    {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
+	    LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT)), AllCheapestPathsB200Function, AllCheapestPathsBind));
 	// shortest_path_count / all_shortest_paths: no reference function is replaced; raw UDFs over the CSR CTE (the
 	// reference's MATCH rewriter rejects ALL SHORTEST)
 	loader.RegisterFunction(ScalarFunction(

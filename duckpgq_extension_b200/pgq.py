@@ -8,6 +8,8 @@ like the reference's own sqllogictests:
     iterativelength(id, v_size, src, dst)                             iterativelength.cpp:34-152
     shortestpath(id, v_size, src, dst)                                shortest_path.cpp:43-217
     cheapest_path(id, v_size, src, dst)                               (no reference function: the cheapest path's list)
+    cheapest_path_count(id, v_size, src, dst)                         (no reference function: ALL CHEAPEST's count)
+    all_cheapest_paths(id, v_size, src, dst, max_paths)               (no reference function: ALL CHEAPEST's lists)
     shortest_path_count(id, v_size, src, dst)                         (no reference function: ALL SHORTEST's count)
     all_shortest_paths(id, v_size, src, dst, max_paths)               (no reference function: ALL SHORTEST's lists)
     shortest_k_paths(id, v_size, src, dst, k)                         (no reference function: SHORTEST k's walks)
@@ -297,6 +299,47 @@ class DeviceCSR:
             self._lib.pgq_free(elems)
         paths = [flat[offs[i]: offs[i] + lens[i]].tolist() if ov[i] else None for i in range(p)]
         return paths, st.as_dict()
+
+    def cheapest_path_count(self, src, dst, src_valid=None, dst_valid=None):
+        """-> (counts int64, valid uint8, stats dict): the number of cheapest paths of each row, the walks of edges its
+        costs make tight, saturated at INT64_MAX, which also stands for infinitely many (include/duckpgq_b200.h,
+        pgq_cheapest_path_count)."""
+        src, dst = _i64(src), _i64(dst)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        dv = None if dst_valid is None else np.ascontiguousarray(dst_valid, dtype=np.uint8)
+        cnt = np.zeros(max(p, 1), dtype=np.int64)
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        st = _native.PgqStats()
+        _check(self._lib.pgq_cheapest_path_count(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv), _p64(cnt),
+                                                 _pu8(ov), C.byref(st)))
+        return cnt[:p], ov[:p], st.as_dict()
+
+    def all_cheapest_paths(self, src, dst, max_paths: int = 0, src_valid=None, dst_valid=None):
+        """-> (per row: list of [src, e1, v1, ..., dst] paths or None, counts int64, stats dict): the first
+        min(count, max_paths) cheapest paths of each row (all of them for max_paths = 0), fewest edges first, in step
+        order within a length; path 0 is cheapest_path's (include/duckpgq_b200.h, pgq_all_cheapest_paths)."""
+        src, dst = _i64(src), _i64(dst)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        dv = None if dst_valid is None else np.ascontiguousarray(dst_valid, dtype=np.uint8)
+        cnt, npaths, first = (np.zeros(max(p, 1), dtype=np.int64) for _ in range(3))
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        offs, elems = C.POINTER(C.c_int64)(), C.POINTER(C.c_int64)()
+        total = C.c_int64(0)
+        st = _native.PgqStats()
+        _check(self._lib.pgq_all_cheapest_paths(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv), int(max_paths),
+                                                _p64(cnt), _p64(npaths), _p64(first), _pu8(ov), C.byref(offs),
+                                                C.byref(elems), C.byref(total), C.byref(st)))
+        try:
+            woff = np.ctypeslib.as_array(offs, shape=(total.value + 1,)).copy()
+            flat = np.ctypeslib.as_array(elems, shape=(int(woff[-1]),)).copy() if woff[-1] else np.zeros(0, np.int64)
+        finally:
+            self._lib.pgq_free(offs)
+            self._lib.pgq_free(elems)
+        walks = [flat[woff[j]: woff[j + 1]].tolist() for j in range(total.value)]
+        paths = [walks[first[i]: first[i] + npaths[i]] if ov[i] else None for i in range(p)]
+        return paths, cnt[:p], st.as_dict()
 
     def finalize(self):
         _check(self._lib.pgq_csr_finalize(self._h))
@@ -688,6 +731,38 @@ def cheapest_path(state: DuckPGQState, csr_id: int, v_size: int, src, dst, src_v
     if csr.weight_type() == 0:  # CheapestPathLengthBind's check, cheapest_path_length_function_data.cpp:22-24
         raise ConstraintException(PGQ_ERR_NOT_INITIALIZED, "Need to initialize CSR before doing cheapest path")
     paths, _ = csr.cheapest_path(src, dst, src_valid, dst_valid)
+    state.csr_to_delete.add(csr_id)
+    return paths
+
+
+def _lookup_weighted(state: DuckPGQState, csr_id: int) -> DeviceCSR:
+    csr = state.csr_list.get(csr_id)
+    if csr is None:  # DuckPGQState::GetCSR, duckpgq_state.cpp:180-186
+        raise ConstraintException(PGQ_ERR_INVALID_ID, f"CSR not found with ID {csr_id}")
+    state.csr_to_delete.add(csr_id)
+    csr.finalize()
+    if csr.weight_type() == 0:  # CheapestPathLengthBind's check, cheapest_path_length_function_data.cpp:22-24
+        raise ConstraintException(PGQ_ERR_NOT_INITIALIZED, "Need to initialize CSR before doing cheapest path")
+    return csr
+
+
+def cheapest_path_count(state: DuckPGQState, csr_id: int, v_size: int, src, dst, src_valid=None, dst_valid=None):
+    """cheapest_path_count(INT, BIGINT, BIGINT, BIGINT) -> BIGINT: the number of cheapest paths, saturated at INT64_MAX
+    (also for infinitely many), or NULL (no reference function; looked up and marked as cheapest_path is).  Returns
+    (counts, valid)."""
+    csr = _lookup_weighted(state, csr_id)
+    counts, valid, _ = csr.cheapest_path_count(src, dst, src_valid, dst_valid)
+    state.csr_to_delete.add(csr_id)
+    return counts, valid
+
+
+def all_cheapest_paths(state: DuckPGQState, csr_id: int, v_size: int, src, dst, max_paths: int = 0, src_valid=None,
+                       dst_valid=None):
+    """all_cheapest_paths(INT, BIGINT, BIGINT, BIGINT, BIGINT max_paths) -> LIST(LIST(BIGINT)): per row the first
+    min(count, max_paths) cheapest paths (every one for max_paths = 0) or None (no reference function; looked up and
+    marked as cheapest_path is)."""
+    csr = _lookup_weighted(state, csr_id)
+    paths, _, _ = csr.all_cheapest_paths(src, dst, max_paths, src_valid, dst_valid)
     state.csr_to_delete.add(csr_id)
     return paths
 

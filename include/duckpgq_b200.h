@@ -300,6 +300,55 @@ int pgq_cheapest_path(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const i
                       const uint8_t *dst_valid, int64_t *out_offsets, int64_t *out_lengths, uint8_t *out_valid,
                       int64_t **out_elems, int64_t *out_total, pgq_stats *stats);
 
+/* pgq_cheapest_path_count / pgq_all_cheapest_paths: every cheapest path of a row (SQL/PGQ's ALL CHEAPEST), over a CSR
+ * built with pgq_csr_add_edges_weighted (BIGINT or DOUBLE weights).  No reference function.  For a row (s, t), d is what
+ * pgq_cheapest_path_length computes, and an edge v -> u is tight for the row by pgq_cheapest_path's rule: d(v) + w ==
+ * d(u) in the weight type's arithmetic (int64 addition; double addition rounded to nearest, compared as values: -0.0 ==
+ * 0.0, a NaN equals nothing).
+ *   - a cheapest path is a walk [s, e1, v1, ..., eh, t] made only of tight edges, in pgq_shortestpath's format (vertex
+ *     rowids; edge rowids from the CSR's edge ids, CSR positions when it was uploaded without ids).  Parallel edges give
+ *     distinct paths.  For BIGINT weights with d(s) = 0 and no overflow these are exactly the walks whose weights,
+ *     summed from 0, equal the cost.  For DOUBLE weights the tight-edge rule is the contract: with edges 0 -> 1 (0.1),
+ *     1 -> 2 (0.2) and 0 -> 2 (0.3), only 0 -> 2 is tight, since 0.1 + 0.2 != 0.3 in double.
+ *   - count = the number of such walks, saturated at INT64_MAX, which means "at least INT64_MAX, or infinitely many".  It
+ *     is infinite exactly when a cycle of tight edges lies on a tight s -> t walk (a zero-weight self-loop or two-cycle
+ *     on a route is enough); a tight cycle that s reaches but that does not reach t changes nothing.  s == t: the count
+ *     includes [s] and every closed tight walk through s (1 when every weight is above zero).
+ *   - NULL (out_valid 0, count 0, no paths): a NULL source or destination (src_valid / dst_valid, both nullable), a NULL
+ *     pgq_cheapest_path_length cost, or no tight walk from s to t: exactly the rows on which pgq_cheapest_path is NULL.
+ *   - order: by the number of edges ascending; within one length as pgq_all_shortest_paths orders paths (walking back
+ *     from t, a step is (the parent's ORIGINAL id, the edge's position in the parent's adjacency), steps compared
+ *     lexicographically from t back to s).  Path 0 is pgq_cheapest_path's path: it has the fewest edges, and at each
+ *     remaining length the walk back picks a parent whose depth over tight edges is one less.  With every weight 1
+ *     (BIGINT), count and paths equal pgq_shortest_path_count / pgq_all_shortest_paths, order included.
+ * pgq_all_cheapest_paths lists the first min(count, max_paths) paths of each row (all of them for max_paths == 0; a row
+ * with infinitely many still gets its first max_paths), in pgq_shortest_k_paths' layout: row i's out_npaths[i] paths are
+ * the call's paths out_first_path[i] .. + out_npaths[i]; path j is (*out_elems)[(*out_path_offsets)[j] ..
+ * (*out_path_offsets)[j + 1]); *out_total_paths paths in all.  Both arrays are allocated by the library (also for zero
+ * rows): release them with pgq_free().
+ *   - errors: max_paths < 0 -> PGQ_ERR_INVALID_ARG; max_paths == 0 with a count of INT64_MAX -> PGQ_ERR_UNSUPPORTED; an
+ *     unweighted, missing or unfinalised CSR and ids outside [0, n) give pgq_cheapest_path's errors; a path the result
+ *     needs longer than 65533 edges, or a row still counting after 65533 edges -> PGQ_ERR_UNSUPPORTED (this bounds the
+ *     call); a row whose count layers, (H + 1) x n_ab x 8 bytes (H its last listed path's length), exceed the layer
+ *     budget (4 GiB) -> PGQ_ERR_UNSUPPORTED; an element total that overflows int64 or cannot be allocated ->
+ *     PGQ_ERR_OOM; both checked before anything of that size is allocated.
+ *   - the call: rows take lanes and batches exactly as in pgq_cheapest_path_length, whose sweeps run first.  Behind each
+ *     batch's sweeps, a BFS back from the lanes' targets over their tight edges finds B(t), the vertices with a tight
+ *     walk to t (s outside B(t): NULL); then the tight walks from s inside B(t) are counted layer by layer.  A lane stops
+ *     after the layer h where the counts are zero on all of B(t) (the count is exact), where its total saturates, or
+ *     once h >= |B(t)| with counts still alive (the count is infinite), but not before it has max_paths paths to list.
+ *   - stats: batches, levels (Bellman-Ford sweeps) and lanes as pgq_cheapest_path_length's for the same rows;
+ *     push_levels = the sum over batches of the tight backward BFS's levels (1 + the largest tight distance to a lane's
+ *     target: the last level adds nothing); pull_levels = the sum over batches of the count layers h >= 1 computed (its
+ *     lanes' largest stopping layer); kernel_launches, h2d_bytes, d2h_bytes and total_ms cover the whole call. */
+int pgq_cheapest_path_count(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const int64_t *dst,
+                            const uint8_t *src_valid, const uint8_t *dst_valid, int64_t *out_count, uint8_t *out_valid,
+                            pgq_stats *stats);
+int pgq_all_cheapest_paths(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const int64_t *dst,
+                           const uint8_t *src_valid, const uint8_t *dst_valid, int64_t max_paths, int64_t *out_count,
+                           int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid, int64_t **out_path_offsets,
+                           int64_t **out_elems, int64_t *out_total_paths, pgq_stats *stats);
+
 /* pgq_shortest_path_count / pgq_all_shortest_paths: every shortest path of a row (SQL/PGQ's ALL SHORTEST, which the
  * reference rejects).  No reference function.  For a row (s, t) with h = the BFS depth of t from s along out-edges:
  *   - a shortest path is any list [s, e1, v1, ..., eh, t] of h edges along out-edges, in pgq_shortestpath's format
