@@ -17,9 +17,9 @@ INCLUDE = os.path.join(ROOT, "include")
 LIB_DIR = os.path.join(_PKG, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libduckpgq_b200.so")
 SOURCES = ["pgq_csr.cu", "pgq_bfs.cu", "pgq_api.cu", "pgq_cheapest.cu", "pgq_allshortest.cu", "pgq_kshortest.cu",
-           "pgq_kpaths_modes.cu",
+           "pgq_kpaths_modes.cu", "pgq_cheapest_k.cu",
            "pgq_multi.cu", "pgq_analytics.cu"]
-HEADERS = ["pgq_internal.h", "pgq_tile.cuh", "pgq_pull.cuh", "pgq_count.cuh"]
+HEADERS = ["pgq_internal.h", "pgq_tile.cuh", "pgq_pull.cuh", "pgq_count.cuh", "pgq_bf.cuh", "pgq_kpaths.cuh"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -127,6 +127,9 @@ SYMBOLS = {
                                        C.POINTER(_P64), C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
     "pgq_shortest_k_paths_mode": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, C.c_int64, C.c_int32, _P64,
                                             _P64, _PU8, C.POINTER(_P64), C.POINTER(_P64), _P64, C.POINTER(PgqStats)]),
+    "pgq_cheapest_k_paths": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, C.c_int64, C.c_int32, _P64, _P64,
+                                       _PU8, C.POINTER(_P64), C.POINTER(_P64), C.POINTER(_VP), _P64,
+                                       C.POINTER(PgqStats)]),
     "pgq_shortest_k_groups": (C.c_int, [_VP, C.c_int64, _P64, _P64, _PU8, _PU8, _VP, C.c_int64, C.c_int32, C.c_int64,
                                         _P64, _P64, _P64, _PU8, _P64, _P64, _PU8, C.POINTER(_P64), C.POINTER(_P64),
                                         _P64, C.POINTER(PgqStats)]),

@@ -173,6 +173,13 @@ enum WsSlot : int {
 	WS_AC_ALIVE = 123, WS_AC_INF = 124, WS_AC_ACTIVE = 125, WS_AC_COUNTERS = 126, WS_AC_COUNT = 127, WS_AC_NPATHS = 128,
 	WS_AC_ROW_ELEMS = 129, WS_AC_LAST = 130, WS_AC_FIRST = 131, WS_AC_ELEM_OFF = 132, WS_AC_GROUP_LANE = 133,
 	WS_AC_GROUP_SRC = 134, WS_AC_LAYERS = 135, WS_AC_WALK_OFF = 136, WS_AC_ELEMS = 137, WS_AC_SCAN_TOTAL = 138,
+	// cheapest_k_paths (pgq_cheapest_k.cu), which runs the rounds of the path modes (WS_KM_*: ids, spurs, lists, seed
+	// flags, lane map, spur lengths and offsets, TRAIL's ban bitmap and table, steps) over the step lists: a round's
+	// root costs; a batch's distances [n][W] as order-preserving keys, dirty bitmap and flags, tight levels [n][W]
+	// uint16, banned-vertex masks [n][W / 64], the tight BFS's two vertex frontiers, grew and done masks; the spurs'
+	// step weights.
+	WS_CK_ROOT = 139, WS_CK_DIST = 140, WS_CK_DIRTY = 141, WS_CK_FLAGS = 142, WS_CK_LEVEL = 143, WS_CK_VBAN = 144,
+	WS_CK_FRONT = 145, WS_CK_GREW = 146, WS_CK_DONE = 147, WS_CK_STEP_W = 148,
 	WS_SLOTS // (the last block holds the highest numbers)
 };
 
@@ -208,6 +215,8 @@ constexpr int ws_ac[] = {WS_AC_STEP_PAR, WS_AC_PSRC, WS_AC_PDST, WS_AC_LANE_ROW,
                          WS_AC_ACTIVE, WS_AC_COUNTERS, WS_AC_COUNT, WS_AC_NPATHS, WS_AC_ROW_ELEMS, WS_AC_LAST,
                          WS_AC_FIRST, WS_AC_ELEM_OFF, WS_AC_GROUP_LANE, WS_AC_GROUP_SRC, WS_AC_LAYERS, WS_AC_WALK_OFF,
                          WS_AC_ELEMS, WS_AC_SCAN_TOTAL};
+constexpr int ws_ck[] = {WS_CK_ROOT, WS_CK_DIST, WS_CK_DIRTY, WS_CK_FLAGS, WS_CK_LEVEL, WS_CK_VBAN, WS_CK_FRONT,
+                         WS_CK_GREW, WS_CK_DONE, WS_CK_STEP_W};
 constexpr int ws_analytics[] = {WS_LCC_SRC, WS_LCC_OUT, WS_LCC_OUT_VALID, WS_LCC_BIG_ROWS, WS_LCC_BIG_CNT,
                                 WS_LCC_SRC_VALID, WS_LCC_BITMAP, WS_AN_REF_OFF, WS_AN_SCAN, WS_PR_KEY_A, WS_PR_KEY_B,
                                 WS_PR_VAL_A, WS_PR_VAL_B, WS_PR_IN_OFF, WS_PR_SCAN, WS_PR_DFLAG, WS_PR_RANK,
@@ -236,7 +245,7 @@ constexpr bool ws_apart(const int (&a)[A], const int (&...b)[B]) {
 	return (ws_disjoint(a, b) && ...);
 }
 static_assert(ws_apart(ws_masks, ws_radix, ws_staging, ws_driver, ws_csr, ws_bf, ws_cp, ws_as, ws_ks, ws_km, ws_kg,
-                       ws_ac, ws_analytics, ws_keys, ws_key_staging),
+                       ws_ac, ws_ck, ws_analytics, ws_keys, ws_key_staging),
               "only the BFS drivers may write the search masks");
 static_assert(ws_apart(ws_staging, ws_driver, ws_bf), "a path entry point's staged columns live while its driver runs");
 static_assert(ws_apart(ws_cp, ws_staging, ws_bf), "the tight search runs on the distances and columns of its call");
@@ -251,6 +260,9 @@ static_assert(ws_apart(ws_kg, ws_staging, ws_driver, ws_radix, ws_as, ws_ks),
 static_assert(ws_apart(ws_ac, ws_staging, ws_bf, ws_as, ws_ks, ws_kg, ws_cp, ws_radix),
               "the tight walk search lives across the sweep batches, over their distances, the columns of its call and the "
               "step lists; the walk search's own slots stay apart");
+static_assert(ws_apart(ws_ck, ws_staging, ws_bf, ws_km, ws_ks, ws_ac, ws_cp, ws_as, ws_radix),
+              "the Bellman-Ford spur searches live across their rounds, beside the rounds' own slots, over the step lists "
+              "and the columns of their call; the other searches' slots stay apart");
 static_assert(WS_OUT_PATH_OFFSETS < WS_SLOTS && WS_OUT_PATH_VALID < WS_SLOTS, "every slot has a buffer");
 static_assert(ws_apart(ws_radix, ws_csr, ws_analytics, ws_keys), "radix_sort_pairs' scratch is apart from its callers'");
 static_assert(ws_apart(ws_key_staging, ws_keys, ws_csr, ws_radix), "a key build's staged columns live while it builds");

@@ -33,34 +33,13 @@
 #include <vector>
 
 #include "pgq_count.cuh"
+#include "pgq_kpaths.cuh"
 #include "pgq_tile.cuh"
 
-#define KM_PATH_MAX 65533 // the longest path a result may hold (all_shortest_paths' depth limit)
 #define KM_BUDGET ((int64_t)4 << 30)
 
 // The batch's counters: [0] lanes still searching; [1] a lane reached a level beyond KM_PATH_MAX
 enum { KM_ACTIVE = 0, KM_TOO_LONG = 1 };
-
-// One spur search: its spur node and target (internal ids) and its ban lists in the round's list array: vb the banned
-// vertices (internal ids), d the deviation bans and eb the banned edges (out-CSR positions)
-struct KmSpur {
-	int32_t u, t, nvb, nd, neb, pad;
-	int64_t vb, d, eb;
-};
-
-__device__ __forceinline__ bool km_in(const int32_t *__restrict__ list, int cnt, int32_t x) {
-	for (int i = 0; i < cnt; i++) {
-		if (list[i] == x) {
-			return true;
-		}
-	}
-	return false;
-}
-
-// entry e (to v) of u's adjacency may start the spur
-__device__ __forceinline__ bool km_first_ok(const KmSpur &sp, const int32_t *__restrict__ lists, int32_t e, int32_t v) {
-	return !km_in(lists + sp.d, sp.nd, e) && !km_in(lists + sp.eb, sp.neb, e) && !km_in(lists + sp.vb, sp.nvb, v);
-}
 
 // internal ids of the rows' sources and targets
 __global__ void k_km_ids(int64_t cnt, const int64_t *__restrict__ ids, const int32_t *__restrict__ perm, int32_t *pids) {
@@ -125,27 +104,6 @@ __global__ void __launch_bounds__(256) k_km_seed(int cnt, int wd, int W, const i
 			atomicOr(&grew[word], bit);
 		}
 	}
-}
-
-// the lanes whose banned positions include e, within mask word j: keys sorted, key = position * 512 + lane
-__device__ __forceinline__ u64 km_ban_mask(const int64_t *__restrict__ keys, int64_t nkeys, int64_t e, int j) {
-	int64_t lo = 0, hi = nkeys;
-	while (lo < hi) {
-		const int64_t mid = (lo + hi) >> 1;
-		if (keys[mid] < e * 512) {
-			lo = mid + 1;
-		} else {
-			hi = mid;
-		}
-	}
-	u64 mask = 0;
-	for (; lo < nkeys && (keys[lo] >> 9) == e; lo++) {
-		const int l = (int)(keys[lo] & 511);
-		if ((l >> 6) == j) {
-			mask |= 1ull << (l & 63);
-		}
-	}
-	return mask;
 }
 
 // One forward level over the out-CSR: every out-edge r -> x passes r's frontier bits of the lanes still searching to
@@ -320,24 +278,24 @@ __global__ void __launch_bounds__(256) k_km_walk(int cnt, int W, int64_t n, cons
 	}
 }
 
-static inline unsigned km_grid(int64_t want, int64_t cap) {
-	return (unsigned)std::max<int64_t>(1, std::min<int64_t>(want, cap));
-}
-
-// a path of a row: its vertices (internal ids), out-CSR positions, elements [s, e1, v1, ..., t] and the spur index it
-// deviated at
+// a path of a row: its vertices (internal ids), out-CSR positions, elements [s, e1, v1, ..., t], the spur index it
+// deviated at and, when its search has costs, the costs of its prefixes (cost[i]: its first i steps)
 struct KmPath {
 	std::vector<int32_t> v, pos;
-	std::vector<int64_t> el;
+	std::vector<int64_t> el, cost;
 	int64_t dev = 0;
 	int64_t h() const {
 		return (int64_t)pos.size();
 	}
-	// (h, then the steps (parent's original id, position) from t back to s): the result's order, and the identity of a
-	// path of the row
-	std::vector<int64_t> key() const {
+	// (the cost when the search has costs, h, then the steps (parent's original id, position) from t back to s): the
+	// result's order, and the identity of a path of the row.  A cost is >= 0 and never -0.0 (a sum from +0.0 of weights
+	// >= 0), so its raw bits order as its value in both weight types.
+	std::vector<int64_t> key(bool costs) const {
 		std::vector<int64_t> k;
-		k.reserve(2 * pos.size() + 1);
+		k.reserve(2 * pos.size() + 2);
+		if (costs) {
+			k.push_back(cost.back());
+		}
 		k.push_back(h());
 		for (int64_t i = h() - 1; i >= 0; i--) {
 			k.push_back(el[2 * i]);
@@ -385,22 +343,124 @@ static int km_lanes_cap(const pgq_options *opts, int64_t n) {
 }
 
 // a round's lane width: the cap, halved while the round's searches are at most half of it (ks_lanes' rule)
-static int km_lanes(const pgq_options *opts, int cap, int64_t searches) {
-	int w = cap;
-	while (!(opts && opts->lanes) && w > 64 && searches <= w / 2) {
+static int km_lanes(const pgq_options *opts, const KmSearch &search, int64_t searches) {
+	int w = search.cap;
+	while (!(opts && opts->lanes) && w > search.lane_min && searches <= w / 2) {
 		w >>= 1;
 	}
 	return w;
 }
 
-// shortest_k_paths_mode (kg null) and shortest_k_groups in the TRAIL, ACYCLIC and SIMPLE modes: the rounds of the top.
-// The arguments are checked.
-static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, const uint8_t *src_valid,
-                  const uint8_t *dst_valid, const pgq_options *opts, int64_t k, int32_t path_mode, const KmGroups *kg,
-                  int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid, int64_t **out_path_offsets,
-                  int64_t **out_elems, int64_t *out_total_paths, pgq_stats *stats) {
+// shortest_k_paths_mode's spur search: the BFS of the top, level by level over bit masks
+struct KmBfs : KmSearch {
+	pgq_csr *csr;
+	const u64 *step_key = nullptr;
+	const int32_t *step_pos = nullptr;
+	u64 *seen = nullptr, *front = nullptr, *next = nullptr, *done = nullptr, *grew = nullptr, *ctr = nullptr;
+	uint16_t *level = nullptr;
+	KmBfs(pgq_csr *c, const pgq_options *opts) : csr(c) {
+		cap = km_lanes_cap(opts, c->n);
+	}
+	int begin(Workspace *ws, const u64 *sk, const int32_t *sp) override {
+		const int64_t n = csr->n;
+		const int wd_cap = cap / 64;
+		step_key = sk;
+		step_pos = sp;
+		PGQ_TRY(pgq_ws_reserve(ws, WS_KM_SEEN, (size_t)n * wd_cap * sizeof(u64), (void **)&seen));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_KM_FRONT, (size_t)n * wd_cap * sizeof(u64), (void **)&front));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_KM_NEXT, (size_t)n * wd_cap * sizeof(u64), (void **)&next));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_KM_LEVEL, (size_t)n * cap * sizeof(uint16_t), (void **)&level));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_KM_DONE, (size_t)wd_cap * sizeof(u64), (void **)&done));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_KM_GREW, (size_t)wd_cap * sizeof(u64), (void **)&grew));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_KM_COUNTERS, 256, (void **)&ctr));
+		return PGQ_OK;
+	}
+	int has_seed(Workspace *ws, int64_t ns, const KmSpur *spurs, const int32_t *lists, const std::vector<int64_t> &,
+	             uint8_t *has, pgq_stats *st) override {
+		k_km_has_seed<<<km_grid((ns + 7) / 8, (int64_t)csr->ctx->sm_count * 16), 256, 0, ws->stream>>>(
+		    ns, spurs, lists, csr->out.off, csr->out.adj, has);
+		PGQ_CUDA(cudaGetLastError());
+		st->kernel_launches++;
+		return PGQ_OK;
+	}
+	int search(Workspace *ws, const KmBatch &b, pgq_stats *st) override {
+		cudaStream_t s = ws->stream;
+		const int64_t n = csr->n, m = csr->m;
+		const int sms = csr->ctx->sm_count;
+		const int W = b.W, wd = W / 64, cnt = b.cnt;
+		const unsigned edge_grid = km_grid((m + 255) / 256, (int64_t)sms * 16);
+		const unsigned vert_grid = km_grid((n + 255) / 256, (int64_t)sms * 8);
+		PGQ_CUDA(cudaMemsetAsync(seen, 0, (size_t)n * wd * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(front, 0, (size_t)n * wd * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(next, 0, (size_t)n * wd * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(level, 0xff, (size_t)n * W * sizeof(uint16_t), s));
+		PGQ_CUDA(cudaMemsetAsync(done, 0, (size_t)wd * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(grew, 0, (size_t)wd * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(b.hlen, 0, (size_t)W * sizeof(int32_t), s));
+		PGQ_CUDA(cudaMemsetAsync(ctr, 0, 2 * sizeof(u64), s));
+		k_km_seed<<<b.lane_grid, 256, 0, s>>>(cnt, wd, W, b.lane_spur, b.spurs, b.lists, csr->out.off, csr->out.adj,
+		                                      seen, front, grew, level, b.ban_bits);
+		PGQ_CUDA(cudaGetLastError());
+		st->kernel_launches++;
+		for (int lv = 2;; lv++) {
+			u64 h_ctr[2];
+			PGQ_CUDA(cudaMemsetAsync(&ctr[KM_ACTIVE], 0, sizeof(u64), s));
+			k_km_finish<<<1, 1024, 0, s>>>(cnt, wd, W, b.lane_spur, b.spurs, seen, level, grew, done, b.hlen, ctr);
+			PGQ_CUDA(cudaGetLastError());
+			st->kernel_launches++;
+			PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, s));
+			PGQ_CUDA(cudaMemcpyAsync(b.h_hlen, b.hlen, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+			PGQ_CUDA(cudaStreamSynchronize(s));
+			st->d2h_bytes += (int64_t)sizeof(h_ctr) + cnt * (int64_t)sizeof(int32_t);
+			if (h_ctr[KM_TOO_LONG]) {
+				return pgq_fail(PGQ_ERR_UNSUPPORTED, "a spur search went beyond %d edges", KM_PATH_MAX);
+			}
+			if (!h_ctr[KM_ACTIVE]) {
+				break;
+			}
+			k_km_level<<<edge_grid, 256, 0, s>>>(m, n, wd, csr->out.off, csr->out.adj, front, seen, done, b.ban_bits,
+			                                     b.keys, b.nkeys, next);
+			k_km_fold<<<vert_grid, 256, 0, s>>>(n, wd, W, lv, seen, front, next, grew, level, ctr);
+			PGQ_CUDA(cudaGetLastError());
+			st->kernel_launches += 2;
+			st->levels++;
+		}
+		return PGQ_OK;
+	}
+	int walk(Workspace *ws, const KmBatch &b, const int64_t *lane_off, int2 *steps, longlong2 *step_elems, int64_t *,
+	         pgq_stats *st) override {
+		k_km_walk<<<b.lane_grid, 256, 0, ws->stream>>>(b.cnt, b.W, csr->n, b.lane_spur, b.spurs, b.lists, b.hlen,
+		                                               lane_off, level, csr->in.off, step_key, step_pos, csr->perm,
+		                                               csr->inv, csr->out.off, csr->out.adj, csr->edge_ids, steps,
+		                                               step_elems);
+		PGQ_CUDA(cudaGetLastError());
+		st->kernel_launches++;
+		return PGQ_OK;
+	}
+};
+
+int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, const uint8_t *src_valid,
+           const uint8_t *dst_valid, const pgq_options *opts, int64_t k, int32_t path_mode, const KmGroups *kg,
+           KmSearch &search, int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid,
+           int64_t **out_path_offsets, int64_t **out_elems, void **out_costs, int64_t *out_total_paths,
+           pgq_stats *stats) {
 	const bool trail = path_mode == PGQ_PATH_TRAIL;
+	const bool costs = search.costs;
+	const bool f64 = csr->weight_type == 2;
 	const int64_t n = csr->n, m = csr->m;
+	// c + w in the weight type's arithmetic (a path's sum runs over the edges its search found, below the sentinel)
+	auto add = [f64](int64_t c, int64_t w) {
+		if (!f64) {
+			return c + w;
+		}
+		double a, b;
+		memcpy(&a, &c, sizeof(a));
+		memcpy(&b, &w, sizeof(b));
+		const double r = a + b;
+		int64_t bits;
+		memcpy(&bits, &r, sizeof(bits));
+		return bits;
+	};
 	std::vector<int64_t> ids; // the rows whose ids are both valid: sources, then targets
 	std::vector<KmRow> rows;
 	for (int64_t i = 0; i < p; i++) {
@@ -420,17 +480,24 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 	for (const KmRow &r : rows) {
 		ids.push_back(dst[r.row]);
 	}
-	const int cap = km_lanes_cap(opts, n);
+	const int cap = search.cap;
 	pgq_stats st;
 	memset(&st, 0, sizeof(st));
-	st.lanes = km_lanes(opts, cap, 0);
+	st.lanes = km_lanes(opts, search, 0);
 	if (p == 0) {
 		*out_path_offsets = (int64_t *)calloc(1, sizeof(int64_t));
 		*out_elems = (int64_t *)malloc(sizeof(int64_t));
-		if (!*out_path_offsets || !*out_elems) {
+		if (out_costs) {
+			*out_costs = malloc(sizeof(int64_t));
+		}
+		if (!*out_path_offsets || !*out_elems || (out_costs && !*out_costs)) {
 			free(*out_path_offsets);
 			free(*out_elems);
 			*out_path_offsets = *out_elems = nullptr;
+			if (out_costs) {
+				free(*out_costs);
+				*out_costs = nullptr;
+			}
 			return pgq_fail(PGQ_ERR_OOM, "host allocation failed");
 		}
 		if (stats) {
@@ -444,9 +511,6 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
 	const int sms = csr->ctx->sm_count;
-	const int wd_cap = cap / 64;
-	u64 *seen, *front, *next, *done, *grew, *ctr;
-	uint16_t *level;
 	int32_t *hlen, *pids, *lane_spur;
 	int64_t *lane_off;
 	uint32_t *ban_bits = nullptr;
@@ -455,13 +519,6 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 	PGQ_TRY(stage_column(ws, WS_KM_IDS, ids.data(), ids.size() * sizeof(int64_t), (const void **)&d_ids));
 	st.h2d_bytes += (int64_t)(ids.size() * sizeof(int64_t));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_KM_PIDS, ids.size() * sizeof(int32_t), (void **)&pids));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KM_SEEN, (size_t)n * wd_cap * sizeof(u64), (void **)&seen));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KM_FRONT, (size_t)n * wd_cap * sizeof(u64), (void **)&front));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KM_NEXT, (size_t)n * wd_cap * sizeof(u64), (void **)&next));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KM_LEVEL, (size_t)n * cap * sizeof(uint16_t), (void **)&level));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KM_DONE, (size_t)wd_cap * sizeof(u64), (void **)&done));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KM_GREW, (size_t)wd_cap * sizeof(u64), (void **)&grew));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KM_COUNTERS, 256, (void **)&ctr));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_KM_HLEN, (size_t)cap * sizeof(int32_t), (void **)&hlen));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_KM_LANE_OFF, (size_t)cap * sizeof(int64_t), (void **)&lane_off));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_KM_LANE_SPUR, (size_t)cap * sizeof(int32_t), (void **)&lane_spur));
@@ -484,8 +541,7 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 	const u64 *step_key = nullptr;
 	const int32_t *step_pos = nullptr;
 	PGQ_TRY(build_step_lists(csr, ws, s, &step_key, &step_pos, &st.kernel_launches));
-	const unsigned edge_grid = km_grid((m + 255) / 256, (int64_t)sms * 16);
-	const unsigned vert_grid = km_grid((n + 255) / 256, (int64_t)sms * 8);
+	PGQ_TRY(search.begin(ws, step_key, step_pos));
 	// ---- rounds ----
 	for (int64_t i = 0; i < S; i++) { // s == t: A[0] = [s], no search
 		KmRow &r = rows[i];
@@ -493,7 +549,10 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 			KmPath q;
 			q.v.push_back(r.s);
 			q.el.push_back(src[r.row]);
-			r.known.insert(q.key());
+			if (costs) {
+				q.cost.push_back(0); // (+0 in both weight types)
+			}
+			r.known.insert(q.key(costs));
 			r.acc.push_back(std::move(q));
 			r.groups = 1;
 			r.live = k > 1;
@@ -503,6 +562,7 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 		std::vector<KmSpur> spurs;
 		std::vector<KmSpurRef> refs;
 		std::vector<int32_t> lists;
+		std::vector<int64_t> roots; // with costs: each spur's root cost
 		for (int64_t i = 0; i < S; i++) {
 			KmRow &r = rows[i];
 			if (!r.live) {
@@ -515,19 +575,21 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 				KmSpur sp = {r.s, r.t, 0, 0, 0, 0, 0, 0, 0};
 				spurs.push_back(sp);
 				refs.push_back({(int32_t)i, 0});
+				roots.push_back(0);
 				continue;
 			}
 			const KmPath &P = r.acc.back();
 			const int64_t L = P.h();
 			const bool closed = r.s == r.t;
-			int64_t j0 = P.dev, j1 = trail ? L : L - 1;
+			// TRAIL and WALK spur at j = L too: past t, and back to it
+			int64_t j0 = P.dev, j1 = trail || path_mode == PGQ_PATH_WALK ? L : L - 1;
 			if (path_mode == PGQ_PATH_SIMPLE && closed && L == 0) {
 				j0 = j1 = 0;
 			}
 			for (int64_t j = j0; j <= j1; j++) {
 				KmSpur sp = {P.v[j], r.t, 0, 0, 0, 0, 0, 0, 0};
 				sp.vb = (int64_t)lists.size();
-				if (!trail) {
+				if (path_mode == PGQ_PATH_ACYCLIC || path_mode == PGQ_PATH_SIMPLE) {
 					for (int64_t x = 0; x <= j; x++) {
 						if (!(closed && P.v[x] == r.t)) {
 							lists.push_back(P.v[x]);
@@ -549,6 +611,7 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 				sp.neb = (int32_t)((int64_t)lists.size() - sp.eb);
 				spurs.push_back(sp);
 				refs.push_back({(int32_t)i, (int32_t)j});
+				roots.push_back(costs ? P.cost[j] : 0);
 			}
 		}
 		// the spurs that take a lane
@@ -564,10 +627,7 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 				PGQ_TRY(pgq_ws_reserve(ws, WS_KM_LISTS, 0, (void **)&d_lists));
 			}
 			PGQ_TRY(pgq_ws_reserve(ws, WS_KM_HAS_SEED, (size_t)ns, (void **)&d_has));
-			k_km_has_seed<<<km_grid((ns + 7) / 8, (int64_t)sms * 16), 256, 0, s>>>(ns, d_spurs, d_lists, csr->out.off,
-			                                                                    csr->out.adj, d_has);
-			PGQ_CUDA(cudaGetLastError());
-			st.kernel_launches++;
+			PGQ_TRY(search.has_seed(ws, ns, d_spurs, d_lists, roots, d_has, &st));
 			std::vector<uint8_t> has((size_t)ns);
 			PGQ_CUDA(cudaMemcpyAsync(has.data(), d_has, (size_t)ns, cudaMemcpyDeviceToHost, s));
 			PGQ_CUDA(cudaStreamSynchronize(s));
@@ -580,8 +640,7 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 			}
 		}
 		const int64_t nl = (int64_t)lane_of.size();
-		const int W = km_lanes(opts, cap, nl);
-		const int wd = W / 64;
+		const int W = km_lanes(opts, search, nl);
 		st.lanes = std::max<int32_t>(st.lanes, W);
 		st.searches += nl;
 		// ---- the round's batches ----
@@ -592,14 +651,6 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 			PGQ_CUDA(cudaMemcpyAsync(lane_spur, lane_of.data() + b0, (size_t)cnt * sizeof(int32_t), cudaMemcpyHostToDevice,
 			                         s));
 			st.h2d_bytes += cnt * (int64_t)sizeof(int32_t);
-			PGQ_CUDA(cudaMemsetAsync(seen, 0, (size_t)n * wd * sizeof(u64), s));
-			PGQ_CUDA(cudaMemsetAsync(front, 0, (size_t)n * wd * sizeof(u64), s));
-			PGQ_CUDA(cudaMemsetAsync(next, 0, (size_t)n * wd * sizeof(u64), s));
-			PGQ_CUDA(cudaMemsetAsync(level, 0xff, (size_t)n * W * sizeof(uint16_t), s));
-			PGQ_CUDA(cudaMemsetAsync(done, 0, (size_t)wd * sizeof(u64), s));
-			PGQ_CUDA(cudaMemsetAsync(grew, 0, (size_t)wd * sizeof(u64), s));
-			PGQ_CUDA(cudaMemsetAsync(hlen, 0, (size_t)W * sizeof(int32_t), s));
-			PGQ_CUDA(cudaMemsetAsync(ctr, 0, 2 * sizeof(u64), s));
 			// TRAIL: the batch's banned positions as sorted (position, lane) keys
 			std::vector<int64_t> keys;
 			const int64_t *d_keys = nullptr;
@@ -618,34 +669,10 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 					st.h2d_bytes += (int64_t)(keys.size() * sizeof(int64_t));
 				}
 			}
-			k_km_seed<<<lane_grid, 256, 0, s>>>(cnt, wd, W, lane_spur, d_spurs, d_lists, csr->out.off, csr->out.adj, seen,
-			                                    front, grew, level, d_keys ? ban_bits : nullptr);
-			PGQ_CUDA(cudaGetLastError());
-			st.kernel_launches++;
 			std::vector<int32_t> h_hlen((size_t)cnt);
-			for (int lv = 2;; lv++) {
-				u64 h_ctr[2];
-				PGQ_CUDA(cudaMemsetAsync(&ctr[KM_ACTIVE], 0, sizeof(u64), s));
-				k_km_finish<<<1, 1024, 0, s>>>(cnt, wd, W, lane_spur, d_spurs, seen, level, grew, done, hlen, ctr);
-				PGQ_CUDA(cudaGetLastError());
-				st.kernel_launches++;
-				PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, s));
-				PGQ_CUDA(cudaMemcpyAsync(h_hlen.data(), hlen, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-				PGQ_CUDA(cudaStreamSynchronize(s));
-				st.d2h_bytes += (int64_t)sizeof(h_ctr) + cnt * (int64_t)sizeof(int32_t);
-				if (h_ctr[KM_TOO_LONG]) {
-					return pgq_fail(PGQ_ERR_UNSUPPORTED, "a spur search went beyond %d edges", KM_PATH_MAX);
-				}
-				if (!h_ctr[KM_ACTIVE]) {
-					break;
-				}
-				k_km_level<<<edge_grid, 256, 0, s>>>(m, n, wd, csr->out.off, csr->out.adj, front, seen, done,
-				                                     d_keys ? ban_bits : nullptr, d_keys, (int64_t)keys.size(), next);
-				k_km_fold<<<vert_grid, 256, 0, s>>>(n, wd, W, lv, seen, front, next, grew, level, ctr);
-				PGQ_CUDA(cudaGetLastError());
-				st.kernel_launches += 2;
-				st.levels++;
-			}
+			const KmBatch b = {cnt,       W,      lane_grid, lane_spur, d_spurs, d_lists, d_keys ? ban_bits : nullptr,
+			                   d_keys,    (int64_t)keys.size(), hlen, h_hlen.data()};
+			PGQ_TRY(search.search(ws, b, &st));
 			// ---- walk the found spurs back and add their candidates to the rows' pools ----
 			std::vector<int64_t> h_off((size_t)cnt);
 			int64_t tot = 0;
@@ -658,18 +685,23 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 			}
 			int2 *d_steps;
 			longlong2 *d_sel;
+			int64_t *d_w = nullptr;
 			PGQ_TRY(pgq_ws_reserve(ws, WS_KM_STEPS, (size_t)tot * sizeof(int2), (void **)&d_steps));
 			PGQ_TRY(pgq_ws_reserve(ws, WS_KM_STEP_ELEMS, (size_t)tot * sizeof(longlong2), (void **)&d_sel));
+			if (costs) {
+				PGQ_TRY(pgq_ws_reserve(ws, WS_CK_STEP_W, (size_t)tot * sizeof(int64_t), (void **)&d_w));
+			}
 			PGQ_CUDA(cudaMemcpyAsync(lane_off, h_off.data(), (size_t)cnt * sizeof(int64_t), cudaMemcpyHostToDevice, s));
-			k_km_walk<<<lane_grid, 256, 0, s>>>(cnt, W, n, lane_spur, d_spurs, d_lists, hlen, lane_off, level, csr->in.off,
-			                                    step_key, step_pos, csr->perm, csr->inv, csr->out.off, csr->out.adj,
-			                                    csr->edge_ids, d_steps, d_sel);
-			PGQ_CUDA(cudaGetLastError());
-			st.kernel_launches++;
+			PGQ_TRY(search.walk(ws, b, lane_off, d_steps, d_sel, d_w, &st));
 			std::vector<int2> h_steps((size_t)tot);
 			std::vector<longlong2> h_sel((size_t)tot);
+			std::vector<int64_t> h_w(costs ? (size_t)tot : 0);
 			PGQ_CUDA(cudaMemcpyAsync(h_steps.data(), d_steps, (size_t)tot * sizeof(int2), cudaMemcpyDeviceToHost, s));
 			PGQ_CUDA(cudaMemcpyAsync(h_sel.data(), d_sel, (size_t)tot * sizeof(longlong2), cudaMemcpyDeviceToHost, s));
+			if (costs) {
+				PGQ_CUDA(cudaMemcpyAsync(h_w.data(), d_w, (size_t)tot * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+				st.d2h_bytes += tot * (int64_t)sizeof(int64_t);
+			}
 			PGQ_CUDA(cudaStreamSynchronize(s));
 			st.h2d_bytes += cnt * (int64_t)sizeof(int64_t);
 			st.d2h_bytes += tot * (int64_t)(sizeof(int2) + sizeof(longlong2));
@@ -685,11 +717,17 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 				if (round == 0) {
 					q.v.push_back(r.s);
 					q.el.push_back(src[r.row]);
+					if (costs) {
+						q.cost.push_back(0);
+					}
 				} else {
 					const KmPath &P = r.acc.back();
 					q.v.assign(P.v.begin(), P.v.begin() + ref.j + 1);
 					q.pos.assign(P.pos.begin(), P.pos.begin() + ref.j);
 					q.el.assign(P.el.begin(), P.el.begin() + 2 * ref.j + 1);
+					if (costs) {
+						q.cost.assign(P.cost.begin(), P.cost.begin() + ref.j + 1);
+					}
 				}
 				for (int64_t i = 0; i < h; i++) {
 					const int2 stp = h_steps[(size_t)(h_off[(size_t)l] + i)];
@@ -699,8 +737,11 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 					q.v.push_back(last ? r.t : h_steps[(size_t)(h_off[(size_t)l] + i + 1)].x);
 					q.el.push_back(sel.y);
 					q.el.push_back(last ? dst[r.row] : h_sel[(size_t)(h_off[(size_t)l] + i + 1)].x);
+					if (costs) {
+						q.cost.push_back(add(q.cost.back(), h_w[(size_t)(h_off[(size_t)l] + i)]));
+					}
 				}
-				std::vector<int64_t> key = q.key();
+				std::vector<int64_t> key = q.key(costs);
 				if (r.known.insert(key).second) {
 					r.pool.emplace(std::move(key), std::move(q));
 				}
@@ -766,9 +807,11 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 	PGQ_CUDA(cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end));
 	int64_t *h_off = (int64_t *)malloc((size_t)(npaths + 1) * sizeof(int64_t));
 	int64_t *h_elems = (int64_t *)malloc((size_t)std::max<u64>(elem_total, 1) * sizeof(int64_t));
-	if (!h_off || !h_elems) {
+	int64_t *h_costs = out_costs ? (int64_t *)malloc((size_t)std::max<u64>(npaths, 1) * sizeof(int64_t)) : nullptr;
+	if (!h_off || !h_elems || (out_costs && !h_costs)) {
 		free(h_off);
 		free(h_elems);
+		free(h_costs);
 		return pgq_fail(PGQ_ERR_OOM, "host allocation of %llu path elements failed", (unsigned long long)elem_total);
 	}
 	memset(out_npaths, 0, (size_t)p * sizeof(int64_t));
@@ -801,6 +844,9 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 		out_first_path[i] = np;
 		if (ri < rows.size() && rows[ri].row == i) {
 			for (const KmPath &q : rows[ri].acc) {
+				if (h_costs) {
+					h_costs[np] = q.cost.back();
+				}
 				h_off[np++] = ne;
 				memcpy(h_elems + ne, q.el.data(), q.el.size() * sizeof(int64_t));
 				ne += (int64_t)q.el.size();
@@ -812,6 +858,9 @@ static int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 	st.total_ms = ms;
 	*out_path_offsets = h_off;
 	*out_elems = h_elems;
+	if (out_costs) {
+		*out_costs = h_costs;
+	}
 	*out_total_paths = np;
 	if (stats) {
 		*stats = st;
@@ -833,8 +882,9 @@ extern "C" int pgq_shortest_k_paths_mode(pgq_csr *csr, int64_t p, const int64_t 
 	}
 	PGQ_TRY(ks_check_call(csr, p, src, dst, opts, k, out_npaths, out_first_path, out_valid, out_path_offsets, out_elems,
 	                      out_total_paths));
-	return km_run(csr, p, src, dst, src_valid, dst_valid, opts, k, path_mode, nullptr, out_npaths, out_first_path,
-	              out_valid, out_path_offsets, out_elems, out_total_paths, stats);
+	KmBfs bfs(csr, opts);
+	return km_run(csr, p, src, dst, src_valid, dst_valid, opts, k, path_mode, nullptr, bfs, out_npaths, out_first_path,
+	              out_valid, out_path_offsets, out_elems, nullptr, out_total_paths, stats);
 }
 
 extern "C" int pgq_shortest_k_groups(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst,
@@ -862,6 +912,7 @@ extern "C" int pgq_shortest_k_groups(pgq_csr *csr, int64_t p, const int64_t *src
 		               out_total_paths, stats);
 	}
 	const KmGroups kg = {max_paths, out_count, out_ngroups, out_last_len, out_complete};
-	return km_run(csr, p, src, dst, src_valid, dst_valid, opts, k, path_mode, &kg, out_npaths, out_first_path,
-	              out_valid, out_path_offsets, out_elems, out_total_paths, stats);
+	KmBfs bfs(csr, opts);
+	return km_run(csr, p, src, dst, src_valid, dst_valid, opts, k, path_mode, &kg, bfs, out_npaths, out_first_path,
+	              out_valid, out_path_offsets, out_elems, nullptr, out_total_paths, stats);
 }

@@ -74,6 +74,7 @@ static std::atomic<int64_t> g_calls_cheapest_path {0};
 static std::atomic<int64_t> g_calls_path_count {0};
 static std::atomic<int64_t> g_calls_cheapest_count {0};
 static std::atomic<int64_t> g_calls_all_cheapest {0};
+static std::atomic<int64_t> g_calls_cheapest_k {0};
 static std::atomic<int64_t> g_calls_all_shortest {0};
 static std::atomic<int64_t> g_calls_shortest_k {0};
 static std::atomic<int64_t> g_calls_shortest_k_mode {0};
@@ -982,7 +983,7 @@ static void AllShortestPathsB200Function(DataChunk &args, ExpressionState &state
 // The k shortest walks of a row (include/duckpgq_b200.h, pgq_shortest_k_paths), called as a raw UDF over the CSR CTE:
 // the MATCH rewriter stays the reference's, which rejects SHORTEST k (match.cpp:84-86).  The bind is shortestpath's
 // and also wants a constant k >= 1; the CSR lookup is shortestpath's.
-static unique_ptr<FunctionData> ShortestKPathsBind(BindScalarFunctionInput &input) {
+static void CheckConstantK(BindScalarFunctionInput &input) {
 	auto &arguments = input.GetArguments();
 	if (!arguments[4]->IsFoldable()) {
 		throw InvalidInputException("k must be constant.");
@@ -991,6 +992,10 @@ static unique_ptr<FunctionData> ShortestKPathsBind(BindScalarFunctionInput &inpu
 	if (k.IsNull() || k.GetValue<int64_t>() < 1) {
 		throw InvalidInputException("k must be 1 or more.");
 	}
+}
+
+static unique_ptr<FunctionData> ShortestKPathsBind(BindScalarFunctionInput &input) {
+	CheckConstantK(input);
 	return IterativeLengthFunctionData::IterativeLengthBind(input);
 }
 
@@ -1006,7 +1011,7 @@ static int32_t PathModeId(const string &name) {
 
 // shortest_k_paths(INTEGER, BIGINT, BIGINT, BIGINT, BIGINT k, VARCHAR mode): the 5-argument bind, and a constant mode
 // that names a path mode
-static unique_ptr<FunctionData> ShortestKPathsModeBind(BindScalarFunctionInput &input) {
+static void CheckConstantMode(BindScalarFunctionInput &input) {
 	auto &arguments = input.GetArguments();
 	if (!arguments[5]->IsFoldable()) {
 		throw InvalidInputException("the path mode must be constant.");
@@ -1015,6 +1020,10 @@ static unique_ptr<FunctionData> ShortestKPathsModeBind(BindScalarFunctionInput &
 	if (mode.IsNull() || PathModeId(mode.GetValue<string>()) < 0) {
 		throw InvalidInputException("the path mode must be WALK, TRAIL, ACYCLIC or SIMPLE.");
 	}
+}
+
+static unique_ptr<FunctionData> ShortestKPathsModeBind(BindScalarFunctionInput &input) {
+	CheckConstantMode(input);
 	return ShortestKPathsBind(input);
 }
 
@@ -1425,6 +1434,91 @@ static void AllCheapestPathsB200Function(DataChunk &args, ExpressionState &state
 	GetDuckPGQState(info.context)->csr_to_delete.insert(info.csr_id);
 }
 
+// ---- cheapest_k_paths / cheapest_k_costs (no reference function) ----------------------------------------------
+// The k cheapest paths of a row in a path mode and their costs (include/duckpgq_b200.h, pgq_cheapest_k_paths),
+// SQL/PGQ's CHEAPEST k, raw UDFs over the weighted CSR CTE like cheapest_path.  The binds are cheapest_path's with
+// shortest_k_paths' checks of a constant k >= 1 and, with a 6th argument, of a constant path mode.  cheapest_k_costs
+// returns a LIST of the CSR's weight type, chosen as cheapest_path_length's bind chooses its result
+// (cheapest_path_length_function_data.cpp:25-29).  Both count as cheapest_k_paths_calls.
+static unique_ptr<FunctionData> CheapestKBind(BindScalarFunctionInput &input) {
+	CheckConstantK(input);
+	if (input.GetArguments().size() > 5) {
+		CheckConstantMode(input);
+	}
+	return CheapestPathBind(input);
+}
+
+static unique_ptr<FunctionData> CheapestKPathsBind(BindScalarFunctionInput &input) {
+	auto data = CheapestKBind(input);
+	input.GetBoundFunction().SetReturnType(LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT)));
+	return data;
+}
+
+static unique_ptr<FunctionData> CheapestKCostsBind(BindScalarFunctionInput &input) {
+	auto data = CheapestKBind(input);
+	CSR *csr = GetDuckPGQState(input.GetClientContext())->GetCSR(data->Cast<CheapestPathLengthFunctionData>().csr_id);
+	input.GetBoundFunction().SetReturnType(LogicalType::LIST(csr->w.empty() ? LogicalType::DOUBLE : LogicalType::BIGINT));
+	return data;
+}
+
+// Both UDFs: pgq_cheapest_k_paths over the chunk's rows, then the rows' path lists, or their cost lists (the raw 8-byte
+// costs: BIGINT and DOUBLE have the same width).  opts stay null: the call picks its own lane width.
+static void CheapestKRows(DataChunk &args, ExpressionState &state, Vector &result, bool costs) {
+	auto &func_expr = state.expr.Cast<BoundFunctionExpression>();
+	auto &info = func_expr.BindInfo()->Cast<CheapestPathLengthFunctionData>();
+	pgq_csr *device_csr = CheapestCsr(info.context, info.csr_id, costs ? "cheapest_k_costs" : "cheapest_k_paths");
+	int64_t k = args.data[4].GetValue(0).GetValue<int64_t>(); // (constant: CheapestKBind)
+	int32_t mode = args.ColumnCount() > 5 ? PathModeId(args.data[5].GetValue(0).GetValue<string>()) : PGQ_PATH_WALK;
+	idx_t count = args.size();
+	CheapestPairs pairs(args);
+	vector<int64_t> npaths(count), first(count);
+	vector<uint8_t> out_valid(count);
+	int64_t *offsets = nullptr, *elems = nullptr;
+	void *cost_bits = nullptr;
+	int64_t paths = 0;
+	int st = pgq_cheapest_k_paths(device_csr, static_cast<int64_t>(count), pairs.src.data(), pairs.dst.data(),
+	                              pairs.src_valid.data(), pairs.dst_valid.data(), nullptr, k, mode, npaths.data(),
+	                              first.data(), out_valid.data(), &offsets, &elems, costs ? &cost_bits : nullptr, &paths,
+	                              nullptr);
+	if (st != PGQ_OK) {
+		ThrowStatus(st);
+	}
+	g_calls_cheapest_k++;
+	g_pairs += static_cast<int64_t>(count);
+	if (!costs) {
+		SetPathLists(result, count, offsets, elems, paths, first, npaths, out_valid);
+	} else {
+		result.SetVectorType(VectorType::FLAT_VECTOR);
+		auto result_data = FlatVector::GetDataMutable<list_entry_t>(result);
+		ValidityMask &result_validity = FlatVector::ValidityMutable(result);
+		ListVector::Reserve(result, static_cast<idx_t>(paths));
+		if (paths > 0) {
+			memcpy(FlatVector::GetDataMutable<int64_t>(ListVector::GetChildMutable(result)), cost_bits,
+			       static_cast<size_t>(paths) * sizeof(int64_t));
+		}
+		ListVector::SetListSize(result, static_cast<idx_t>(paths));
+		for (idx_t i = 0; i < count; i++) {
+			result_data[i].offset = static_cast<idx_t>(first[i]);
+			result_data[i].length = static_cast<idx_t>(npaths[i]);
+			if (!out_valid[i]) {
+				result_validity.SetInvalid(i);
+			}
+		}
+	}
+	pgq_free(offsets);
+	pgq_free(elems);
+	pgq_free(cost_bits);
+	GetDuckPGQState(info.context)->csr_to_delete.insert(info.csr_id);
+}
+
+static void CheapestKPathsB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	CheapestKRows(args, state, result, false);
+}
+
+static void CheapestKCostsB200Function(DataChunk &args, ExpressionState &state, Vector &result) {
+	CheapestKRows(args, state, result, true);
+}
+
 // ---- local_clustering_coefficient / pagerank / weakly_connected_component ---------------------------------------
 // Registered through WrapScalar, so the signatures and binds are the reference's; the reference callback is not
 // called.  The device CSR is found like a path function's (the device build, or an upload of the host CSR).
@@ -1548,7 +1642,8 @@ static void B200StatsFunction(DataChunk &args, ExpressionState &state, Vector &r
 	              ",shortest_k_groups_calls=" + std::to_string(g_calls_shortest_k_groups.load()) +
 	              ",shortest_k_groups_count_calls=" + std::to_string(g_calls_shortest_k_groups_count.load()) +
 	              ",cheapest_path_count_calls=" + std::to_string(g_calls_cheapest_count.load()) +
-	              ",all_cheapest_paths_calls=" + std::to_string(g_calls_all_cheapest.load());
+	              ",all_cheapest_paths_calls=" + std::to_string(g_calls_all_cheapest.load()) +
+	              ",cheapest_k_paths_calls=" + std::to_string(g_calls_cheapest_k.load());
 	result.SetVectorType(VectorType::CONSTANT_VECTOR);
 	ConstantVector::GetData<string_t>(result)[0] = StringVector::AddString(result, text);
 }
@@ -1662,6 +1757,23 @@ static void LoadInternal(ExtensionLoader &loader) {
 	    "all_cheapest_paths",
 	    {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT},
 	    LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT)), AllCheapestPathsB200Function, AllCheapestPathsBind));
+	// cheapest_k_paths / cheapest_k_costs: CHEAPEST k's paths and their costs, raw UDFs like cheapest_path (5 arguments:
+	// WALK; a 6th, VARCHAR mode)
+	const vector<LogicalType> ck_args {LogicalType::INTEGER, LogicalType::BIGINT, LogicalType::BIGINT, LogicalType::BIGINT,
+	                                   LogicalType::BIGINT};
+	vector<LogicalType> ck_mode_args = ck_args;
+	ck_mode_args.push_back(LogicalType::VARCHAR);
+	ScalarFunctionSet cheapest_k {Identifier("cheapest_k_paths")};
+	for (auto &sig : {ck_args, ck_mode_args}) {
+		cheapest_k.AddFunction(ScalarFunction(sig, LogicalType::LIST(LogicalType::LIST(LogicalType::BIGINT)),
+		                                      CheapestKPathsB200Function, CheapestKPathsBind));
+	}
+	loader.RegisterFunction(cheapest_k);
+	ScalarFunctionSet cheapest_k_costs {Identifier("cheapest_k_costs")};
+	for (auto &sig : {ck_args, ck_mode_args}) {
+		cheapest_k_costs.AddFunction(ScalarFunction(sig, LogicalType::ANY, CheapestKCostsB200Function, CheapestKCostsBind));
+	}
+	loader.RegisterFunction(cheapest_k_costs);
 	// shortest_path_count / all_shortest_paths: no reference function is replaced; raw UDFs over the CSR CTE (the
 	// reference's MATCH rewriter rejects ALL SHORTEST)
 	loader.RegisterFunction(ScalarFunction(

@@ -554,6 +554,43 @@ class DeviceCSR:
         paths = [walks[first[i]: first[i] + npaths[i]] if ov[i] else None for i in range(p)]
         return paths, npaths[:p], st.as_dict()
 
+    def cheapest_k_paths(self, src, dst, k: int, src_valid=None, dst_valid=None, options: Optional[Options] = None,
+                         mode: str = "WALK"):
+        """-> (per row: list of [src, e1, v1, ..., dst] paths or None, per row: list of costs (int for BIGINT weights,
+        float for DOUBLE) or None, npaths int64, stats dict): the first min(k, total) paths of each row in the path mode
+        ("WALK", "TRAIL", "ACYCLIC" or "SIMPLE", any case), cheapest first, then by length and step order, over a CSR
+        with weights >= 0 (include/duckpgq_b200.h, pgq_cheapest_k_paths)."""
+        path_mode = path_mode_id(mode)
+        src, dst = _i64(src), _i64(dst)
+        p = src.shape[0]
+        sv = None if src_valid is None else np.ascontiguousarray(src_valid, dtype=np.uint8)
+        dv = None if dst_valid is None else np.ascontiguousarray(dst_valid, dtype=np.uint8)
+        npaths = np.zeros(max(p, 1), dtype=np.int64)
+        first = np.zeros(max(p, 1), dtype=np.int64)
+        ov = np.zeros(max(p, 1), dtype=np.uint8)
+        offs, elems = C.POINTER(C.c_int64)(), C.POINTER(C.c_int64)()
+        costs = C.c_void_p()
+        total = C.c_int64(0)
+        st = _native.PgqStats()
+        opts = (options or Options()).c()
+        _check(self._lib.pgq_cheapest_k_paths(self._h, p, _p64(src), _p64(dst), _pu8(sv), _pu8(dv), C.byref(opts),
+                                              int(k), path_mode, _p64(npaths), _p64(first), _pu8(ov), C.byref(offs),
+                                              C.byref(elems), C.byref(costs), C.byref(total), C.byref(st)))
+        try:
+            woff = np.ctypeslib.as_array(offs, shape=(total.value + 1,)).copy()
+            flat = np.ctypeslib.as_array(elems, shape=(int(woff[-1]),)).copy() if woff[-1] else np.zeros(0, np.int64)
+            cbits = (np.ctypeslib.as_array(C.cast(costs, C.POINTER(C.c_int64)), shape=(total.value,)).copy()
+                     if total.value else np.zeros(0, np.int64))
+        finally:
+            self._lib.pgq_free(offs)
+            self._lib.pgq_free(elems)
+            self._lib.pgq_free(costs)
+        cvals = (cbits.view(np.float64) if self.weight_type() == 2 else cbits).tolist()
+        walks = [flat[woff[j]: woff[j + 1]].tolist() for j in range(total.value)]
+        paths = [walks[first[i]: first[i] + npaths[i]] if ov[i] else None for i in range(p)]
+        cost_rows = [cvals[first[i]: first[i] + npaths[i]] if ov[i] else None for i in range(p)]
+        return paths, cost_rows, npaths[:p], st.as_dict()
+
     def shortest_k_groups(self, src, dst, k: int, max_paths: int = 0, src_valid=None, dst_valid=None,
                           options: Optional[Options] = None, mode: str = "WALK"):
         """-> (per row: list of [src, e1, v1, ..., dst] paths or None, counts int64, ngroups int64, last_len int64,
@@ -765,6 +802,18 @@ def all_cheapest_paths(state: DuckPGQState, csr_id: int, v_size: int, src, dst, 
     paths, _, _ = csr.all_cheapest_paths(src, dst, max_paths, src_valid, dst_valid)
     state.csr_to_delete.add(csr_id)
     return paths
+
+
+def cheapest_k_paths(state: DuckPGQState, csr_id: int, v_size: int, src, dst, k: int, src_valid=None, dst_valid=None,
+                     options: Optional[Options] = None, mode: str = "WALK"):
+    """cheapest_k_paths(INT, BIGINT, BIGINT, BIGINT, BIGINT k[, VARCHAR mode]) -> LIST(LIST(BIGINT)): per row the first
+    min(k, total) paths of the path mode, cheapest first, or None (no reference function; looked up and marked as
+    cheapest_path is).  Returns (paths, costs): costs per row in the CSR's weight type, or None."""
+    path_mode_id(mode)
+    csr = _lookup_weighted(state, csr_id)
+    paths, costs, _, _ = csr.cheapest_k_paths(src, dst, k, src_valid, dst_valid, options, mode)
+    state.csr_to_delete.add(csr_id)
+    return paths, costs
 
 
 def _lookup_for_path(state: DuckPGQState, csr_id: int, lengths: bool) -> DeviceCSR:

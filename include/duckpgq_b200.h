@@ -472,6 +472,58 @@ int pgq_shortest_k_paths_mode(pgq_csr *csr, int64_t n_pairs, const int64_t *src,
                               int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths,
                               pgq_stats *stats);
 
+/* pgq_cheapest_k_paths: the k cheapest paths of a row in a path mode (SQL/PGQ's CHEAPEST k; no reference function),
+ * over a CSR built with pgq_csr_add_edges_weighted (BIGINT or DOUBLE weights).  For a row (s, t), a path mode M (a
+ * pgq_path_mode; another value -> PGQ_ERR_INVALID_ARG) and k >= 1:
+ *   - weights: every weight must be >= 0 (-0.0 is not below zero); a CSR with a weight below zero (a spur search would
+ *     need negative-cycle detection, and the cheapest ACYCLIC path under a negative cycle is NP-hard to find) ->
+ *     PGQ_ERR_UNSUPPORTED, checked before any work.  An edge of NaN weight belongs to no path.
+ *   - cost(P) = P's weights added left to right from 0 in the weight type's arithmetic (int64 addition; double addition
+ *     rounded to nearest).  A list is not a path when its cost is NaN or reaches pgq_cheapest_path_length's sentinel
+ *     (INT64_MAX / 2; DBL_MAX / 2), tested before each addition (for BIGINT w < sentinel - c), so nothing overflows.
+ *     Prefix costs never decrease, so a row has a path exactly when pgq_cheapest_path_length's cost is not NULL.
+ *   - format, modes and NULL rows are pgq_shortest_k_paths_mode's: a path is [s, e1, v1, ..., eh, t]; WALK, TRAIL,
+ *     ACYCLIC and SIMPLE admit paths by the same rules, TRAIL's adjacency-entry edges and the s == t cases included;
+ *     NULL (out_valid 0, no paths): a NULL id, or no admitted path.
+ *   - order: by cost ascending (compared as values), then by h, then by the steps from t back to s as
+ *     pgq_shortest_k_paths orders them.  The result is the first min(k, total) admitted paths in that order; with
+ *     weights >= 0 that prefix exists even when zero-cost cycles make WALK's total infinite.  s == t: path 0 is [s]
+ *     with cost 0.  k = 1 gives pgq_cheapest_path's path in every mode, with pgq_cheapest_path_length's cost; with every
+ *     weight 0 or every weight 1 (BIGINT) the paths are pgq_shortest_k_paths_mode's.
+ *   - DOUBLE: the order above is exact for BIGINT.  For DOUBLE it holds whenever every sum involved is exact (dyadic
+ *     weights, for example); when a sum rounds, the construction below is the contract, as the tight-edge rule is for
+ *     pgq_all_cheapest_paths.  With edges 0 -> 1 (0.1), 1 -> 2 (0.2) and 0 -> 2 (0.3), WALK's two paths from 0 to 2 are
+ *     [0, e, 2] (cost 0.3) and then [0, e, 1, e, 2] (cost 0.1 + 0.2 = 0.30000000000000004).
+ *   - outputs: pgq_shortest_k_paths' layout (out_npaths, out_first_path, out_valid, *out_path_offsets, *out_elems,
+ *     *out_total_paths), and when out_costs is not null, *out_costs = the *out_total_paths paths' costs as raw 8-byte
+ *     values of the weight type.  The arrays are allocated by the library (also for zero rows): release with pgq_free().
+ *   - errors: k < 1 -> PGQ_ERR_INVALID_ARG; opts->lanes not 0, 32, 64, 128 or 256 -> PGQ_ERR_INVALID_ARG; an unweighted,
+ *     missing or unfinalised CSR -> pgq_cheapest_path's errors; ids outside [0, n) in a row whose ids are both valid ->
+ *     PGQ_ERR_RANGE; shard_count > 1 -> PGQ_ERR_UNSUPPORTED; a spur search whose tight depth passes 65534, or a row that
+ *     accepts a path longer than 65533 edges -> PGQ_ERR_UNSUPPORTED; an element total that overflows int64 or cannot be
+ *     allocated -> PGQ_ERR_OOM, checked before anything of that size is allocated.  opts->direction, alpha and flags
+ *     are not used, and no result depends on the lane width.
+ *   - the call (DESIGN.md §3): pgq_shortest_k_paths_mode's rounds (Yen's algorithm with Lawler's rule, its spur ranges,
+ *     bans, D and pool) with the pool keyed by (cost, h, steps), and WALK spurring at dev <= j <= L like TRAIL, with no
+ *     bans beyond D.  A spur search from u = P[j] with root R is a lane of a batched Bellman-Ford: each admissible first
+ *     edge u -> x seeds d(x) = min(cost(R) + w); sweeps relax the lane's unbanned edges to the fixed point; a BFS over
+ *     the lane's tight edges (d(v) + w == d(x) as values, pgq_cheapest_path's rule) from the tight seeds levels the
+ *     vertices; and the walk back from t takes, at level >= 2, the first step-list entry whose parent has level - 1 and
+ *     whose edge is tight and not banned, at level 1 the first admissible tight position of u's adjacency.  A spur with
+ *     no admissible seed takes no lane.  W = opts->lanes, or for 0 the widest of 256, 128, 64, 32 whose distance array
+ *     n x W x 8 bytes fits 2 GiB, halved while W > 32 and the round's searches are at most W / 2; a round's searches take
+ *     lanes in (row, j) order, and batches never mix rounds.
+ *   - stats: batches (spur batches over all rounds); lanes (the widest W of the call); searches (spur searches that took
+ *     a lane); levels (Bellman-Ford sweeps summed over batches: at least one per batch, otherwise not deterministic);
+ *     push_levels (tight-BFS levels summed over batches: a batch expands while a lane that has not levelled its target
+ *     grew at the last level); kernel_launches, h2d_bytes, d2h_bytes and total_ms (the whole call).  The other counters
+ *     are 0. */
+int pgq_cheapest_k_paths(pgq_csr *csr, int64_t n_pairs, const int64_t *src, const int64_t *dst,
+                         const uint8_t *src_valid, const uint8_t *dst_valid, const pgq_options *opts, int64_t k,
+                         int32_t path_mode, int64_t *out_npaths, int64_t *out_first_path, uint8_t *out_valid,
+                         int64_t **out_path_offsets, int64_t **out_elems, void **out_costs, int64_t *out_total_paths,
+                         pgq_stats *stats);
+
 /* pgq_shortest_k_groups: the paths of the k shortest lengths of a row (SQL/PGQ's SHORTEST k GROUP; the reference
  * carries the selector in its AST and rejects it).  No reference function.  For a row (s, t), a path mode M (a
  * pgq_path_mode; another value -> PGQ_ERR_INVALID_ARG) and k >= 1:
