@@ -100,6 +100,15 @@ SYMBOLS = {
                                                 C.POINTER(_VP)]),
     "pgq_csr_build_keys_undirected_device": (C.c_int, [_VP, C.c_int64, _VP, _VP, C.c_int64, _VP, _VP, _VP, _VP,
                                                        C.POINTER(_VP)]),
+    "pgq_csr_build_weighted": (C.c_int, [_VP, C.c_int64, C.c_int64, _P64, _P64, _P64, _P64, C.POINTER(C.c_double),
+                                         C.POINTER(_VP)]),
+    "pgq_csr_build_device_weighted": (C.c_int, [_VP, C.c_int64, C.c_int64, _VP, _VP, _VP, _VP, _VP, C.POINTER(_VP)]),
+    "pgq_csr_upload_weighted": (C.c_int, [_VP, C.c_int64, C.c_int64, _P64, _P64, _P64, _P64, C.POINTER(C.c_double),
+                                          C.POINTER(_VP)]),
+    "pgq_csr_build_keys_weighted": (C.c_int, [_VP, C.c_int64, _P64, _PU8, C.c_int64, _P64, _P64, _PU8, _PU8, _P64,
+                                              C.POINTER(C.c_double), _PU8, C.POINTER(_VP)]),
+    "pgq_csr_build_keys_weighted_device": (C.c_int, [_VP, C.c_int64, _VP, _VP, C.c_int64, _VP, _VP, _VP, _VP, _VP, _VP,
+                                                     _VP, C.POINTER(_VP)]),
     "pgq_csr_download": (C.c_int, [_VP, _P64, _P64, _P64]),
     "pgq_csr_info": (C.c_int, [_VP, _P64, _P64, _P64]),
     "pgq_csr_weight_type": (C.c_int, [_VP, C.POINTER(C.c_int)]),

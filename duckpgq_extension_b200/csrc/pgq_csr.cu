@@ -1597,6 +1597,9 @@ static int finalize_from_rows(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 		k_histogram<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(csr->st_src, m, csr->out.off);
 	}
 	PGQ_TRY(pgq_scan_exclusive_i32(csr->out.off, csr->out.off, n + 1, scan_tmp, s));
+	if (csr->st_w) { // (a one-shot build stages its weight column, and so records its weight type, even for m = 0)
+		PGQ_TRY(dev_alloc(csr, (void **)&csr->w_bits, (size_t)std::max<int64_t>(m, 1) * sizeof(int64_t)));
+	}
 	if (m > 0) {
 		int32_t *keys_out, *perm_in, *perm_out, *keys_res;
 		PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_EDGE_A, (size_t)m * sizeof(int32_t), (void **)&keys_out));
@@ -1610,9 +1613,6 @@ static int finalize_from_rows(pgq_csr *csr, Workspace *ws, cudaStream_t s) {
 		PGQ_CUDA(cudaGetLastError());
 		// (st_src is staging and may be clobbered: the out-degree histogram above already used it)
 		PGQ_TRY(radix_sort_pairs(ws, csr->st_src, keys_out, perm_in, perm_out, m, end_bit, s, &keys_res, &perm_out));
-		if (csr->st_w) {
-			PGQ_TRY(dev_alloc(csr, (void **)&csr->w_bits, (size_t)m * sizeof(int64_t)));
-		}
 		k_gather_edges<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(perm_out, csr->st_dst, csr->st_eid, csr->st_w, m,
 		                                                       csr->out.adj, csr->edge_ids, csr->w_bits);
 		PGQ_CUDA(cudaGetLastError());
@@ -1669,8 +1669,32 @@ extern "C" int pgq_csr_finalize(pgq_csr *csr) {
 	return PGQ_OK;
 }
 
-// The edge rows of pgq_csr_build into the staging columns (ids narrowed and range-checked).
-static int upload_rows(pgq_csr *csr, const int64_t *src, const int64_t *dst, const int64_t *eid) {
+// The weight column of a one-shot build: exactly one of the BIGINT / DOUBLE pointers, as for
+// pgq_csr_add_edges_weighted, and even for m = 0 (the pointer names the type).  -> its bits and the weight type.
+static int weight_arg(const int64_t *w_i64, const double *w_f64, const void **w, int *weight_type) {
+	if ((w_i64 != nullptr) == (w_f64 != nullptr)) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "exactly one of weight_i64 / weight_f64 must be given");
+	}
+	*w = w_i64 ? (const void *)w_i64 : (const void *)w_f64;
+	*weight_type = w_i64 ? 1 : 2;
+	return PGQ_OK;
+}
+
+// The staging columns of a one-shot build of `rows` edge rows, with a weight column when weight_type != 0.
+static int alloc_staging(pgq_csr *csr, int64_t rows, int weight_type) {
+	const size_t cap = (size_t)std::max<int64_t>(rows, 1);
+	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_src, cap * sizeof(int32_t)));
+	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_dst, cap * sizeof(int32_t)));
+	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_eid, cap * sizeof(int64_t)));
+	if (weight_type) {
+		PGQ_TRY(dev_alloc(csr, (void **)&csr->st_w, cap * sizeof(int64_t)));
+	}
+	csr->weight_type = weight_type;
+	return PGQ_OK;
+}
+
+// The edge rows of pgq_csr_build into the staging columns (ids narrowed and range-checked; weights as 8-byte patterns).
+static int upload_rows(pgq_csr *csr, const int64_t *src, const int64_t *dst, const int64_t *eid, const void *w) {
 	const int64_t n = csr->n, m = csr->m;
 	WsGuard g(csr->ctx);
 	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
@@ -1678,6 +1702,9 @@ static int upload_rows(pgq_csr *csr, const int64_t *src, const int64_t *dst, con
 	PGQ_TRY(upload_narrow(g.ws, src, m, 0, n, csr->st_src, csr->d_err, s));
 	PGQ_TRY(upload_narrow(g.ws, dst, m, 0, n, csr->st_dst, csr->d_err, s));
 	cudaError_t e = cudaMemcpyAsync(csr->st_eid, eid, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, s);
+	if (e == cudaSuccess && w) {
+		e = cudaMemcpyAsync(csr->st_w, w, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, s);
+	}
 	if (e == cudaSuccess) {
 		e = cudaStreamSynchronize(s);
 	}
@@ -1689,8 +1716,8 @@ static int upload_rows(pgq_csr *csr, const int64_t *src, const int64_t *dst, con
 	return PGQ_OK;
 }
 
-extern "C" int pgq_csr_build(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *src, const int64_t *dst,
-                             const int64_t *eid, pgq_csr **out) {
+static int csr_build(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *src, const int64_t *dst, const int64_t *eid,
+                     const void *w, int weight_type, pgq_csr **out) {
 	if (!ctx || !out || (m > 0 && (!src || !dst))) {
 		return pgq_fail(PGQ_ERR_INVALID_ARG, "null argument");
 	}
@@ -1710,17 +1737,14 @@ extern "C" int pgq_csr_build(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *
 	// bulk form: whole columns in large pieces (the chunk-wise staging rings are for DataChunk-sized calls)
 	{
 		std::lock_guard<std::mutex> g(csr->mu);
-		const size_t cap = (size_t)std::max<int64_t>(m, 1);
-		st = dev_alloc(csr, (void **)&csr->st_src, cap * sizeof(int32_t));
-		if (st == PGQ_OK) st = dev_alloc(csr, (void **)&csr->st_dst, cap * sizeof(int32_t));
-		if (st == PGQ_OK) st = dev_alloc(csr, (void **)&csr->st_eid, cap * sizeof(int64_t));
+		st = alloc_staging(csr, m, weight_type);
 		csr->edge_size = m;
 		csr->m = m;
 		csr->staged = m;
 		csr->edge_init = true;
 	}
 	if (st == PGQ_OK && m > 0) {
-		st = upload_rows(csr, src, dst, eid);
+		st = upload_rows(csr, src, dst, eid, w);
 	}
 	if (st == PGQ_OK) {
 		st = pgq_csr_finalize(csr);
@@ -1733,6 +1757,20 @@ extern "C" int pgq_csr_build(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *
 	return PGQ_OK;
 }
 
+extern "C" int pgq_csr_build(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *src, const int64_t *dst,
+                             const int64_t *eid, pgq_csr **out) {
+	return csr_build(ctx, n, m, src, dst, eid, nullptr, 0, out);
+}
+
+extern "C" int pgq_csr_build_weighted(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *src, const int64_t *dst,
+                                      const int64_t *eid, const int64_t *weight_i64, const double *weight_f64,
+                                      pgq_csr **out) {
+	const void *w;
+	int weight_type;
+	PGQ_TRY(weight_arg(weight_i64, weight_f64, &w, &weight_type));
+	return csr_build(ctx, n, m, src, dst, eid, w, weight_type, out);
+}
+
 __global__ void k_range_check_i32(const int32_t *__restrict__ ids, int64_t count, int64_t n, int *err) {
 	for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
 		if (ids[i] < 0 || ids[i] >= n) {
@@ -1741,18 +1779,17 @@ __global__ void k_range_check_i32(const int32_t *__restrict__ ids, int64_t count
 	}
 }
 
-// Copies the device edge columns of pgq_csr_build_device into the staging columns and builds from them.
-static int build_from_device_rows(pgq_csr *csr, const int32_t *d_src, const int32_t *d_dst, const int64_t *d_eid) {
+// Copies the device edge columns of pgq_csr_build_device (and its weights, d_w != NULL) into the staging columns and
+// builds from them.
+static int build_from_device_rows(pgq_csr *csr, const int32_t *d_src, const int32_t *d_dst, const int64_t *d_eid,
+                                  const void *d_w, int weight_type) {
 	const int64_t n = csr->n, m = csr->m;
 	WsGuard g(csr->ctx);
 	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
 	cudaStream_t s = g.ws->stream;
 	int *d_err;
-	const size_t cap = (size_t)std::max<int64_t>(m, 1);
 	PGQ_TRY(pgq_ws_reserve(g.ws, WS_CSR_ERR, 256, (void **)&d_err));
-	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_src, cap * sizeof(int32_t)));
-	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_dst, cap * sizeof(int32_t)));
-	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_eid, cap * sizeof(int64_t)));
+	PGQ_TRY(alloc_staging(csr, m, weight_type));
 	cudaMemsetAsync(d_err, 0, sizeof(int), s);
 	// the columns may have been produced on any stream of the caller (torch's, cuDF's): the copies below
 	// run on a stream of ours, so wait for the whole device once rather than race the producer
@@ -1767,6 +1804,9 @@ static int build_from_device_rows(pgq_csr *csr, const int32_t *d_src, const int3
 		} else {
 			k_iota64<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->st_eid, m);
 		}
+		if (d_w) {
+			cudaMemcpyAsync(csr->st_w, d_w, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToDevice, s);
+		}
 	}
 	int flag = 0;
 	PGQ_TRY(read_flag(d_err, s, &flag));
@@ -1778,8 +1818,8 @@ static int build_from_device_rows(pgq_csr *csr, const int32_t *d_src, const int3
 	return PGQ_OK;
 }
 
-extern "C" int pgq_csr_build_device(pgq_ctx *ctx, int64_t n, int64_t m, const int32_t *d_src, const int32_t *d_dst,
-                                    const int64_t *d_eid, pgq_csr **out) {
+static int csr_build_device(pgq_ctx *ctx, int64_t n, int64_t m, const int32_t *d_src, const int32_t *d_dst,
+                            const int64_t *d_eid, const void *d_w, int weight_type, pgq_csr **out) {
 	if (!ctx || !out || (m > 0 && (!d_src || !d_dst))) {
 		return pgq_fail(PGQ_ERR_INVALID_ARG, "null argument");
 	}
@@ -1796,7 +1836,7 @@ extern "C" int pgq_csr_build_device(pgq_ctx *ctx, int64_t n, int64_t m, const in
 	csr->edge_size = m;
 	csr->staged = m;
 	csr->edge_init = true;
-	const int st = build_from_device_rows(csr, d_src, d_dst, d_eid);
+	const int st = build_from_device_rows(csr, d_src, d_dst, d_eid, d_w, weight_type);
 	if (st != PGQ_OK) {
 		pgq_csr_free(csr);
 		return st;
@@ -1804,6 +1844,20 @@ extern "C" int pgq_csr_build_device(pgq_ctx *ctx, int64_t n, int64_t m, const in
 	free_staging(csr);
 	*out = csr;
 	return PGQ_OK;
+}
+
+extern "C" int pgq_csr_build_device(pgq_ctx *ctx, int64_t n, int64_t m, const int32_t *d_src, const int32_t *d_dst,
+                                    const int64_t *d_eid, pgq_csr **out) {
+	return csr_build_device(ctx, n, m, d_src, d_dst, d_eid, nullptr, 0, out);
+}
+
+extern "C" int pgq_csr_build_device_weighted(pgq_ctx *ctx, int64_t n, int64_t m, const int32_t *d_src,
+                                             const int32_t *d_dst, const int64_t *d_eid, const int64_t *d_weight_i64,
+                                             const double *d_weight_f64, pgq_csr **out) {
+	const void *d_w;
+	int weight_type;
+	PGQ_TRY(weight_arg(d_weight_i64, d_weight_f64, &d_w, &weight_type));
+	return csr_build_device(ctx, n, m, d_src, d_dst, d_eid, d_w, weight_type, out);
 }
 
 // ---- CSR from vertex-key and edge-key columns ------------------------------------------------------
@@ -1946,6 +2000,31 @@ __global__ void k_key_expand(const int32_t *__restrict__ off, const int32_t *__r
 	}
 }
 
+// A weighted key build: status[3] = max(m - k) over the edges k that join (ms >= 1) and have a NULL weight, so that
+// m - status[3] is the first of them.  Runs beside k_key_edges, before the status block goes to the host.
+__global__ void k_key_null_weight(const int32_t *__restrict__ ms, const uint8_t *__restrict__ w_valid, int64_t m,
+                                  unsigned long long *status) {
+	for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += (int64_t)gridDim.x * blockDim.x) {
+		if (ms[k] > 0 && !w_valid[k]) {
+			atomicMax(&status[3], (unsigned long long)(m - k));
+		}
+	}
+}
+
+// edge k's weight at the rows k_key_expand gave it, off[k] .. off[k + 1] - 1: the CTE hands k.w to create_csr_edge on
+// every joined row
+__global__ void k_key_expand_weights(const int32_t *__restrict__ off, const int64_t *__restrict__ w, int64_t m,
+                                     int64_t *__restrict__ out_w) {
+	for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += (int64_t)gridDim.x * blockDim.x) {
+		const int64_t p = off[k];
+		const int c = off[k + 1] - off[k];
+		const int64_t x = w[k];
+		for (int j = 0; j < c; j++) {
+			out_w[p + j] = x;
+		}
+	}
+}
+
 // The vertex table's (key, rowid) pairs sorted by key: the nv = (*pos)[n] non-NULL ones first (the scan scratch in
 // WS_KEY_SCAN has room for max(n, m) + 1 elements).
 static int sort_vertex_keys(pgq_csr *csr, Workspace *ws, cudaStream_t s, const int64_t *vkey, const uint8_t *vvalid,
@@ -1977,10 +2056,12 @@ static int sort_vertex_keys(pgq_csr *csr, Workspace *ws, cudaStream_t s, const i
 	return PGQ_OK;
 }
 
-// The key -> rowid join of the CSR CTE on device columns, then the common build.  Sets csr->m.
+// The key -> rowid join of the CSR CTE on device columns, then the common build.  Sets csr->m.  A weighted build
+// (weight_type != 0) gives every row of edge k the weight w[k]; w_valid (nullable) may mark NULL weights only on edges
+// that join nothing.
 static int build_from_keys(pgq_csr *csr, Workspace *ws, cudaStream_t s, const int64_t *vkey, const uint8_t *vvalid,
                            const int64_t *skey, const int64_t *dkey, const uint8_t *svalid, const uint8_t *dvalid,
-                           int64_t m) {
+                           int64_t m, const int64_t *w, const uint8_t *w_valid, int weight_type) {
 	const int64_t n = csr->n;
 	const unsigned grid_m = grid_for(m, 256, (int64_t)csr->ctx->sm_count * 16);
 	int32_t *pos, *scan_tmp, *sorted_row, *ms, *src_lo, *dst_row;
@@ -1991,33 +2072,42 @@ static int build_from_keys(pgq_csr *csr, Workspace *ws, cudaStream_t s, const in
 	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_EDGE_A, eb * sizeof(int32_t), (void **)&ms));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_EDGE_B, eb * sizeof(int32_t), (void **)&src_lo));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_KEY_EDGE_C, eb * sizeof(int32_t), (void **)&dst_row));
-	PGQ_CUDA(cudaMemsetAsync(d_status, 0, 3 * sizeof(unsigned long long), s));
+	PGQ_CUDA(cudaMemsetAsync(d_status, 0, 4 * sizeof(unsigned long long), s));
 	PGQ_TRY(sort_vertex_keys(csr, ws, s, vkey, vvalid, m, &pos, &scan_tmp, &sorted_key, &sorted_row));
 	if (m > 0) {
 		PGQ_CUDA(cudaMemsetAsync(ms + m, 0, sizeof(int32_t), s));
 		k_key_edges<<<grid_m, 256, 0, s>>>(sorted_key, sorted_row, pos + n, skey, dkey, svalid, dvalid, m, ms, src_lo,
 		                                    dst_row, d_status);
 		PGQ_CUDA(cudaGetLastError());
+		if (weight_type && w_valid) {
+			k_key_null_weight<<<grid_m, 256, 0, s>>>(ms, w_valid, m, d_status);
+			PGQ_CUDA(cudaGetLastError());
+		}
 	}
-	unsigned long long st[3] = {0, 0, 0};
+	unsigned long long st[4] = {0, 0, 0, 0};
 	PGQ_CUDA(cudaMemcpyAsync(st, d_status, sizeof(st), cudaMemcpyDeviceToHost, s));
 	PGQ_CUDA(cudaStreamSynchronize(s));
 	if (st[2] || st[0] != st[1]) {
 		return pgq_fail(PGQ_ERR_CONSTRAINT, "%s", pgq_status_text(PGQ_ERR_CONSTRAINT));
+	}
+	if (st[3]) {
+		return pgq_fail(PGQ_ERR_INVALID_ARG, "create_csr_edge: edge row %lld joins but its weight is NULL",
+		                (long long)(m - (int64_t)st[3]));
 	}
 	const int64_t rows = (int64_t)st[0];
 	if (rows >= 0x7fffffffLL) {
 		return pgq_fail(PGQ_ERR_RANGE, "the edge join yields %lld rows: beyond the int32 device CSR", (long long)rows);
 	}
 	csr->m = csr->edge_size = csr->staged = rows;
-	const size_t cap = (size_t)std::max<int64_t>(rows, 1);
-	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_src, cap * sizeof(int32_t)));
-	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_dst, cap * sizeof(int32_t)));
-	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_eid, cap * sizeof(int64_t)));
+	PGQ_TRY(alloc_staging(csr, rows, weight_type));
 	if (rows > 0) {
 		PGQ_TRY(pgq_scan_exclusive_i32(ms, ms, m + 1, scan_tmp, s)); // ms -> first row of every edge, ms[m] = rows
 		k_key_expand<<<grid_m, 256, 0, s>>>(ms, src_lo, dst_row, sorted_row, m, csr->st_src, csr->st_dst, csr->st_eid);
 		PGQ_CUDA(cudaGetLastError());
+		if (weight_type) {
+			k_key_expand_weights<<<grid_m, 256, 0, s>>>(ms, w, m, csr->st_w);
+			PGQ_CUDA(cudaGetLastError());
+		}
 	}
 	return finalize_from_rows(csr, ws, s);
 }
@@ -2369,7 +2459,8 @@ static int build_from_keys_undirected(pgq_csr *csr, Workspace *ws, cudaStream_t 
 // The columns staged on the device when they are on the host, then the directed or the undirected build.
 static int build_from_key_columns(pgq_csr *csr, const int64_t *vkey, const uint8_t *vvalid, int64_t m,
                                   const int64_t *skey, const int64_t *dkey, const uint8_t *svalid,
-                                  const uint8_t *dvalid, bool host, bool undirected) {
+                                  const uint8_t *dvalid, const int64_t *w, const uint8_t *wvalid, int weight_type,
+                                  bool host, bool undirected) {
 	const int64_t n = csr->n;
 	WsGuard g(csr->ctx);
 	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
@@ -2382,6 +2473,8 @@ static int build_from_key_columns(pgq_csr *csr, const int64_t *vkey, const uint8
 		PGQ_TRY(stage_column(ws, WS_KEY_IN_DKEY, dkey, m8, (const void **)&dkey));
 		PGQ_TRY(stage_column(ws, WS_KEY_IN_SVALID, svalid, (size_t)m, (const void **)&svalid));
 		PGQ_TRY(stage_column(ws, WS_KEY_IN_DVALID, dvalid, (size_t)m, (const void **)&dvalid));
+		PGQ_TRY(stage_column(ws, WS_KEY_IN_W, w, m8, (const void **)&w));
+		PGQ_TRY(stage_column(ws, WS_KEY_IN_WVALID, wvalid, (size_t)m, (const void **)&wvalid));
 	} else {
 		// the columns may have been produced on any stream of the caller: wait for the whole device once
 		cudaError_t e = cudaDeviceSynchronize();
@@ -2391,14 +2484,16 @@ static int build_from_key_columns(pgq_csr *csr, const int64_t *vkey, const uint8
 		}
 	}
 	PGQ_TRY(undirected ? build_from_keys_undirected(csr, ws, ws->stream, vkey, vvalid, skey, dkey, svalid, dvalid, m)
-	                   : build_from_keys(csr, ws, ws->stream, vkey, vvalid, skey, dkey, svalid, dvalid, m));
+	                   : build_from_keys(csr, ws, ws->stream, vkey, vvalid, skey, dkey, svalid, dvalid, m, w, wvalid,
+	                                     weight_type));
 	g.settled = true;
 	return PGQ_OK;
 }
 
 static int csr_build_keys(pgq_ctx *ctx, int64_t n, const int64_t *vkey, const uint8_t *vvalid, int64_t m,
                           const int64_t *skey, const int64_t *dkey, const uint8_t *svalid, const uint8_t *dvalid,
-                          bool host, bool undirected, pgq_csr **out) {
+                          const void *w, const uint8_t *wvalid, int weight_type, bool host, bool undirected,
+                          pgq_csr **out) {
 	if (!ctx || !out || (n > 0 && !vkey) || (m > 0 && (!skey || !dkey))) {
 		return pgq_fail(PGQ_ERR_INVALID_ARG, "null argument");
 	}
@@ -2412,7 +2507,8 @@ static int csr_build_keys(pgq_ctx *ctx, int64_t n, const int64_t *vkey, const ui
 	csr->ctx = ctx;
 	csr->n = n;
 	csr->edge_init = true;
-	const int st = build_from_key_columns(csr, vkey, vvalid, m, skey, dkey, svalid, dvalid, host, undirected);
+	const int st = build_from_key_columns(csr, vkey, vvalid, m, skey, dkey, svalid, dvalid, (const int64_t *)w, wvalid,
+	                                      weight_type, host, undirected);
 	if (st != PGQ_OK) {
 		pgq_csr_free(csr);
 		return st;
@@ -2427,7 +2523,7 @@ extern "C" int pgq_csr_build_keys(pgq_ctx *ctx, int64_t n_vertices, const int64_
                                   const int64_t *edge_dst_keys, const uint8_t *edge_src_valid,
                                   const uint8_t *edge_dst_valid, pgq_csr **out) {
 	return csr_build_keys(ctx, n_vertices, vertex_keys, vertex_key_valid, n_edges, edge_src_keys, edge_dst_keys,
-	                      edge_src_valid, edge_dst_valid, true, false, out);
+	                      edge_src_valid, edge_dst_valid, nullptr, nullptr, 0, true, false, out);
 }
 
 extern "C" int pgq_csr_build_keys_device(pgq_ctx *ctx, int64_t n_vertices, const int64_t *d_vertex_keys,
@@ -2436,7 +2532,34 @@ extern "C" int pgq_csr_build_keys_device(pgq_ctx *ctx, int64_t n_vertices, const
                                          const uint8_t *d_edge_src_valid, const uint8_t *d_edge_dst_valid,
                                          pgq_csr **out) {
 	return csr_build_keys(ctx, n_vertices, d_vertex_keys, d_vertex_key_valid, n_edges, d_edge_src_keys,
-	                      d_edge_dst_keys, d_edge_src_valid, d_edge_dst_valid, false, false, out);
+	                      d_edge_dst_keys, d_edge_src_valid, d_edge_dst_valid, nullptr, nullptr, 0, false, false, out);
+}
+
+extern "C" int pgq_csr_build_keys_weighted(pgq_ctx *ctx, int64_t n_vertices, const int64_t *vertex_keys,
+                                           const uint8_t *vertex_key_valid, int64_t n_edges,
+                                           const int64_t *edge_src_keys, const int64_t *edge_dst_keys,
+                                           const uint8_t *edge_src_valid, const uint8_t *edge_dst_valid,
+                                           const int64_t *weight_i64, const double *weight_f64,
+                                           const uint8_t *weight_valid, pgq_csr **out) {
+	const void *w;
+	int weight_type;
+	PGQ_TRY(weight_arg(weight_i64, weight_f64, &w, &weight_type));
+	return csr_build_keys(ctx, n_vertices, vertex_keys, vertex_key_valid, n_edges, edge_src_keys, edge_dst_keys,
+	                      edge_src_valid, edge_dst_valid, w, weight_valid, weight_type, true, false, out);
+}
+
+extern "C" int pgq_csr_build_keys_weighted_device(pgq_ctx *ctx, int64_t n_vertices, const int64_t *d_vertex_keys,
+                                                  const uint8_t *d_vertex_key_valid, int64_t n_edges,
+                                                  const int64_t *d_edge_src_keys, const int64_t *d_edge_dst_keys,
+                                                  const uint8_t *d_edge_src_valid, const uint8_t *d_edge_dst_valid,
+                                                  const int64_t *d_weight_i64, const double *d_weight_f64,
+                                                  const uint8_t *d_weight_valid, pgq_csr **out) {
+	const void *d_w;
+	int weight_type;
+	PGQ_TRY(weight_arg(d_weight_i64, d_weight_f64, &d_w, &weight_type));
+	return csr_build_keys(ctx, n_vertices, d_vertex_keys, d_vertex_key_valid, n_edges, d_edge_src_keys,
+	                      d_edge_dst_keys, d_edge_src_valid, d_edge_dst_valid, d_w, d_weight_valid, weight_type, false,
+	                      false, out);
 }
 
 extern "C" int pgq_csr_build_keys_undirected(pgq_ctx *ctx, int64_t n_vertices, const int64_t *vertex_keys,
@@ -2445,7 +2568,7 @@ extern "C" int pgq_csr_build_keys_undirected(pgq_ctx *ctx, int64_t n_vertices, c
                                              const uint8_t *edge_src_valid, const uint8_t *edge_dst_valid,
                                              pgq_csr **out) {
 	return csr_build_keys(ctx, n_vertices, vertex_keys, vertex_key_valid, n_edges, edge_src_keys, edge_dst_keys,
-	                      edge_src_valid, edge_dst_valid, true, true, out);
+	                      edge_src_valid, edge_dst_valid, nullptr, nullptr, 0, true, true, out);
 }
 
 extern "C" int pgq_csr_build_keys_undirected_device(pgq_ctx *ctx, int64_t n_vertices, const int64_t *d_vertex_keys,
@@ -2454,12 +2577,13 @@ extern "C" int pgq_csr_build_keys_undirected_device(pgq_ctx *ctx, int64_t n_vert
                                                     const uint8_t *d_edge_src_valid, const uint8_t *d_edge_dst_valid,
                                                     pgq_csr **out) {
 	return csr_build_keys(ctx, n_vertices, d_vertex_keys, d_vertex_key_valid, n_edges, d_edge_src_keys,
-	                      d_edge_dst_keys, d_edge_src_valid, d_edge_dst_valid, false, true, out);
+	                      d_edge_dst_keys, d_edge_src_valid, d_edge_dst_valid, nullptr, nullptr, 0, false, true, out);
 }
 
 // The finished CSR of pgq_csr_upload is turned back into edge rows in CSR position order (which IS the arrival order
-// per source) and goes through the same pipeline as a device-side build.
-static int build_from_csr_arrays(pgq_csr *csr, const int64_t *v, const int64_t *e, const int64_t *edge_ids) {
+// per source) and goes through the same pipeline as a device-side build; w (nullable) holds a weight per position.
+static int build_from_csr_arrays(pgq_csr *csr, const int64_t *v, const int64_t *e, const int64_t *edge_ids,
+                                 const void *w, int weight_type) {
 	const int64_t n = csr->n, m = csr->m;
 	WsGuard g(csr->ctx);
 	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
@@ -2467,12 +2591,9 @@ static int build_from_csr_arrays(pgq_csr *csr, const int64_t *v, const int64_t *
 	cudaStream_t s = ws->stream;
 	int *d_err;
 	int32_t *off_tmp;
-	const size_t cap = (size_t)std::max<int64_t>(m, 1);
 	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_ERR, 256, (void **)&d_err));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_CSR_VERTEX_D, (size_t)(n + 2) * sizeof(int32_t), (void **)&off_tmp));
-	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_src, cap * sizeof(int32_t)));
-	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_dst, cap * sizeof(int32_t)));
-	PGQ_TRY(dev_alloc(csr, (void **)&csr->st_eid, cap * sizeof(int64_t)));
+	PGQ_TRY(alloc_staging(csr, m, weight_type));
 	cudaMemsetAsync(d_err, 0, sizeof(int), s);
 	// v[0..n] are the row offsets in the reference layout (v[n+1] == v[n] == m is padding)
 	PGQ_TRY(upload_narrow(ws, v, n + 1, 0, m + 1, off_tmp, d_err, s));
@@ -2492,14 +2613,17 @@ static int build_from_csr_arrays(pgq_csr *csr, const int64_t *v, const int64_t *
 		} else {
 			k_iota64<<<grid_for(m, 256, (int64_t)csr->ctx->sm_count * 8), 256, 0, s>>>(csr->st_eid, m);
 		}
+		if (w) {
+			cudaMemcpyAsync(csr->st_w, w, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, s);
+		}
 	}
 	PGQ_TRY(finalize_from_rows(csr, ws, s));
 	g.settled = true;
 	return PGQ_OK;
 }
 
-extern "C" int pgq_csr_upload(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *v, const int64_t *e,
-                              const int64_t *edge_ids, pgq_csr **out) {
+static int csr_upload(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *v, const int64_t *e, const int64_t *edge_ids,
+                      const void *w, int weight_type, pgq_csr **out) {
 	if (!ctx || !out || !v || (m > 0 && !e)) {
 		return pgq_fail(PGQ_ERR_INVALID_ARG, "null argument");
 	}
@@ -2516,7 +2640,7 @@ extern "C" int pgq_csr_upload(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t 
 	csr->edge_size = m;
 	csr->staged = m;
 	csr->edge_init = true;
-	const int st = build_from_csr_arrays(csr, v, e, edge_ids);
+	const int st = build_from_csr_arrays(csr, v, e, edge_ids, w, weight_type);
 	if (st != PGQ_OK) {
 		pgq_csr_free(csr);
 		return st;
@@ -2524,6 +2648,20 @@ extern "C" int pgq_csr_upload(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t 
 	free_staging(csr);
 	*out = csr;
 	return PGQ_OK;
+}
+
+extern "C" int pgq_csr_upload(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *v, const int64_t *e,
+                              const int64_t *edge_ids, pgq_csr **out) {
+	return csr_upload(ctx, n, m, v, e, edge_ids, nullptr, 0, out);
+}
+
+extern "C" int pgq_csr_upload_weighted(pgq_ctx *ctx, int64_t n, int64_t m, const int64_t *v, const int64_t *e,
+                                       const int64_t *edge_ids, const int64_t *w_i64, const double *w_f64,
+                                       pgq_csr **out) {
+	const void *w;
+	int weight_type;
+	PGQ_TRY(weight_arg(w_i64, w_f64, &w, &weight_type));
+	return csr_upload(ctx, n, m, v, e, edge_ids, w, weight_type, out);
 }
 
 extern "C" int pgq_csr_download(pgq_csr *csr, int64_t *v_out, int64_t *e_out, int64_t *edge_ids_out) {

@@ -180,6 +180,8 @@ enum WsSlot : int {
 	// step weights.
 	WS_CK_ROOT = 139, WS_CK_DIST = 140, WS_CK_DIRTY = 141, WS_CK_FLAGS = 142, WS_CK_LEVEL = 143, WS_CK_VBAN = 144,
 	WS_CK_FRONT = 145, WS_CK_GREW = 146, WS_CK_DONE = 147, WS_CK_STEP_W = 148,
+	// a weighted key build's staged weight column and its validity (with the other WS_KEY_IN_* columns)
+	WS_KEY_IN_W = 149, WS_KEY_IN_WVALID = 150,
 	WS_SLOTS // (the last block holds the highest numbers)
 };
 
@@ -228,7 +230,7 @@ constexpr int ws_keys[] = {WS_KEY_STATUS, WS_KEY_POS, WS_KEY_SCAN, WS_KEY_SORT_A
                            WS_UKEY_SORT_A, WS_UKEY_SORT_B, WS_UKEY_IDX_A, WS_UKEY_IDX_B, WS_UKEY_AUX, WS_UKEY_R_ROW,
                            WS_UKEY_M_ROW, WS_UKEY_DCNT, WS_UKEY_NULL_MULT, WS_UKEY_H_LO, WS_UKEY_H_MULT};
 constexpr int ws_key_staging[] = {WS_KEY_IN_VKEY, WS_KEY_IN_VVALID, WS_KEY_IN_SKEY, WS_KEY_IN_DKEY, WS_KEY_IN_SVALID,
-                                  WS_KEY_IN_DVALID};
+                                  WS_KEY_IN_DVALID, WS_KEY_IN_W, WS_KEY_IN_WVALID};
 template <size_t A, size_t B>
 constexpr bool ws_disjoint(const int (&a)[A], const int (&b)[B]) {
 	for (int x : a) {

@@ -268,7 +268,7 @@ public:
 
 	// The device CSR a path function runs on: the one built from the create_csr_* chunks (finalised on first
 	// use), else -- the CSR was created before this extension was loaded, or its device build failed while the
-	// host arrays exist -- an upload of the host CSR.
+	// host arrays exist -- an upload of the host CSR, with its weights when it has them.
 	pgq_csr *ForPathFunction(int32_t id, CSR &host, int64_t v_size) {
 		if (auto entry = Find(id)) {
 			if (entry->error.empty()) {
@@ -304,7 +304,18 @@ public:
 		}
 		const int64_t *edge_ids = host.edge_ids.size() >= static_cast<idx_t>(m) ? host.edge_ids.data() : nullptr;
 		pgq_csr *device = nullptr;
-		int st = pgq_csr_upload(DeviceContext(), v_size, m, v, host.e.data(), edge_ids, &device);
+		int st;
+		if (host.initialized_w && !(host.w.empty() && host.w_double.empty())) {
+			// the weights of create_csr_edge's 8-argument overloads, told apart as csr_get_w_type does
+			const bool f64 = host.w.empty();
+			if ((f64 ? host.w_double.size() : host.w.size()) < static_cast<idx_t>(m)) {
+				throw InvalidInputException("duckpgq_b200: CSR weights do not cover the edge array");
+			}
+			st = pgq_csr_upload_weighted(DeviceContext(), v_size, m, v, host.e.data(), edge_ids,
+			                             f64 ? nullptr : host.w.data(), f64 ? host.w_double.data() : nullptr, &device);
+		} else {
+			st = pgq_csr_upload(DeviceContext(), v_size, m, v, host.e.data(), edge_ids, &device);
+		}
 		if (st != PGQ_OK) {
 			ThrowStatus(st);
 		}

@@ -206,6 +206,44 @@ int pgq_csr_build_keys_undirected_device(pgq_ctx *ctx, int64_t n_vertices, const
                                          const int64_t *d_edge_src_keys, const int64_t *d_edge_dst_keys,
                                          const uint8_t *d_edge_src_valid, const uint8_t *d_edge_dst_valid,
                                          pgq_csr **out);
+/* The weighted one-shot builds: the same inputs, checks and results as the unweighted entry point each one names, plus
+ * the weight column of the 8-argument create_csr_edge (csr_creation.cpp:141-198,227-235), in the form of
+ * pgq_csr_add_edges_weighted: exactly one of the *_i64 (BIGINT) / *_f64 (DOUBLE) pointers, else PGQ_ERR_INVALID_ARG.
+ * The pointer names the weight type even when there are no edges, so it must be given for n_edges = 0 as well (it is
+ * not read then), and such a CSR reports that type -- unlike a chunked build that never received a row, which stays
+ * at type 0.  The cheapest functions answer on an edgeless weighted CSR as on any weighted graph without the path.
+ *   - positions: the weight of a CSR position is the weight of the input row that became that position.  For the
+ *     rows forms that is the order pgq_csr_build gives (stable by source); pgq_csr_upload_weighted takes one weight
+ *     per CSR position (the reference's CSR::w / CSR::w_double, compressed_sparse_row.hpp:32-40).  In the key forms
+ *     edge k becomes ms(k) rows, one per matching source row, and every one of them carries w[k], as the CTE's join
+ *     hands k.w to create_csr_edge on every joined row;
+ *   - bits: BIGINT and DOUBLE weights are copied as 8-byte patterns (NaN payloads and -0.0 survive);
+ *     pgq_csr_weight_type answers 1 or 2 and pgq_csr_download_weights returns the column in CSR position order;
+ *   - NULL weights (the key forms only; weight_valid nullable = all valid): an edge that joins (gives at least one
+ *     row) with a NULL weight -> PGQ_ERR_INVALID_ARG, the message names its edge row.  An edge that joins nothing may
+ *     have a NULL weight: its row never reaches create_csr_edge.  (The reference skips a NULL-weight row and leaves a
+ *     malformed CSR; DESIGN.md section 7.)  The check runs on the device beside the join's own;
+ *   - there is no weighted form of pgq_csr_build_keys_undirected: the reference's undirected CTE carries no weights,
+ *     and its de-duplication of (p, q) pairs would have to pick one weight out of several. */
+int pgq_csr_build_weighted(pgq_ctx *ctx, int64_t n_vertices, int64_t n_edges, const int64_t *src_rowid,
+                           const int64_t *dst_rowid, const int64_t *edge_rowid, const int64_t *weight_i64,
+                           const double *weight_f64, pgq_csr **out);
+int pgq_csr_build_device_weighted(pgq_ctx *ctx, int64_t n_vertices, int64_t n_edges, const int32_t *d_src_rowid,
+                                  const int32_t *d_dst_rowid, const int64_t *d_edge_rowid,
+                                  const int64_t *d_weight_i64, const double *d_weight_f64, pgq_csr **out);
+int pgq_csr_upload_weighted(pgq_ctx *ctx, int64_t n_vertices, int64_t n_edges, const int64_t *v, const int64_t *e,
+                            const int64_t *edge_ids, const int64_t *w_i64, const double *w_f64, pgq_csr **out);
+int pgq_csr_build_keys_weighted(pgq_ctx *ctx, int64_t n_vertices, const int64_t *vertex_keys,
+                                const uint8_t *vertex_key_valid, int64_t n_edges, const int64_t *edge_src_keys,
+                                const int64_t *edge_dst_keys, const uint8_t *edge_src_valid,
+                                const uint8_t *edge_dst_valid, const int64_t *weight_i64, const double *weight_f64,
+                                const uint8_t *weight_valid, pgq_csr **out);
+int pgq_csr_build_keys_weighted_device(pgq_ctx *ctx, int64_t n_vertices, const int64_t *d_vertex_keys,
+                                       const uint8_t *d_vertex_key_valid, int64_t n_edges,
+                                       const int64_t *d_edge_src_keys, const int64_t *d_edge_dst_keys,
+                                       const uint8_t *d_edge_src_valid, const uint8_t *d_edge_dst_valid,
+                                       const int64_t *d_weight_i64, const double *d_weight_f64,
+                                       const uint8_t *d_weight_valid, pgq_csr **out);
 /* get_csr_v / get_csr_e (src/core/functions/table/pgq_scan.cpp:84-111): copy the CSR back in the
  * reference's layout.  Any output pointer may be NULL. */
 int pgq_csr_download(pgq_csr *csr, int64_t *v_out /* n+2 */, int64_t *e_out /* m */, int64_t *edge_ids_out /* m */);
