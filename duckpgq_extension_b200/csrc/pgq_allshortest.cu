@@ -241,10 +241,6 @@ __global__ void k_as_unrank(int b0, int L, int64_t n, const int32_t *__restrict_
 	}
 }
 
-static inline unsigned as_grid(int64_t want, int64_t cap) {
-	return (unsigned)std::max<int64_t>(1, std::min<int64_t>(want, cap));
-}
-
 // The hook of both functions (see the top)
 struct AllShortest : PathHook {
 	pgq_csr *csr;
@@ -262,7 +258,7 @@ struct AllShortest : PathHook {
 		PGQ_TRY(pgq_ws_reserve(b.ws, WS_AS_SIGMA, (size_t)std::max<int64_t>(n_ab, 1) * b.L * sizeof(int64_t),
 		                       (void **)&sigma));
 		PGQ_CUDA(cudaMemsetAsync(&ctr[AS_K], 0, sizeof(u64), s));
-		const unsigned row_grid = as_grid((b.rows_ub + 255) / 256, (int64_t)sms * 8);
+		const unsigned row_grid = grid_size((b.rows_ub + 255) / 256, (int64_t)sms * 8);
 		k_as_depth<<<row_grid, 256, 0, s>>>(b.b0, b.L, b.batch_rows, b.batch_n, b.row_lane, b.pdst, b.level, ctr);
 		PGQ_CUDA(cudaGetLastError());
 		u64 h_ctr[3] = {0, 0, 0};
@@ -270,7 +266,7 @@ struct AllShortest : PathHook {
 		PGQ_CUDA(cudaStreamSynchronize(s));
 		const int K = (int)h_ctr[AS_K];
 		for (int k = 1; k <= K; k++) {
-			k_sigma_level<<<as_grid((n_ab + 7) / 8, (int64_t)sms * 8), 256, 0, s>>>(k, n_ab, b.L, csr->in.off, csr->in.adj,
+			k_sigma_level<<<grid_size((n_ab + 7) / 8, (int64_t)sms * 8), 256, 0, s>>>(k, n_ab, b.L, csr->in.off, csr->in.adj,
 			                                                                      b.level, sigma);
 		}
 		k_as_rows<<<row_grid, 256, 0, s>>>(b.b0, b.L, b.batch_rows, b.batch_n, b.row_lane, b.psrc, b.pdst, b.level, sigma,
@@ -295,7 +291,7 @@ struct AllShortest : PathHook {
 		PGQ_TRY(pgq_ws_grow(b.ws, WS_WALK, (size_t)total * sizeof(int64_t), (size_t)*b.walk_bound * sizeof(int64_t), s,
 		                    (void **)&walk));
 		*b.walk_bound = (int64_t)total;
-		k_as_unrank<<<as_grid(b.rows_ub, (int64_t)sms * 16), 256, 0, s>>>(
+		k_as_unrank<<<grid_size(b.rows_ub, (int64_t)sms * 16), 256, 0, s>>>(
 		    b.b0, b.L, csr->n, b.batch_rows, b.batch_n, b.row_lane, b.pdst, d_dst, b.level, sigma, csr->in.off, step_key,
 		    step_pos, csr->perm, csr->edge_ids, npaths, plen, b.out_lengths, b.slot_off, walk);
 		PGQ_CUDA(cudaGetLastError());
@@ -320,7 +316,7 @@ int build_step_lists(pgq_csr *csr, Workspace *ws, cudaStream_t s, const u64 **ke
 	if (m == 0) {
 		return PGQ_OK;
 	}
-	k_as_step_keys<<<as_grid((n + 7) / 8, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(
+	k_as_step_keys<<<grid_size((n + 7) / 8, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(
 	    n, csr->out.off, csr->out.adj, csr->inv, reinterpret_cast<u64 *>(ka), pa);
 	PGQ_CUDA(cudaGetLastError());
 	int end_bit = 1;
@@ -411,7 +407,7 @@ static int all_shortest(pgq_csr *csr, int64_t p, const int64_t *src, const int64
 	// (the driver times itself from its own start: the work before it is timed here and added)
 	PGQ_CUDA(cudaEventRecord(ws->ev_begin, s));
 	PGQ_CUDA(cudaMemsetAsync(hook.ctr, 0, 256, s));
-	k_as_init_rows<<<as_grid((p + 255) / 256, 4096), 256, 0, s>>>(p, d_src, d_dst, d_valid, hook.count, hook.npaths,
+	k_as_init_rows<<<grid_size((p + 255) / 256, 4096), 256, 0, s>>>(p, d_src, d_dst, d_valid, hook.count, hook.npaths,
 	                                                            hook.plen);
 	PGQ_CUDA(cudaGetLastError());
 	int64_t pre_launches = 1;

@@ -553,10 +553,6 @@ extern "C" int pgq_cheapest_path(pgq_csr *csr, int64_t p, const int64_t *src, co
 }
 
 // ---- cheapest_path_count / all_cheapest_paths: the walk engine over the tight edges of a batch (see the top) ---------
-// The call's counters: [0] a backward level added a bit (k_ks_reach_update); [1] lanes still counting; [2] a lane still
-// counts after layer KS_WALK_MAX
-enum { AC_CHANGED = 0, AC_ACTIVE = 1, AC_TOO_LONG = 2 };
-
 // The tight edges of a batch as the walk kernels' edge filter (pgq_count.cuh).  The kernels walk the step lists, whose
 // entry e carries the out-CSR position pos[e] of its edge, and so its weight; kernel lane l is lane lane_map[l] of the
 // batch (l itself without a map).  The rule is k_tight_level's: d(from) + w == d(to) in the weight type's arithmetic.
@@ -667,7 +663,7 @@ __global__ void k_ac_start(int cnt, int wd, bool list, const int32_t *__restrict
 		last[row] = c0 ? 0 : -1;
 		if (in_b) {
 			atomicOr(&act[l >> 6], 1ull << (l & 63));
-			atomicAdd(&ctr[AC_ACTIVE], 1ull);
+			atomicAdd(&ctr[KS_ACTIVE], 1ull);
 		}
 	}
 }
@@ -704,230 +700,101 @@ __global__ void k_ac_step(int h, int cnt, int L, int64_t n_ab, bool list, int64_
 		count[row] = infinite ? (int64_t)AS_MAX : (int64_t)tot;
 		const bool stop = !live || tot == AS_MAX || (infinite && (!list || max_paths == 0 || listed + take >= (u64)max_paths));
 		if (h >= KS_WALK_MAX && !stop) {
-			ctr[AC_TOO_LONG] = 1;
+			ctr[KS_TOO_LONG] = 1;
 		}
 		if (stop) {
 			atomicAnd(&act[l >> 6], ~(1ull << (l & 63)));
 		} else {
-			atomicAdd(&ctr[AC_ACTIVE], 1ull);
+			atomicAdd(&ctr[KS_ACTIVE], 1ull);
 		}
 	}
 }
 
-static inline unsigned ac_grid(int64_t want, int64_t cap) {
-	return (unsigned)std::max<int64_t>(1, std::min<int64_t>(want, cap));
-}
-
-static inline u64 ac_sat_add(u64 a, u64 b) { // a, b <= INT64_MAX
-	return a > AS_MAX - b ? AS_MAX : a + b;
-}
-
-// What both calls keep across the batches: the per-row results on the device ([p]) and, for the lists, the walks so far
+// What both calls keep across the batches: the walk engine, the per-row counts on the device ([p]) and the call's choices
 struct AcCall {
+	Walk w;
 	bool list;
 	int64_t max_paths, budget;
-	const u64 *step_key;
-	const int32_t *step_pos, *step_par;
-	int64_t *count, *npaths, *elems_row, *last, *first, *elem_off;
+	int64_t *count;
 	uint8_t *valid;
-	u64 walks, elem_total; // listed so far
 };
 
 // The tight walk search of every batch, behind its sweeps (run_bf's AfterSweeps): the tight backward reach, the counting
 // pass, and for the lists the storing pass and the unranking, whose offsets continue the previous batch's.
 template <bool F64>
 struct TightWalks {
-	pgq_csr *csr;
-	Workspace *ws;
-	const int64_t *d_src, *d_dst;
 	const uint8_t *d_sv, *d_dv;
-	pgq_stats *st;
 	AcCall *call;
 	int operator()(int b0, int cnt, int L, const u64 *dist) const {
+		Walk &w = call->w;
+		pgq_csr *csr = w.csr;
+		Workspace *ws = w.ws;
 		cudaStream_t s = ws->stream;
-		const int64_t n = csr->n, m = csr->m, n_ab = csr->n_ab;
-		const int sms = csr->ctx->sm_count;
+		const int64_t n = csr->n, n_ab = csr->n_ab;
 		const int wd = (L + 63) / 64;
 		const int64_t cells = std::max<int64_t>(n, 1) * wd;
-		const size_t layer = (size_t)std::max<int64_t>(n_ab, 1) * L * sizeof(u64);
-		int32_t *psrc, *pdst, *lane_row;
-		uint32_t *open, *alive, *inf;
-		u64 *reach, *front, *next, *om_a, *om_b, *total, *act, *ctr;
+		int32_t *lane_row;
+		uint32_t *open, *inf;
 		unsigned long long *bsize;
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_PSRC, (size_t)L * sizeof(int32_t), (void **)&psrc));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_PDST, (size_t)L * sizeof(int32_t), (void **)&pdst));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_LANE_ROW, (size_t)L * sizeof(int32_t), (void **)&lane_row));
+		PGQ_TRY(walk_reserve_lanes(w, L, L));
+		PGQ_TRY(pgq_ws_reserve(ws, WS_KS_LANE_ROW, (size_t)L * sizeof(int32_t), (void **)&lane_row));
 		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_OPEN, (size_t)L * sizeof(uint32_t), (void **)&open));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_REACH, (size_t)cells * sizeof(u64), (void **)&reach));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_FRONT, (size_t)cells * sizeof(u64), (void **)&front));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_NEXT, (size_t)cells * sizeof(u64), (void **)&next));
 		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_BSIZE, (size_t)L * sizeof(u64), (void **)&bsize));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_OMEGA_A, layer, (void **)&om_a));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_OMEGA_B, layer, (void **)&om_b));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_TOTAL, (size_t)L * sizeof(u64), (void **)&total));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_ALIVE, (size_t)L * sizeof(uint32_t), (void **)&alive));
 		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_INF, (size_t)L * sizeof(uint32_t), (void **)&inf));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_ACTIVE, (size_t)wd * sizeof(u64), (void **)&act));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_COUNTERS, 256, (void **)&ctr));
-		PGQ_CUDA(cudaMemsetAsync(reach, 0, (size_t)cells * sizeof(u64), s));
-		PGQ_CUDA(cudaMemsetAsync(front, 0, (size_t)cells * sizeof(u64), s));
-		PGQ_CUDA(cudaMemsetAsync(next, 0, (size_t)cells * sizeof(u64), s));
+		w.lane_row = lane_row;
+		PGQ_CUDA(cudaMemsetAsync(w.reach, 0, (size_t)cells * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(w.front, 0, (size_t)cells * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(w.next, 0, (size_t)cells * sizeof(u64), s));
 		PGQ_CUDA(cudaMemsetAsync(bsize, 0, (size_t)L * sizeof(u64), s));
-		PGQ_CUDA(cudaMemsetAsync(alive, 0, (size_t)L * sizeof(uint32_t), s));
-		PGQ_CUDA(cudaMemsetAsync(act, 0, (size_t)wd * sizeof(u64), s));
-		const TightEdges<F64> tight {dist, L, csr->w_bits, call->step_pos, nullptr};
-		k_ac_lanes<F64><<<(cnt + 127) / 128, 128, 0, s>>>(b0, cnt, L, wd, d_src, d_dst, d_sv, d_dv, csr->perm, n, dist, psrc,
-		                                                 pdst, lane_row, open, reach, front);
+		PGQ_CUDA(cudaMemsetAsync(w.alive, 0, (size_t)L * sizeof(uint32_t), s));
+		PGQ_CUDA(cudaMemsetAsync(w.act, 0, (size_t)wd * sizeof(u64), s));
+		const TightEdges<F64> tight {dist, L, csr->w_bits, w.step_pos, nullptr};
+		k_ac_lanes<F64><<<(cnt + 127) / 128, 128, 0, s>>>(b0, cnt, L, wd, w.src, w.dst, d_sv, d_dv, csr->perm, n, dist, w.psrc,
+		                                                 w.pdst, lane_row, open, w.reach, w.front);
 		PGQ_CUDA(cudaGetLastError());
-		st->kernel_launches++;
-		// ---- the tight backward reach ----
-		u64 h_ctr[3];
-		const unsigned edge_grid = ac_grid((m + 255) / 256, (int64_t)sms * 16);
-		for (;;) {
-			PGQ_CUDA(cudaMemsetAsync(&ctr[AC_CHANGED], 0, sizeof(u64), s));
-			if (m > 0) {
-				k_ks_reach_level<<<edge_grid, 256, 0, s>>>(m, n_ab, wd, csr->in.off, call->step_par, front, reach, next, tight);
-				st->kernel_launches++;
-			}
-			k_ks_reach_update<<<ac_grid((cells + 255) / 256, (int64_t)sms * 8), 256, 0, s>>>(cells, reach, front, next, ctr);
-			PGQ_CUDA(cudaGetLastError());
-			st->kernel_launches++;
-			st->push_levels++;
-			PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(u64), cudaMemcpyDeviceToHost, s));
-			PGQ_CUDA(cudaStreamSynchronize(s));
-			if (!h_ctr[AC_CHANGED]) {
-				break;
-			}
-		}
-		k_ac_bsize<<<ac_grid(n, (int64_t)sms * 8), L, 0, s>>>(n, wd, reach, bsize);
-		PGQ_CUDA(cudaMemsetAsync(ctr, 0, 3 * sizeof(u64), s));
-		k_ac_start<<<(cnt + 255) / 256, 256, 0, s>>>(cnt, wd, call->list, lane_row, psrc, pdst, open, reach, total, inf, act,
-		                                             call->count, call->npaths, call->elems_row, call->last, ctr);
-		PGQ_CUDA(cudaGetLastError());
-		st->kernel_launches += 2;
-		PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, s));
-		PGQ_CUDA(cudaStreamSynchronize(s));
-		// ---- the counting pass ----
-		const unsigned chunk_grid = ac_grid((m + KS_CHUNK * 8 - 1) / (KS_CHUNK * 8), (int64_t)sms * 16);
-		u64 *prev = om_a, *cur = om_b;
-		for (int h = 1; h_ctr[AC_ACTIVE] > 0; h++) {
-			PGQ_CUDA(cudaMemsetAsync(cur, 0, layer, s));
-			PGQ_CUDA(cudaMemsetAsync(&ctr[AC_ACTIVE], 0, sizeof(u64), s));
-			if (m > 0) {
-				k_ks_omega<<<chunk_grid, 256, 0, s>>>(h, m, n_ab, L, cnt, csr->in.off, call->step_par, psrc, prev, cur, reach,
-				                                      act, wd, alive, tight);
-				st->kernel_launches++;
-			}
-			k_ac_step<<<(cnt + 255) / 256, 256, 0, s>>>(h, cnt, L, n_ab, call->list, call->max_paths, lane_row, pdst, cur,
-			                                            bsize, alive, total, inf, act, call->count, call->npaths,
-			                                            call->elems_row, call->last, ctr);
-			PGQ_CUDA(cudaGetLastError());
-			st->kernel_launches++;
-			st->pull_levels++;
-			PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, s));
-			PGQ_CUDA(cudaStreamSynchronize(s));
-			if (h_ctr[AC_TOO_LONG]) {
-				return pgq_fail(PGQ_ERR_UNSUPPORTED, "a row still counts cheapest paths after %d edges", KS_WALK_MAX);
-			}
-			std::swap(prev, cur);
-		}
+		w.st->kernel_launches++;
+		PGQ_TRY(walk_reach(w, wd, cells, tight));
+		k_ac_bsize<<<grid_size(n, (int64_t)csr->ctx->sm_count * 8), L, 0, s>>>(n, wd, w.reach, bsize);
+		w.st->kernel_launches++;
+		auto start = [&]() {
+			k_ac_start<<<(cnt + 255) / 256, 256, 0, s>>>(cnt, wd, call->list, lane_row, w.psrc, w.pdst, open, w.reach, w.total,
+			                                             inf, w.act, call->count, w.npaths, w.elems_row, w.last, w.ctr);
+		};
+		auto step = [&](int h, const u64 *cur) {
+			k_ac_step<<<(cnt + 255) / 256, 256, 0, s>>>(h, cnt, L, n_ab, call->list, call->max_paths, lane_row, w.pdst, cur,
+			                                            bsize, w.alive, w.total, inf, w.act, call->count, w.npaths,
+			                                            w.elems_row, w.last, w.ctr);
+		};
+		PGQ_TRY(walk_count(w, L, cnt, wd, w.psrc, tight, start, step, &w.st->pull_levels,
+		                   "a row still counts cheapest paths after"));
 		if (!call->list) {
 			return PGQ_OK;
 		}
 		// ---- the batch's walks and elements: checked, then placed behind the previous batches' ----
 		std::vector<int64_t> h_count((size_t)cnt), h_np((size_t)cnt), h_el((size_t)cnt), h_last((size_t)cnt);
 		PGQ_CUDA(cudaMemcpyAsync(h_count.data(), call->count + b0, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-		PGQ_CUDA(cudaMemcpyAsync(h_np.data(), call->npaths + b0, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-		PGQ_CUDA(cudaMemcpyAsync(h_el.data(), call->elems_row + b0, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-		PGQ_CUDA(cudaMemcpyAsync(h_last.data(), call->last + b0, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaMemcpyAsync(h_np.data(), w.npaths + b0, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaMemcpyAsync(h_el.data(), w.elems_row + b0, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaMemcpyAsync(h_last.data(), w.last + b0, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
 		PGQ_CUDA(cudaStreamSynchronize(s));
-		st->d2h_bytes += 4 * cnt * (int64_t)sizeof(int64_t);
-		u64 walks = call->walks, elem_total = call->elem_total;
+		w.st->d2h_bytes += 4 * cnt * (int64_t)sizeof(int64_t);
 		for (int l = 0; l < cnt; l++) {
 			if (call->max_paths == 0 && (u64)h_count[(size_t)l] == AS_MAX) {
 				return pgq_fail(PGQ_ERR_UNSUPPORTED, "row %lld has INT64_MAX or infinitely many cheapest paths: list them with "
 				                "max_paths > 0", (long long)(b0 + l));
 			}
-			walks = ac_sat_add(walks, (u64)h_np[(size_t)l]);
-			elem_total = ac_sat_add(elem_total, (u64)h_el[(size_t)l]);
 		}
-		if (elem_total > (AS_MAX / sizeof(int64_t)) || walks > (AS_MAX / sizeof(int64_t)) - 1) {
-			return pgq_fail(PGQ_ERR_OOM, "the cheapest paths of one call hold too many elements (%llu)",
-			                (unsigned long long)elem_total);
-		}
-		int64_t *d_scan, *walk_off, *d_elems;
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_SCAN_TOTAL, sizeof(int64_t), (void **)&d_scan));
-		pgq_path_offsets((int64_t)call->elem_total, b0, (int64_t)b0 + cnt, call->elem_off, call->elems_row, call->valid,
-		                 d_scan, s);
-		pgq_path_offsets((int64_t)call->walks, b0, (int64_t)b0 + cnt, call->first, call->npaths, call->valid, d_scan, s);
-		PGQ_CUDA(cudaGetLastError());
-		st->kernel_launches += 2;
-		PGQ_TRY(pgq_ws_grow(ws, WS_AC_WALK_OFF, (size_t)(walks + 1) * sizeof(int64_t), (size_t)call->walks * sizeof(int64_t),
-		                    s, (void **)&walk_off));
-		PGQ_TRY(pgq_ws_grow(ws, WS_AC_ELEMS, (size_t)elem_total * sizeof(int64_t),
-		                    (size_t)call->elem_total * sizeof(int64_t), s, (void **)&d_elems));
-		call->walks = walks;
-		call->elem_total = elem_total;
-		// ---- the storing pass and the unranking, group by group (ks_run's grouping under the layer budget) ----
-		int32_t *glane, *gsrc;
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_GROUP_LANE, (size_t)L * sizeof(int32_t), (void **)&glane));
-		PGQ_TRY(pgq_ws_reserve(ws, WS_AC_GROUP_SRC, (size_t)L * sizeof(int32_t), (void **)&gsrc));
-		std::vector<int32_t> grp;
-		int64_t grp_h = 0;
-		auto layer_bytes = [&](int64_t h, int64_t rows) { return (double)(h + 1) * (double)n_ab * (double)rows * 8.0; };
-		auto run_group = [&]() -> int {
-			const int ng = (int)grp.size();
-			if (ng == 0) {
-				return PGQ_OK;
-			}
-			u64 *layers;
-			PGQ_TRY(pgq_ws_reserve(ws, WS_AC_LAYERS, (size_t)std::max<int64_t>(grp_h, 1) * n_ab * ng * sizeof(u64),
-			                       (void **)&layers));
-			PGQ_CUDA(cudaMemcpyAsync(glane, grp.data(), (size_t)ng * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-			k_ks_group_src<<<ac_grid((ng + 255) / 256, 64), 256, 0, s>>>(ng, glane, psrc, gsrc);
-			PGQ_CUDA(cudaGetLastError());
-			st->kernel_launches++;
-			st->h2d_bytes += ng * (int64_t)sizeof(int32_t);
-			if (grp_h > 0) {
-				PGQ_CUDA(cudaMemsetAsync(layers, 0, (size_t)grp_h * n_ab * ng * sizeof(u64), s));
-			}
-			const TightEdges<F64> gtight {dist, L, csr->w_bits, call->step_pos, glane};
-			for (int64_t h = 1; h <= grp_h && m > 0; h++) {
-				u64 *lcur = layers + (h - 1) * n_ab * ng;
-				const u64 *lprev = h >= 2 ? layers + (h - 2) * n_ab * ng : nullptr;
-				k_ks_omega<<<chunk_grid, 256, 0, s>>>((int)h, m, n_ab, ng, ng, csr->in.off, call->step_par, gsrc, lprev, lcur,
-				                                      nullptr, nullptr, 0, nullptr, gtight);
-				st->kernel_launches++;
-			}
-			k_ks_unrank<<<ac_grid(ng, (int64_t)sms * 16), 256, 0, s>>>(
-			    ng, ng, n, n_ab, glane, lane_row, psrc, pdst, d_src, d_dst, layers, csr->in.off, call->step_key,
-			    call->step_pos, csr->perm, csr->edge_ids, call->npaths, call->last, call->first, call->elem_off, walk_off,
-			    d_elems, gtight);
-			PGQ_CUDA(cudaGetLastError());
-			st->kernel_launches++;
-			// (the next group reuses the group buffers)
-			PGQ_CUDA(cudaStreamSynchronize(s));
-			grp.clear();
-			grp_h = 0;
-			return PGQ_OK;
-		};
+		PGQ_TRY(walk_offsets(w, b0, (int64_t)b0 + cnt, h_np.data(), h_el.data(), call->valid));
+		// ---- the storing pass and the unranking, group by group over the batch's lanes ----
+		std::vector<WalkLane> listed;
 		for (int l = 0; l < cnt; l++) {
-			if (h_np[(size_t)l] == 0) {
-				continue;
+			if (h_np[(size_t)l] > 0) {
+				listed.push_back({l, (int64_t)b0 + l, h_last[(size_t)l]});
 			}
-			const int64_t h = h_last[(size_t)l];
-			if (layer_bytes(h, 1) > (double)call->budget) {
-				return pgq_fail(PGQ_ERR_UNSUPPORTED, "the cheapest paths of row %lld need %.0f bytes of count layers, over the "
-				                "budget of %lld", (long long)(b0 + l), layer_bytes(h, 1), (long long)call->budget);
-			}
-			const int64_t gh = std::max(grp_h, h);
-			if (!grp.empty() && layer_bytes(gh, (int64_t)grp.size() + 1) > (double)call->budget) {
-				PGQ_TRY(run_group());
-			}
-			grp.push_back(l);
-			grp_h = std::max(grp_h, h);
 		}
-		return run_group();
+		return walk_store(w, listed, L, call->budget, [&](const int32_t *glane) {
+			return TightEdges<F64> {dist, L, csr->w_bits, w.step_pos, glane};
+		});
 	}
 };
 
@@ -940,22 +807,14 @@ static int ac_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 	memset(&st, 0, sizeof(st));
 	if (p == 0) {
 		if (list) {
-			*out_path_offsets = (int64_t *)calloc(1, sizeof(int64_t));
-			*out_elems = (int64_t *)malloc(sizeof(int64_t));
-			if (!*out_path_offsets || !*out_elems) {
-				free(*out_path_offsets);
-				free(*out_elems);
-				*out_path_offsets = *out_elems = nullptr;
-				return pgq_fail(PGQ_ERR_OOM, "host allocation failed");
-			}
+			PGQ_TRY(empty_lists(out_path_offsets, out_elems));
 		}
 		if (stats) {
 			*stats = st;
 		}
 		return PGQ_OK;
 	}
-	AcCall call;
-	memset(&call, 0, sizeof(call));
+	AcCall call = {};
 	call.list = list;
 	call.max_paths = max_paths;
 	PGQ_TRY(layer_budget(&call.budget));
@@ -965,96 +824,57 @@ static int ac_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
 	const int64_t n = csr->n, n_ab = csr->n_ab;
-	int64_t *d_src, *d_dst, *d_cost;
+	Walk &w = call.w;
+	w.csr = csr;
+	w.ws = ws;
+	w.st = &st;
+	w.what = "cheapest paths";
+	int64_t *d_cost;
 	uint8_t *d_sv, *d_dv, *d_cv;
 	const size_t b8 = (size_t)p * sizeof(int64_t);
 	PGQ_CUDA(cudaEventRecord(ws->ev_begin, s));
-	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
-	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d_dst));
+	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&w.src));
+	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&w.dst));
 	PGQ_TRY(stage_column(ws, WS_IN_VALID, src_valid, (size_t)p, (const void **)&d_sv));
 	PGQ_TRY(stage_column(ws, WS_IN_DST_VALID, dst_valid, (size_t)p, (const void **)&d_dv));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_LEN, b8, (void **)&d_cost)); // the sweeps' costs
 	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_cv));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_PATH_VALID, (size_t)p, (void **)&call.valid));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_COUNT, b8, (void **)&call.count));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_NPATHS, b8, (void **)&call.npaths));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_ROW_ELEMS, b8, (void **)&call.elems_row));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_LAST, b8, (void **)&call.last));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_FIRST, b8, (void **)&call.first));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_ELEM_OFF, b8, (void **)&call.elem_off));
+	PGQ_TRY(walk_reserve_rows(w, p));
 	st.h2d_bytes = 2 * (int64_t)b8 + (src_valid ? p : 0) + (dst_valid ? p : 0);
 	// the step lists, and each entry's parent: the tight kernels' in-lists
 	int32_t *step_par;
-	PGQ_TRY(build_step_lists(csr, ws, s, &call.step_key, &call.step_pos, &st.kernel_launches));
+	PGQ_TRY(build_step_lists(csr, ws, s, &w.step_key, &w.step_pos, &st.kernel_launches));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_AC_STEP_PAR, (size_t)std::max<int64_t>(csr->m, 1) * sizeof(int32_t), (void **)&step_par));
 	if (csr->m > 0) {
-		k_ac_step_par<<<ac_grid((n_ab + 7) / 8, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(n, n_ab, csr->in.off,
-		                                                                                     call.step_key, csr->perm,
-		                                                                                     step_par);
+		k_ac_step_par<<<grid_size((n_ab + 7) / 8, (int64_t)csr->ctx->sm_count * 16), 256, 0, s>>>(n, n_ab, csr->in.off,
+		                                                                                       w.step_key, csr->perm,
+		                                                                                       step_par);
 		PGQ_CUDA(cudaGetLastError());
 		st.kernel_launches++;
 	}
-	call.step_par = step_par;
+	w.in_list = step_par;
 	if (csr->weight_type == 2) {
-		const TightWalks<true> walks {csr, ws, d_src, d_dst, d_sv, d_dv, &st, &call};
-		PGQ_TRY(run_bf<true>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_cost, d_cv, &st, walks));
+		PGQ_TRY(run_bf<true>(csr, ws, p, w.src, w.dst, d_sv, d_dv, d_cost, d_cv, &st, TightWalks<true> {d_sv, d_dv, &call}));
 	} else {
-		const TightWalks<false> walks {csr, ws, d_src, d_dst, d_sv, d_dv, &st, &call};
-		PGQ_TRY(run_bf<false>(csr, ws, p, d_src, d_dst, d_sv, d_dv, d_cost, d_cv, &st, walks));
+		PGQ_TRY(run_bf<false>(csr, ws, p, w.src, w.dst, d_sv, d_dv, d_cost, d_cv, &st, TightWalks<false> {d_sv, d_dv, &call}));
 	}
-	cudaError_t e = cudaMemcpyAsync(out_count, call.count, b8, cudaMemcpyDeviceToHost, s);
-	st.d2h_bytes += (int64_t)b8 + p;
+	PGQ_CUDA(cudaMemcpyAsync(out_count, call.count, b8, cudaMemcpyDeviceToHost, s));
 	if (!list) {
-		if (e == cudaSuccess) e = cudaEventRecord(ws->ev_end, s);
-		if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-		float ms = 0.f;
-		if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end);
-		g.settled = (e == cudaSuccess);
-		if (e != cudaSuccess) {
-			cudaGetLastError();
-			return pgq_fail(PGQ_ERR_CUDA, "copying the cheapest path counts back failed: %s", cudaGetErrorString(e));
-		}
+		PGQ_TRY(walk_end(g, &st, "cheapest path counts"));
 		for (int64_t i = 0; i < p; i++) {
 			out_valid[i] = out_count[i] > 0;
 		}
-		st.total_ms = ms;
+		st.d2h_bytes += (int64_t)b8 + p;
 		if (stats) {
 			*stats = st;
 		}
 		return PGQ_OK;
 	}
-	const u64 walks = call.walks, elem_total = call.elem_total;
-	int64_t *h_off = (int64_t *)malloc((size_t)(walks + 1) * sizeof(int64_t));
-	int64_t *h_elems = (int64_t *)malloc((size_t)std::max<u64>(elem_total, 1) * sizeof(int64_t));
-	if (!h_off || !h_elems) {
-		free(h_off);
-		free(h_elems);
-		return pgq_fail(PGQ_ERR_OOM, "host allocation of %llu path elements failed", (unsigned long long)elem_total);
-	}
-	if (e == cudaSuccess && walks > 0)
-		e = cudaMemcpyAsync(h_off, ws->buf[WS_AC_WALK_OFF], (size_t)walks * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
-	if (e == cudaSuccess && elem_total > 0)
-		e = cudaMemcpyAsync(h_elems, ws->buf[WS_AC_ELEMS], (size_t)elem_total * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(out_npaths, call.npaths, b8, cudaMemcpyDeviceToHost, s);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(out_first_path, call.first, b8, cudaMemcpyDeviceToHost, s);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(out_valid, call.valid, (size_t)p, cudaMemcpyDeviceToHost, s);
-	if (e == cudaSuccess) e = cudaEventRecord(ws->ev_end, s);
-	if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-	float ms = 0.f;
-	if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end);
-	g.settled = (e == cudaSuccess);
-	if (e != cudaSuccess) {
-		cudaGetLastError();
-		free(h_off);
-		free(h_elems);
-		return pgq_fail(PGQ_ERR_CUDA, "copying the cheapest paths back failed: %s", cudaGetErrorString(e));
-	}
-	h_off[walks] = (int64_t)elem_total;
-	st.total_ms = ms;
-	st.d2h_bytes += 2 * (int64_t)b8 + (int64_t)(walks + elem_total) * (int64_t)sizeof(int64_t);
-	*out_path_offsets = h_off;
-	*out_elems = h_elems;
-	*out_total_paths = (int64_t)walks;
+	PGQ_CUDA(cudaMemcpyAsync(out_npaths, w.npaths, b8, cudaMemcpyDeviceToHost, s));
+	st.d2h_bytes += 3 * (int64_t)b8; // the counts, walks and first walks (walk_lists counts the rest)
+	PGQ_TRY(walk_lists(w, g, p, call.valid, out_first_path, out_valid, out_path_offsets, out_elems, out_total_paths));
 	if (stats) {
 		*stats = st;
 	}

@@ -377,7 +377,7 @@ struct CkSearch : KmSearch {
 	             uint8_t *has, pgq_stats *st) override {
 		PGQ_TRY(stage_column(ws, WS_CK_ROOT, roots.data(), roots.size() * sizeof(int64_t), (const void **)&root));
 		st->h2d_bytes += (int64_t)(roots.size() * sizeof(int64_t));
-		k_ck_has_seed<F64><<<km_grid((ns + 7) / 8, (int64_t)csr->ctx->sm_count * 16), 256, 0, ws->stream>>>(
+		k_ck_has_seed<F64><<<grid_size((ns + 7) / 8, (int64_t)csr->ctx->sm_count * 16), 256, 0, ws->stream>>>(
 		    ns, spurs, lists, root, csr->out.off, csr->out.adj, csr->w_bits, has);
 		PGQ_CUDA(cudaGetLastError());
 		st->kernel_launches++;
@@ -390,8 +390,8 @@ struct CkSearch : KmSearch {
 		const int W = b.W, wd = (W + 63) / 64, cnt = b.cnt;
 		const size_t cells = (size_t)std::max<int64_t>(n, 1) * W;
 		const size_t words = (size_t)n / 32 + 1;
-		const unsigned vert_grid = km_grid((n + 7) / 8, (int64_t)sms * 8);
-		k_bf_init<F64><<<km_grid(((int64_t)cells + 255) / 256, (int64_t)sms * 16), 256, 0, s>>>((int64_t)cells, dist);
+		const unsigned vert_grid = grid_size((n + 7) / 8, (int64_t)sms * 8);
+		k_bf_init<F64><<<grid_size(((int64_t)cells + 255) / 256, (int64_t)sms * 16), 256, 0, s>>>((int64_t)cells, dist);
 		PGQ_CUDA(cudaMemsetAsync(vban, 0, (size_t)n * wd * sizeof(u64), s));
 		PGQ_CUDA(cudaMemsetAsync(dirty, 0, words * sizeof(uint32_t), s));
 		PGQ_CUDA(cudaMemsetAsync(level, 0xff, cells * sizeof(uint16_t), s));

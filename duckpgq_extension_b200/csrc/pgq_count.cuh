@@ -1,6 +1,7 @@
 // pgq_count.cuh -- what the path-counting files share (pgq_allshortest.cu, pgq_kshortest.cu, pgq_cheapest.cu):
-// saturating counts, the step-ordered in-lists, and the walk engine's backward reach, layered walk counts and unranking
-// (pgq_kshortest.cu's top describes them), which all_cheapest_paths runs over the tight edges of each lane.
+// saturating counts, the step-ordered in-lists, and the walk engine (pgq_kshortest.cu's top describes it): its backward
+// reach, layered walk counts and unranking kernels, and the host driver that runs them, for shortest_k_paths over every
+// edge and for all_cheapest_paths over the tight edges of each lane.
 #pragma once
 
 #include "pgq_internal.h"
@@ -43,6 +44,10 @@ int kg_walk(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, con
             int64_t *out_total_paths, pgq_stats *stats);
 
 #define KS_WALK_MAX 65533   // the longest walk a result may hold (all_shortest_paths' depth limit)
+
+// The walk kernels' counters: [0] a backward level added a bit; [1] lanes still counting; [2] a lane needs a walk longer
+// than KS_WALK_MAX
+enum { KS_CHANGED = 0, KS_ACTIVE = 1, KS_TOO_LONG = 2 };
 
 // pgq_kshortest.cu's fold of a backward level (the new bits become the frontier and join the reach; ctr[0] = 1 when
 // a bit was new) and the sources of a storing group's lanes (gsrc[j] = psrc[glane[j]])
@@ -283,3 +288,188 @@ __global__ void __launch_bounds__(256) k_ks_unrank(int ng, int Lg, int64_t n, in
 	}
 }
 
+// ---- the walk engine's host driver ----------------------------------------------------------------------------------
+// A call's walk engine: its CSR, workspace and stats, the in-lists its kernels walk (csr->in.adj, or the step lists'
+// parents), its staged columns and step lists, and its device buffers in the WS_KS_* slots (pgq_internal.h); walks and
+// elem_total count the walks placed so far and their elements.  `what` names the walks in the call's messages.
+struct Walk {
+	pgq_csr *csr;
+	Workspace *ws;
+	pgq_stats *st;
+	const char *what;
+	const int32_t *in_list;
+	const int64_t *src, *dst;
+	const u64 *step_key;
+	const int32_t *step_pos;
+	const int32_t *lane_row;
+	int32_t *psrc, *pdst, *glane, *gsrc;
+	u64 *reach, *front, *next, *om_a, *om_b, *total, *act, *ctr;
+	uint32_t *alive;
+	int64_t *npaths, *elems_row, *last, *first, *elem_off, *walk_off, *elems;
+	u64 walks, elem_total;
+};
+
+// reserve the engine's buffers: its per-row arrays for p rows; its per-lane buffers for `lanes` lane ids in batches W
+// lanes wide (lane_row is the caller's)
+int walk_reserve_rows(Walk &w, int64_t p);
+int walk_reserve_lanes(Walk &w, int64_t lanes, int W);
+
+// The backward reach of a batch, from the targets its caller seeded into reach and front: levels over the in-lists, each
+// passing a lane's bits along the edges `keep` admits for it, until a level adds no bit.  cells = n x wd mask words.
+template <class EdgeFilter>
+int walk_reach(Walk &w, int wd, int64_t cells, const EdgeFilter &keep) {
+	pgq_csr *csr = w.csr;
+	cudaStream_t s = w.ws->stream;
+	const int64_t m = csr->m;
+	const int sms = csr->ctx->sm_count;
+	u64 changed;
+	for (;;) {
+		PGQ_CUDA(cudaMemsetAsync(&w.ctr[KS_CHANGED], 0, sizeof(u64), s));
+		if (m > 0) {
+			k_ks_reach_level<<<grid_size((m + 255) / 256, (int64_t)sms * 16), 256, 0, s>>>(m, csr->n_ab, wd, csr->in.off,
+			                                                                               w.in_list, w.front, w.reach,
+			                                                                               w.next, keep);
+			w.st->kernel_launches++;
+		}
+		k_ks_reach_update<<<grid_size((cells + 255) / 256, (int64_t)sms * 8), 256, 0, s>>>(cells, w.reach, w.front, w.next,
+		                                                                                   w.ctr);
+		PGQ_CUDA(cudaGetLastError());
+		w.st->kernel_launches++;
+		w.st->push_levels++;
+		PGQ_CUDA(cudaMemcpyAsync(&changed, &w.ctr[KS_CHANGED], sizeof(u64), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaStreamSynchronize(s));
+		if (!changed) {
+			return PGQ_OK;
+		}
+	}
+}
+
+// The counting pass of a batch of cnt lanes in layers L wide (psrc: the batch's sources): start() launches the caller's
+// layer-0 kernel, which flags the lanes that count; then, while a lane counts, layer h = 1, 2, ... sums the edges `admit`
+// admits (k_ks_omega) and step(h, cur) launches the caller's step kernel on it.  *layers counts the layers; a lane past
+// KS_WALK_MAX fails the call with too_long.
+template <class EdgeFilter, class Start, class Step>
+int walk_count(Walk &w, int L, int cnt, int wd, const int32_t *psrc, const EdgeFilter &admit, const Start &start,
+               const Step &step, int64_t *layers, const char *too_long) {
+	pgq_csr *csr = w.csr;
+	cudaStream_t s = w.ws->stream;
+	const int64_t m = csr->m, n_ab = csr->n_ab;
+	const size_t layer = (size_t)std::max<int64_t>(n_ab, 1) * L * sizeof(u64);
+	const unsigned chunk_grid = grid_size((m + KS_CHUNK * 8 - 1) / (KS_CHUNK * 8), (int64_t)csr->ctx->sm_count * 16);
+	u64 h_ctr[3];
+	PGQ_CUDA(cudaMemsetAsync(w.ctr, 0, sizeof(h_ctr), s));
+	start();
+	PGQ_CUDA(cudaGetLastError());
+	w.st->kernel_launches++;
+	PGQ_CUDA(cudaMemcpyAsync(h_ctr, w.ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, s));
+	PGQ_CUDA(cudaStreamSynchronize(s));
+	u64 *prev = w.om_a, *cur = w.om_b;
+	for (int h = 1; h_ctr[KS_ACTIVE] > 0; h++) {
+		PGQ_CUDA(cudaMemsetAsync(cur, 0, layer, s));
+		PGQ_CUDA(cudaMemsetAsync(&w.ctr[KS_ACTIVE], 0, sizeof(u64), s));
+		if (m > 0) {
+			k_ks_omega<<<chunk_grid, 256, 0, s>>>(h, m, n_ab, L, cnt, csr->in.off, w.in_list, psrc, prev, cur, w.reach,
+			                                      w.act, wd, w.alive, admit);
+			w.st->kernel_launches++;
+		}
+		step(h, cur);
+		PGQ_CUDA(cudaGetLastError());
+		w.st->kernel_launches++;
+		(*layers)++;
+		PGQ_CUDA(cudaMemcpyAsync(h_ctr, w.ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, s));
+		PGQ_CUDA(cudaStreamSynchronize(s));
+		if (h_ctr[KS_TOO_LONG]) {
+			return pgq_fail(PGQ_ERR_UNSUPPORTED, "%s %d edges", too_long, KS_WALK_MAX);
+		}
+		std::swap(prev, cur);
+	}
+	return PGQ_OK;
+}
+
+// Places the walks of rows [lo, hi) behind the walks placed so far: checks that the call's walks and their elements stay
+// addressable (h_np, h_el: host copies of the rows' walk and element counts), scans the rows' first element and first
+// walk from the running totals (valid = the row has a walk), and grows the offset and element buffers to hold them.
+int walk_offsets(Walk &w, int64_t lo, int64_t hi, const int64_t *h_np, const int64_t *h_el, uint8_t *valid);
+
+// A lane whose row has walks, the longest of them `last` edges long
+struct WalkLane {
+	int32_t lane;
+	int64_t row, last;
+};
+
+// The storing pass and the unranking of `lanes`: packed greedily in order into groups of at most cap lanes whose layers,
+// (H + 1) x n_ab x lanes x 8 B with H the group's longest walk, fit the budget; each group recomputes its layers, every
+// one kept, and unranks its walks into the offsets walk_offsets placed.  filter_for(glane) is the edge filter of a group
+// whose lane j is lane glane[j] of the engine.
+template <class FilterFor>
+int walk_store(Walk &w, const std::vector<WalkLane> &lanes, int cap, int64_t budget, const FilterFor &filter_for) {
+	pgq_csr *csr = w.csr;
+	cudaStream_t s = w.ws->stream;
+	const int64_t n = csr->n, m = csr->m, n_ab = csr->n_ab;
+	const int sms = csr->ctx->sm_count;
+	const unsigned chunk_grid = grid_size((m + KS_CHUNK * 8 - 1) / (KS_CHUNK * 8), (int64_t)sms * 16);
+	std::vector<int32_t> grp;
+	int64_t grp_h = 0;
+	auto layer_bytes = [&](int64_t h, int64_t rows) { return (double)(h + 1) * (double)n_ab * (double)rows * 8.0; };
+	auto run_group = [&]() -> int {
+		const int ng = (int)grp.size();
+		if (ng == 0) {
+			return PGQ_OK;
+		}
+		u64 *layers;
+		PGQ_TRY(pgq_ws_reserve(w.ws, WS_KS_LAYERS, (size_t)std::max<int64_t>(grp_h, 1) * n_ab * ng * sizeof(u64),
+		                       (void **)&layers));
+		PGQ_CUDA(cudaMemcpyAsync(w.glane, grp.data(), (size_t)ng * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+		k_ks_group_src<<<grid_size((ng + 255) / 256, 64), 256, 0, s>>>(ng, w.glane, w.psrc, w.gsrc);
+		PGQ_CUDA(cudaGetLastError());
+		w.st->kernel_launches++;
+		w.st->h2d_bytes += ng * (int64_t)sizeof(int32_t);
+		if (grp_h > 0) {
+			PGQ_CUDA(cudaMemsetAsync(layers, 0, (size_t)grp_h * n_ab * ng * sizeof(u64), s));
+		}
+		const auto admit = filter_for(w.glane);
+		for (int64_t h = 1; h <= grp_h && m > 0; h++) {
+			u64 *lcur = layers + (h - 1) * n_ab * ng;
+			const u64 *lprev = h >= 2 ? layers + (h - 2) * n_ab * ng : nullptr;
+			k_ks_omega<<<chunk_grid, 256, 0, s>>>((int)h, m, n_ab, ng, ng, csr->in.off, w.in_list, w.gsrc, lprev, lcur,
+			                                      nullptr, nullptr, 0, nullptr, admit);
+			w.st->kernel_launches++;
+		}
+		k_ks_unrank<<<grid_size(ng, (int64_t)sms * 16), 256, 0, s>>>(
+		    ng, ng, n, n_ab, w.glane, w.lane_row, w.psrc, w.pdst, w.src, w.dst, layers, csr->in.off, w.step_key,
+		    w.step_pos, csr->perm, csr->edge_ids, w.npaths, w.last, w.first, w.elem_off, w.walk_off, w.elems, admit);
+		PGQ_CUDA(cudaGetLastError());
+		w.st->kernel_launches++;
+		// (the next group reuses the group buffers)
+		PGQ_CUDA(cudaStreamSynchronize(s));
+		grp.clear();
+		grp_h = 0;
+		return PGQ_OK;
+	};
+	for (const WalkLane &ln : lanes) {
+		if (layer_bytes(ln.last, 1) > (double)budget) {
+			return pgq_fail(PGQ_ERR_UNSUPPORTED, "the %s of row %lld need %.0f bytes of count layers, over the budget of "
+			                "%lld", w.what, (long long)ln.row, layer_bytes(ln.last, 1), (long long)budget);
+		}
+		const int64_t gh = std::max(grp_h, ln.last);
+		if (!grp.empty() && ((int64_t)grp.size() == cap || layer_bytes(gh, (int64_t)grp.size() + 1) > (double)budget)) {
+			PGQ_TRY(run_group());
+		}
+		grp.push_back(ln.lane);
+		grp_h = std::max(grp_h, ln.last);
+	}
+	return run_group();
+}
+
+// Ends the call's timing once the work queued so far (e: the first error in queueing it) has finished, and marks the
+// call settled; `what` names the results being copied back in the error
+int walk_end(WsGuard &g, pgq_stats *st, const char *what, cudaError_t e = cudaSuccess);
+
+// Copies the placed walks back as the call's lists (offsets closed by the element total, elements), the rows' first walk
+// and validity (d_valid, p rows), and ends the call's timing.  d2h_bytes counts the lists and the validity; the caller
+// counts the per-row arrays it copies.
+int walk_lists(Walk &w, WsGuard &g, int64_t p, const uint8_t *d_valid, int64_t *out_first_path, uint8_t *out_valid,
+               int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths);
+
+// The lists of a call without rows: offsets {0} and no elements (nor costs, with out_costs), as host allocations
+int empty_lists(int64_t **out_path_offsets, int64_t **out_elems, void **out_costs = nullptr);

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <condition_variable>
 #include <map>
 #include <memory>
@@ -37,6 +38,11 @@ int pgq_fail(int status, const char *fmt, ...);
 			return _s;          \
 		}                       \
 	} while (0)
+
+// a launch's grid: want blocks, at least 1 and at most cap
+static inline unsigned grid_size(int64_t want, int64_t cap) {
+	return (unsigned)std::max<int64_t>(1, std::min<int64_t>(want, cap));
+}
 
 // ---- geometry of the edge-tiled kernels --------------------------------------------------------
 // A "chunk" is 256 consecutive positions of an adjacency array, processed by one warp as 8 steps
@@ -142,11 +148,12 @@ enum WsSlot : int {
 	// WS_OUT_OFFSETS).
 	WS_AS_SIGMA = 59, WS_AS_COUNTERS = 60, WS_AS_STEP_KEY_A = 61, WS_AS_STEP_KEY_B = 62, WS_AS_STEP_POS_A = 63,
 	WS_AS_STEP_POS_B = 64, WS_AS_COUNT = 65, WS_AS_NPATHS = 66, WS_AS_PATH_LEN = 67,
-	// shortest_k_paths (pgq_kshortest.cu), which also reads all_shortest_paths' step lists: each lane's row and internal
-	// ids; a batch's backward reach (reach, frontier and next-frontier masks [n][W / 64]); its two rolling count layers
-	// [n_ab][W], each lane's running total, alive flag and counting bit, the call's counters; per row the walks, their
-	// elements, the last walk's length, the first walk and the first element; a storing group's lanes, their sources
-	// and its layers; and the walks' offsets, their elements and the scans' total.
+	// The walk engine (pgq_count.cuh) of shortest_k_paths (pgq_kshortest.cu) and of all_cheapest_paths (pgq_cheapest.cu),
+	// which also reads all_shortest_paths' step lists: each lane's row and internal ids; a batch's backward reach (reach,
+	// frontier and next-frontier masks [n][W / 64]); its two rolling count layers [n_ab][W], each lane's running total,
+	// alive flag and counting bit, the call's counters; per row the walks, their elements, the last walk's length, the
+	// first walk and the first element; a storing group's lanes, their sources and its layers; and the walks' offsets,
+	// their elements and the scans' total.
 	WS_KS_LANE_ROW = 68, WS_KS_PSRC = 69, WS_KS_PDST = 70, WS_KS_REACH = 71, WS_KS_FRONT = 72, WS_KS_NEXT = 73,
 	WS_KS_OMEGA_A = 74, WS_KS_OMEGA_B = 75, WS_KS_TOTAL = 76, WS_KS_ALIVE = 77, WS_KS_ACTIVE = 78, WS_KS_COUNTERS = 79,
 	WS_KS_NPATHS = 80, WS_KS_ROW_ELEMS = 81, WS_KS_LAST = 82, WS_KS_FIRST = 83, WS_KS_ELEM_OFF = 84,
@@ -162,17 +169,10 @@ enum WsSlot : int {
 	WS_KM_STEPS = 108, WS_KM_STEP_ELEMS = 109,
 	// shortest_k_groups in WALK mode, on top of shortest_k_paths' slots: each lane's length groups found past h = 0
 	WS_KG_GROUPS = 110,
-	// cheapest_path_count / all_cheapest_paths (pgq_cheapest.cu), behind the Bellman-Ford sweeps and over the step lists:
-	// each step-list entry's parent as an internal id; per lane of a sweep batch its internal ids, row and open flag; the
-	// tight backward reach (reach, frontier and next-frontier masks [n][L / 64]) and |B_tight(t)|; the two rolling count
-	// layers [n_ab][L], each lane's running total, alive and infinite flags and counting bit, the counters; per row the
-	// count, the walks listed, their elements, the last one's length, the first walk and the first element; a storing
-	// group's lanes, their sources and its layers; the walks' offsets and elements, and the scans' total.
-	WS_AC_STEP_PAR = 111, WS_AC_PSRC = 112, WS_AC_PDST = 113, WS_AC_LANE_ROW = 114, WS_AC_OPEN = 115, WS_AC_REACH = 116,
-	WS_AC_FRONT = 117, WS_AC_NEXT = 118, WS_AC_BSIZE = 119, WS_AC_OMEGA_A = 120, WS_AC_OMEGA_B = 121, WS_AC_TOTAL = 122,
-	WS_AC_ALIVE = 123, WS_AC_INF = 124, WS_AC_ACTIVE = 125, WS_AC_COUNTERS = 126, WS_AC_COUNT = 127, WS_AC_NPATHS = 128,
-	WS_AC_ROW_ELEMS = 129, WS_AC_LAST = 130, WS_AC_FIRST = 131, WS_AC_ELEM_OFF = 132, WS_AC_GROUP_LANE = 133,
-	WS_AC_GROUP_SRC = 134, WS_AC_LAYERS = 135, WS_AC_WALK_OFF = 136, WS_AC_ELEMS = 137, WS_AC_SCAN_TOTAL = 138,
+	// cheapest_path_count / all_cheapest_paths (pgq_cheapest.cu), behind the Bellman-Ford sweeps, on top of the walk
+	// engine's slots: each step-list entry's parent as an internal id; per lane of a sweep batch its open flag,
+	// |B_tight(t)| and infinite flag; per row the count.
+	WS_AC_STEP_PAR = 111, WS_AC_OPEN = 115, WS_AC_BSIZE = 119, WS_AC_INF = 124, WS_AC_COUNT = 127,
 	// cheapest_k_paths (pgq_cheapest_k.cu), which runs the rounds of the path modes (WS_KM_*: ids, spurs, lists, seed
 	// flags, lane map, spur lengths and offsets, TRAIL's ban bitmap and table, steps) over the step lists: a round's
 	// root costs; a batch's distances [n][W] as order-preserving keys, dirty bitmap and flags, tight levels [n][W]
@@ -212,11 +212,7 @@ constexpr int ws_km[] = {WS_KM_IDS, WS_KM_PIDS, WS_KM_SPURS, WS_KM_LISTS, WS_KM_
                          WS_KM_LANE_OFF, WS_KM_COUNTERS, WS_KM_BAN_BITS, WS_KM_BAN_KEYS, WS_KM_STEPS,
                          WS_KM_STEP_ELEMS};
 constexpr int ws_kg[] = {WS_KG_GROUPS};
-constexpr int ws_ac[] = {WS_AC_STEP_PAR, WS_AC_PSRC, WS_AC_PDST, WS_AC_LANE_ROW, WS_AC_OPEN, WS_AC_REACH, WS_AC_FRONT,
-                         WS_AC_NEXT, WS_AC_BSIZE, WS_AC_OMEGA_A, WS_AC_OMEGA_B, WS_AC_TOTAL, WS_AC_ALIVE, WS_AC_INF,
-                         WS_AC_ACTIVE, WS_AC_COUNTERS, WS_AC_COUNT, WS_AC_NPATHS, WS_AC_ROW_ELEMS, WS_AC_LAST,
-                         WS_AC_FIRST, WS_AC_ELEM_OFF, WS_AC_GROUP_LANE, WS_AC_GROUP_SRC, WS_AC_LAYERS, WS_AC_WALK_OFF,
-                         WS_AC_ELEMS, WS_AC_SCAN_TOTAL};
+constexpr int ws_ac[] = {WS_AC_STEP_PAR, WS_AC_OPEN, WS_AC_BSIZE, WS_AC_INF, WS_AC_COUNT};
 constexpr int ws_ck[] = {WS_CK_ROOT, WS_CK_DIST, WS_CK_DIRTY, WS_CK_FLAGS, WS_CK_LEVEL, WS_CK_VBAN, WS_CK_FRONT,
                          WS_CK_GREW, WS_CK_DONE, WS_CK_STEP_W};
 constexpr int ws_analytics[] = {WS_LCC_SRC, WS_LCC_OUT, WS_LCC_OUT_VALID, WS_LCC_BIG_ROWS, WS_LCC_BIG_CNT,
@@ -253,15 +249,16 @@ static_assert(ws_apart(ws_staging, ws_driver, ws_bf), "a path entry point's stag
 static_assert(ws_apart(ws_cp, ws_staging, ws_bf), "the tight search runs on the distances and columns of its call");
 static_assert(ws_apart(ws_as, ws_staging, ws_driver, ws_radix),
               "path counts and step lists live across the batches of their driver, over the columns of their call");
-static_assert(ws_apart(ws_ks, ws_staging, ws_driver, ws_radix, ws_as),
-              "the walk search lives across its batches and groups, over the columns of its call and the step lists");
+static_assert(ws_apart(ws_ks, ws_staging, ws_driver, ws_radix, ws_as, ws_bf, ws_cp),
+              "the walk search lives across its batches and groups, over the columns of its call and the step lists, and "
+              "across the sweep batches of all_cheapest_paths, over their distances");
 static_assert(ws_apart(ws_km, ws_staging, ws_driver, ws_radix, ws_as, ws_ks),
               "the spur searches live across their rounds, over the step lists; WALK's own slots stay apart");
 static_assert(ws_apart(ws_kg, ws_staging, ws_driver, ws_radix, ws_as, ws_ks),
               "the length groups live across the walk search's batches, beside its own slots");
 static_assert(ws_apart(ws_ac, ws_staging, ws_bf, ws_as, ws_ks, ws_kg, ws_cp, ws_radix),
               "the tight walk search lives across the sweep batches, over their distances, the columns of its call and the "
-              "step lists; the walk search's own slots stay apart");
+              "step lists, beside the walk engine's slots");
 static_assert(ws_apart(ws_ck, ws_staging, ws_bf, ws_km, ws_ks, ws_ac, ws_cp, ws_as, ws_radix),
               "the Bellman-Ford spur searches live across their rounds, beside the rounds' own slots, over the step lists "
               "and the columns of their call; the other searches' slots stay apart");

@@ -53,10 +53,6 @@ __device__ __forceinline__ u64 km_ban_mask(const int64_t *__restrict__ keys, int
 	return mask;
 }
 
-static inline unsigned km_grid(int64_t want, int64_t cap) {
-	return (unsigned)std::max<int64_t>(1, std::min<int64_t>(want, cap));
-}
-
 // One batch of a round as km_run hands it to the spur search: cnt lanes in a batch W wide, lane l searching spur
 // lane_spur[l] of the round's spurs; TRAIL's banned positions as a bitmap over out-CSR positions and the sorted
 // (position * 512 + lane) table (both null when the batch bans none).  The search leaves each lane's spur length in

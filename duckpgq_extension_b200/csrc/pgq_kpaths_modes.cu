@@ -377,7 +377,7 @@ struct KmBfs : KmSearch {
 	}
 	int has_seed(Workspace *ws, int64_t ns, const KmSpur *spurs, const int32_t *lists, const std::vector<int64_t> &,
 	             uint8_t *has, pgq_stats *st) override {
-		k_km_has_seed<<<km_grid((ns + 7) / 8, (int64_t)csr->ctx->sm_count * 16), 256, 0, ws->stream>>>(
+		k_km_has_seed<<<grid_size((ns + 7) / 8, (int64_t)csr->ctx->sm_count * 16), 256, 0, ws->stream>>>(
 		    ns, spurs, lists, csr->out.off, csr->out.adj, has);
 		PGQ_CUDA(cudaGetLastError());
 		st->kernel_launches++;
@@ -388,8 +388,8 @@ struct KmBfs : KmSearch {
 		const int64_t n = csr->n, m = csr->m;
 		const int sms = csr->ctx->sm_count;
 		const int W = b.W, wd = W / 64, cnt = b.cnt;
-		const unsigned edge_grid = km_grid((m + 255) / 256, (int64_t)sms * 16);
-		const unsigned vert_grid = km_grid((n + 255) / 256, (int64_t)sms * 8);
+		const unsigned edge_grid = grid_size((m + 255) / 256, (int64_t)sms * 16);
+		const unsigned vert_grid = grid_size((n + 255) / 256, (int64_t)sms * 8);
 		PGQ_CUDA(cudaMemsetAsync(seen, 0, (size_t)n * wd * sizeof(u64), s));
 		PGQ_CUDA(cudaMemsetAsync(front, 0, (size_t)n * wd * sizeof(u64), s));
 		PGQ_CUDA(cudaMemsetAsync(next, 0, (size_t)n * wd * sizeof(u64), s));
@@ -485,21 +485,7 @@ int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, cons
 	memset(&st, 0, sizeof(st));
 	st.lanes = km_lanes(opts, search, 0);
 	if (p == 0) {
-		*out_path_offsets = (int64_t *)calloc(1, sizeof(int64_t));
-		*out_elems = (int64_t *)malloc(sizeof(int64_t));
-		if (out_costs) {
-			*out_costs = malloc(sizeof(int64_t));
-		}
-		if (!*out_path_offsets || !*out_elems || (out_costs && !*out_costs)) {
-			free(*out_path_offsets);
-			free(*out_elems);
-			*out_path_offsets = *out_elems = nullptr;
-			if (out_costs) {
-				free(*out_costs);
-				*out_costs = nullptr;
-			}
-			return pgq_fail(PGQ_ERR_OOM, "host allocation failed");
-		}
+		PGQ_TRY(empty_lists(out_path_offsets, out_elems, out_costs));
 		if (stats) {
 			*stats = st;
 		}
@@ -526,7 +512,7 @@ int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, cons
 		PGQ_TRY(pgq_ws_reserve(ws, WS_KM_BAN_BITS, (size_t)(m + 31) / 32 * sizeof(uint32_t), (void **)&ban_bits));
 	}
 	if (S > 0) {
-		k_km_ids<<<km_grid((2 * S + 255) / 256, 4096), 256, 0, s>>>(2 * S, d_ids, csr->perm, pids);
+		k_km_ids<<<grid_size((2 * S + 255) / 256, 4096), 256, 0, s>>>(2 * S, d_ids, csr->perm, pids);
 		PGQ_CUDA(cudaGetLastError());
 		st.kernel_launches++;
 	}
@@ -646,7 +632,7 @@ int km_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *dst, cons
 		// ---- the round's batches ----
 		for (int64_t b0 = 0; b0 < nl; b0 += W) {
 			const int cnt = (int)std::min<int64_t>(W, nl - b0);
-			const unsigned lane_grid = km_grid((cnt + 7) / 8, (int64_t)sms * 16);
+			const unsigned lane_grid = grid_size((cnt + 7) / 8, (int64_t)sms * 16);
 			st.batches++;
 			PGQ_CUDA(cudaMemcpyAsync(lane_spur, lane_of.data() + b0, (size_t)cnt * sizeof(int32_t), cudaMemcpyHostToDevice,
 			                         s));

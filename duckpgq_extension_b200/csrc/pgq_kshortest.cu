@@ -33,8 +33,9 @@
 //     and the walk adds the elements of the shorter walks of its row and of its rank's predecessors.
 // shortest_k_groups in WALK mode runs the same four phases (ks_run) with k_kg_step in place of k_ks_step: k counts
 // length groups, max_paths cuts the lists, and each row's rank bound is its listed count (DESIGN.md §3).
-// k_ks_reach_level, k_ks_omega and k_ks_unrank live in pgq_count.cuh, templates over an edge filter: these calls take
-// every edge (AllEdges), all_cheapest_paths (pgq_cheapest.cu) a lane's tight edges.
+// k_ks_reach_level, k_ks_omega and k_ks_unrank live in pgq_count.cuh, templates over an edge filter, with the host
+// driver that runs the phases (walk_*; its non-template parts are defined here): these calls take every edge
+// (AllEdges), all_cheapest_paths (pgq_cheapest.cu) a lane's tight edges.
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -44,10 +45,6 @@
 #include "pgq_tile.cuh"
 
 #define KS_BUDGET ((int64_t)4 << 30)
-
-// The call's counters: [0] a backward level added a bit; [1] lanes still counting; [2] a lane needs a walk longer than
-// KS_WALK_MAX
-enum { KS_CHANGED = 0, KS_ACTIVE = 1, KS_TOO_LONG = 2 };
 
 // internal ids of the lanes' sources and targets
 __global__ void k_ks_lanes(int64_t lanes, const int32_t *__restrict__ lane_row, const int64_t *__restrict__ src,
@@ -187,12 +184,137 @@ __global__ void k_ks_group_src(int ng, const int32_t *__restrict__ glane, const 
 	}
 }
 
+// ---- the walk engine's host driver (pgq_count.cuh) ----
 static inline u64 sat_add_host(u64 a, u64 b) { // a, b <= INT64_MAX
 	return a > AS_MAX - b ? AS_MAX : a + b;
 }
 
-static inline unsigned ks_grid(int64_t want, int64_t cap) {
-	return (unsigned)std::max<int64_t>(1, std::min<int64_t>(want, cap));
+int walk_reserve_rows(Walk &w, int64_t p) {
+	Workspace *ws = w.ws;
+	const size_t b8 = (size_t)p * sizeof(int64_t);
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_NPATHS, b8, (void **)&w.npaths));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ROW_ELEMS, b8, (void **)&w.elems_row));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_LAST, b8, (void **)&w.last));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_FIRST, b8, (void **)&w.first));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ELEM_OFF, b8, (void **)&w.elem_off));
+	return PGQ_OK;
+}
+
+int walk_reserve_lanes(Walk &w, int64_t lanes, int W) {
+	Workspace *ws = w.ws;
+	const int wd = (W + 63) / 64;
+	const size_t cells = (size_t)std::max<int64_t>(w.csr->n, 1) * wd;
+	const size_t layer = (size_t)std::max<int64_t>(w.csr->n_ab, 1) * W;
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_PSRC, (size_t)lanes * sizeof(int32_t), (void **)&w.psrc));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_PDST, (size_t)lanes * sizeof(int32_t), (void **)&w.pdst));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_REACH, cells * sizeof(u64), (void **)&w.reach));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_FRONT, cells * sizeof(u64), (void **)&w.front));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_NEXT, cells * sizeof(u64), (void **)&w.next));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_OMEGA_A, layer * sizeof(u64), (void **)&w.om_a));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_OMEGA_B, layer * sizeof(u64), (void **)&w.om_b));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_TOTAL, (size_t)W * sizeof(u64), (void **)&w.total));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ALIVE, (size_t)W * sizeof(uint32_t), (void **)&w.alive));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ACTIVE, (size_t)wd * sizeof(u64), (void **)&w.act));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_COUNTERS, 256, (void **)&w.ctr));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_GROUP_LANE, (size_t)W * sizeof(int32_t), (void **)&w.glane));
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_GROUP_SRC, (size_t)W * sizeof(int32_t), (void **)&w.gsrc));
+	return PGQ_OK;
+}
+
+int walk_offsets(Walk &w, int64_t lo, int64_t hi, const int64_t *h_np, const int64_t *h_el, uint8_t *valid) {
+	Workspace *ws = w.ws;
+	cudaStream_t s = ws->stream;
+	u64 walks = w.walks, elem_total = w.elem_total;
+	for (int64_t i = 0; i < hi - lo; i++) {
+		walks = sat_add_host(walks, (u64)h_np[i]);
+		elem_total = sat_add_host(elem_total, (u64)h_el[i]);
+	}
+	if (elem_total > (AS_MAX / sizeof(int64_t)) || walks > (AS_MAX / sizeof(int64_t)) - 1) {
+		return pgq_fail(PGQ_ERR_OOM, "the %s of one call hold too many elements (%llu)", w.what,
+		                (unsigned long long)elem_total);
+	}
+	int64_t *d_total;
+	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_SCAN_TOTAL, sizeof(int64_t), (void **)&d_total));
+	pgq_path_offsets((int64_t)w.elem_total, lo, hi, w.elem_off, w.elems_row, valid, d_total, s);
+	pgq_path_offsets((int64_t)w.walks, lo, hi, w.first, w.npaths, valid, d_total, s); // (valid = a row has a walk)
+	PGQ_CUDA(cudaGetLastError());
+	w.st->kernel_launches += 2;
+	// (grown, keeping what earlier batches placed; reserved at their size when there is nothing to keep)
+	auto size = [&](WsSlot slot, u64 count, u64 keep, int64_t **out) {
+		return keep ? pgq_ws_grow(ws, slot, (size_t)count * sizeof(int64_t), (size_t)keep * sizeof(int64_t), s, (void **)out)
+		            : pgq_ws_reserve(ws, slot, (size_t)count * sizeof(int64_t), (void **)out);
+	};
+	PGQ_TRY(size(WS_KS_WALK_OFF, walks + 1, w.walks, &w.walk_off));
+	PGQ_TRY(size(WS_KS_ELEMS, elem_total, w.elem_total, &w.elems));
+	w.walks = walks;
+	w.elem_total = elem_total;
+	return PGQ_OK;
+}
+
+int walk_end(WsGuard &g, pgq_stats *st, const char *what, cudaError_t e) {
+	Workspace *ws = g.ws;
+	if (e == cudaSuccess) e = cudaEventRecord(ws->ev_end, ws->stream);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(ws->stream);
+	float ms = 0.f;
+	if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end);
+	g.settled = (e == cudaSuccess);
+	if (e != cudaSuccess) {
+		cudaGetLastError();
+		return pgq_fail(PGQ_ERR_CUDA, "copying the %s back failed: %s", what, cudaGetErrorString(e));
+	}
+	st->total_ms = ms;
+	return PGQ_OK;
+}
+
+int walk_lists(Walk &w, WsGuard &g, int64_t p, const uint8_t *d_valid, int64_t *out_first_path, uint8_t *out_valid,
+               int64_t **out_path_offsets, int64_t **out_elems, int64_t *out_total_paths) {
+	cudaStream_t s = w.ws->stream;
+	const u64 walks = w.walks, elem_total = w.elem_total;
+	int64_t *h_off = (int64_t *)malloc((size_t)(walks + 1) * sizeof(int64_t));
+	int64_t *h_elems = (int64_t *)malloc((size_t)std::max<u64>(elem_total, 1) * sizeof(int64_t));
+	if (!h_off || !h_elems) {
+		free(h_off);
+		free(h_elems);
+		return pgq_fail(PGQ_ERR_OOM, "host allocation of the %s' %llu elements failed", w.what,
+		                (unsigned long long)elem_total);
+	}
+	cudaError_t e = cudaSuccess;
+	if (walks > 0) e = cudaMemcpyAsync(h_off, w.walk_off, (size_t)walks * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess && elem_total > 0)
+		e = cudaMemcpyAsync(h_elems, w.elems, (size_t)elem_total * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(out_first_path, w.first, (size_t)p * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(out_valid, d_valid, (size_t)p, cudaMemcpyDeviceToHost, s);
+	const int rc = walk_end(g, w.st, w.what, e);
+	if (rc != PGQ_OK) {
+		free(h_off);
+		free(h_elems);
+		return rc;
+	}
+	h_off[walks] = (int64_t)elem_total;
+	w.st->d2h_bytes += p + (int64_t)(walks + elem_total) * (int64_t)sizeof(int64_t);
+	*out_path_offsets = h_off;
+	*out_elems = h_elems;
+	*out_total_paths = (int64_t)walks;
+	return PGQ_OK;
+}
+
+int empty_lists(int64_t **out_path_offsets, int64_t **out_elems, void **out_costs) {
+	*out_path_offsets = (int64_t *)calloc(1, sizeof(int64_t));
+	*out_elems = (int64_t *)malloc(sizeof(int64_t));
+	if (out_costs) {
+		*out_costs = malloc(sizeof(int64_t));
+	}
+	if (!*out_path_offsets || !*out_elems || (out_costs && !*out_costs)) {
+		free(*out_path_offsets);
+		free(*out_elems);
+		*out_path_offsets = *out_elems = nullptr;
+		if (out_costs) {
+			free(*out_costs);
+			*out_costs = nullptr;
+		}
+		return pgq_fail(PGQ_ERR_OOM, "host allocation failed");
+	}
+	return PGQ_OK;
 }
 
 // the layer budget of the storing pass: 4 GiB, or PGQ_B200_KSP_LAYER_BUDGET bytes (tests force regrouping with it)
@@ -279,7 +401,7 @@ static int ks_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
                   int64_t *out_total_paths, pgq_stats *stats) {
 	int64_t budget;
 	PGQ_TRY(layer_budget(&budget));
-	const int64_t n = csr->n, m = csr->m, n_ab = csr->n_ab;
+	const int64_t n = csr->n, n_ab = csr->n_ab;
 	// the lanes: the rows whose ids are both valid, in input order
 	std::vector<int32_t> lane_row;
 	for (int64_t i = 0; i < p; i++) {
@@ -297,20 +419,9 @@ static int ks_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 	memset(&st, 0, sizeof(st));
 	st.lanes = W;
 	st.searches = S;
-	if (p == 0 && kg && kg->count_only) {
-		if (stats) {
-			*stats = st;
-		}
-		return PGQ_OK;
-	}
 	if (p == 0) {
-		*out_path_offsets = (int64_t *)calloc(1, sizeof(int64_t));
-		*out_elems = (int64_t *)malloc(sizeof(int64_t));
-		if (!*out_path_offsets || !*out_elems) {
-			free(*out_path_offsets);
-			free(*out_elems);
-			*out_path_offsets = *out_elems = nullptr;
-			return pgq_fail(PGQ_ERR_OOM, "host allocation failed");
+		if (!(kg && kg->count_only)) {
+			PGQ_TRY(empty_lists(out_path_offsets, out_elems));
 		}
 		if (stats) {
 			*stats = st;
@@ -322,40 +433,21 @@ static int ks_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 	PGQ_TRY(pgq_ws_acquire(csr->ctx, &g.ws));
 	Workspace *ws = g.ws;
 	cudaStream_t s = ws->stream;
-	const int sms = csr->ctx->sm_count;
 	const size_t b8 = (size_t)p * sizeof(int64_t);
-	const int wd = W / 64;
-	const int64_t cells = n * wd;
-	const int64_t *d_src, *d_dst;
-	const int32_t *d_lane_row;
-	int32_t *psrc, *pdst, *gsrc, *glane;
-	u64 *reach, *front, *next, *om_a, *om_b, *total, *act, *ctr;
-	uint32_t *alive;
-	int64_t *npaths, *elems_row, *last, *first, *elem_off;
+	Walk w = {};
+	w.csr = csr;
+	w.ws = ws;
+	w.st = &st;
+	w.what = "walks";
+	w.in_list = csr->in.adj;
 	uint8_t *d_valid;
-	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&d_src));
-	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&d_dst));
+	PGQ_TRY(stage_column(ws, WS_IN_SRC, src, b8, (const void **)&w.src));
+	PGQ_TRY(stage_column(ws, WS_IN_DST, dst, b8, (const void **)&w.dst));
 	PGQ_TRY(stage_column(ws, WS_KS_LANE_ROW, S ? lane_row.data() : nullptr, (size_t)S * sizeof(int32_t),
-	                     (const void **)&d_lane_row));
+	                     (const void **)&w.lane_row));
 	PGQ_TRY(pgq_ws_reserve(ws, WS_OUT_VALID, (size_t)p, (void **)&d_valid));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_PSRC, (size_t)S * sizeof(int32_t), (void **)&psrc));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_PDST, (size_t)S * sizeof(int32_t), (void **)&pdst));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_REACH, (size_t)cells * sizeof(u64), (void **)&reach));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_FRONT, (size_t)cells * sizeof(u64), (void **)&front));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_NEXT, (size_t)cells * sizeof(u64), (void **)&next));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_OMEGA_A, (size_t)n_ab * W * sizeof(u64), (void **)&om_a));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_OMEGA_B, (size_t)n_ab * W * sizeof(u64), (void **)&om_b));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_TOTAL, (size_t)W * sizeof(u64), (void **)&total));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ALIVE, (size_t)W * sizeof(uint32_t), (void **)&alive));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ACTIVE, (size_t)wd * sizeof(u64), (void **)&act));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_COUNTERS, 256, (void **)&ctr));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_NPATHS, b8, (void **)&npaths));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ROW_ELEMS, b8, (void **)&elems_row));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_LAST, b8, (void **)&last));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_FIRST, b8, (void **)&first));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ELEM_OFF, b8, (void **)&elem_off));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_GROUP_SRC, (size_t)W * sizeof(int32_t), (void **)&gsrc));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_GROUP_LANE, (size_t)W * sizeof(int32_t), (void **)&glane));
+	PGQ_TRY(walk_reserve_lanes(w, S, W));
+	PGQ_TRY(walk_reserve_rows(w, p));
 	int64_t *lg = nullptr;
 	std::vector<u64> h_total; // shortest_k_groups: each lane's walk count N and its groups past h = 0
 	std::vector<int64_t> h_lg;
@@ -365,104 +457,67 @@ static int ks_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 		h_lg.resize((size_t)S);
 	}
 	PGQ_CUDA(cudaEventRecord(ws->ev_begin, s));
-	PGQ_CUDA(cudaMemsetAsync(npaths, 0, b8, s));
-	PGQ_CUDA(cudaMemsetAsync(elems_row, 0, b8, s));
-	PGQ_CUDA(cudaMemsetAsync(last, 0xff, b8, s)); // -1: no walk
-	PGQ_CUDA(cudaMemsetAsync(alive, 0, (size_t)W * sizeof(uint32_t), s));
+	PGQ_CUDA(cudaMemsetAsync(w.npaths, 0, b8, s));
+	PGQ_CUDA(cudaMemsetAsync(w.elems_row, 0, b8, s));
+	PGQ_CUDA(cudaMemsetAsync(w.last, 0xff, b8, s)); // -1: no walk
+	PGQ_CUDA(cudaMemsetAsync(w.alive, 0, (size_t)W * sizeof(uint32_t), s));
 	if (S > 0) {
-		k_ks_lanes<<<ks_grid((S + 255) / 256, 4096), 256, 0, s>>>(S, d_lane_row, d_src, d_dst, csr->perm, psrc, pdst);
+		k_ks_lanes<<<grid_size((S + 255) / 256, 4096), 256, 0, s>>>(S, w.lane_row, w.src, w.dst, csr->perm, w.psrc, w.pdst);
 		PGQ_CUDA(cudaGetLastError());
 		st.kernel_launches++;
 	}
-	const u64 *step_key = nullptr;
-	const int32_t *step_pos = nullptr;
 	if (!(kg && kg->count_only)) {
-		PGQ_TRY(build_step_lists(csr, ws, s, &step_key, &step_pos, &st.kernel_launches));
+		PGQ_TRY(build_step_lists(csr, ws, s, &w.step_key, &w.step_pos, &st.kernel_launches));
 	}
-	const unsigned edge_grid = ks_grid((m + 255) / 256, (int64_t)sms * 16);
-	const unsigned chunk_grid = ks_grid((m + KS_CHUNK * 8 - 1) / (KS_CHUNK * 8), (int64_t)sms * 16);
-	const unsigned cell_grid = ks_grid((cells + 255) / 256, (int64_t)sms * 8);
-	u64 h_ctr[3];
 	// ---- per batch: backward reach, then the counting pass ----
 	for (int64_t b0 = 0; b0 < S; b0 += W) {
 		const int cnt = (int)std::min<int64_t>(W, S - b0);
 		const int L = (int)std::min<int64_t>(W, (cnt + 63) / 64 * 64);
 		const int bwd = L / 64;
 		const int64_t bcells = n * bwd;
-		const unsigned lane_grid = ks_grid((cnt + 255) / 256, 64);
+		const unsigned lane_grid = grid_size((cnt + 255) / 256, 64);
+		const int32_t *lrow = w.lane_row + b0, *psrc = w.psrc + b0, *pdst = w.pdst + b0;
 		st.batches++;
-		PGQ_CUDA(cudaMemsetAsync(reach, 0, (size_t)bcells * sizeof(u64), s));
-		PGQ_CUDA(cudaMemsetAsync(front, 0, (size_t)bcells * sizeof(u64), s));
-		PGQ_CUDA(cudaMemsetAsync(next, 0, (size_t)bcells * sizeof(u64), s));
-		PGQ_CUDA(cudaMemsetAsync(act, 0, (size_t)bwd * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(w.reach, 0, (size_t)bcells * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(w.front, 0, (size_t)bcells * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(w.next, 0, (size_t)bcells * sizeof(u64), s));
+		PGQ_CUDA(cudaMemsetAsync(w.act, 0, (size_t)bwd * sizeof(u64), s));
 		if (kg) {
 			PGQ_CUDA(cudaMemsetAsync(lg, 0, (size_t)cnt * sizeof(int64_t), s));
 		}
-		k_ks_reach_seed<<<lane_grid, 256, 0, s>>>(cnt, bwd, pdst + b0, reach, front);
+		k_ks_reach_seed<<<lane_grid, 256, 0, s>>>(cnt, bwd, pdst, w.reach, w.front);
 		PGQ_CUDA(cudaGetLastError());
 		st.kernel_launches++;
-		for (;;) {
-			PGQ_CUDA(cudaMemsetAsync(&ctr[KS_CHANGED], 0, sizeof(u64), s));
-			if (m > 0) {
-				k_ks_reach_level<<<edge_grid, 256, 0, s>>>(m, n_ab, bwd, csr->in.off, csr->in.adj, front, reach, next);
-				st.kernel_launches++;
-			}
-			k_ks_reach_update<<<ks_grid((bcells + 255) / 256, (int64_t)sms * 8), 256, 0, s>>>(bcells, reach, front, next,
-			                                                                                  ctr);
-			PGQ_CUDA(cudaGetLastError());
-			st.kernel_launches++;
-			st.push_levels++;
-			PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(u64), cudaMemcpyDeviceToHost, s));
-			PGQ_CUDA(cudaStreamSynchronize(s));
-			if (!h_ctr[KS_CHANGED]) {
-				break;
-			}
-		}
-		PGQ_CUDA(cudaMemsetAsync(ctr, 0, 3 * sizeof(u64), s));
-		k_ks_start<<<lane_grid, 256, 0, s>>>(cnt, bwd, k, d_lane_row + b0, psrc + b0, pdst + b0, reach, total, act, npaths,
-		                                     elems_row, last, ctr);
-		PGQ_CUDA(cudaGetLastError());
-		st.kernel_launches++;
-		PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, s));
-		PGQ_CUDA(cudaStreamSynchronize(s));
-		u64 *prev = om_a, *cur = om_b;
-		for (int h = 1; h_ctr[KS_ACTIVE] > 0; h++) {
-			PGQ_CUDA(cudaMemsetAsync(cur, 0, (size_t)n_ab * L * sizeof(u64), s));
-			PGQ_CUDA(cudaMemsetAsync(&ctr[KS_ACTIVE], 0, sizeof(u64), s));
-			if (m > 0) {
-				k_ks_omega<<<chunk_grid, 256, 0, s>>>(h, m, n_ab, L, cnt, csr->in.off, csr->in.adj, psrc + b0, prev, cur,
-				                                      reach, act, bwd, alive);
-				st.kernel_launches++;
-			}
+		PGQ_TRY(walk_reach(w, bwd, bcells, AllEdges()));
+		auto start = [&]() {
+			k_ks_start<<<lane_grid, 256, 0, s>>>(cnt, bwd, k, lrow, psrc, pdst, w.reach, w.total, w.act, w.npaths,
+			                                     w.elems_row, w.last, w.ctr);
+		};
+		auto step = [&](int h, const u64 *cur) {
 			if (kg) {
-				k_kg_step<<<lane_grid, 256, 0, s>>>(h, cnt, L, n_ab, k, kg->max_paths, d_lane_row + b0, psrc + b0, pdst + b0,
-				                                    cur, alive, total, lg, act, npaths, elems_row, last, ctr);
+				k_kg_step<<<lane_grid, 256, 0, s>>>(h, cnt, L, n_ab, k, kg->max_paths, lrow, psrc, pdst, cur, w.alive,
+				                                    w.total, lg, w.act, w.npaths, w.elems_row, w.last, w.ctr);
 			} else {
-				k_ks_step<<<lane_grid, 256, 0, s>>>(h, cnt, L, n_ab, k, d_lane_row + b0, pdst + b0, cur, alive, total, act,
-				                                    npaths, elems_row, last, ctr);
+				k_ks_step<<<lane_grid, 256, 0, s>>>(h, cnt, L, n_ab, k, lrow, pdst, cur, w.alive, w.total, w.act, w.npaths,
+				                                    w.elems_row, w.last, w.ctr);
 			}
-			PGQ_CUDA(cudaGetLastError());
-			st.kernel_launches++;
-			st.levels++;
-			PGQ_CUDA(cudaMemcpyAsync(h_ctr, ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, s));
-			PGQ_CUDA(cudaStreamSynchronize(s));
-			if (h_ctr[KS_TOO_LONG]) {
-				return pgq_fail(PGQ_ERR_UNSUPPORTED, "a row needs a walk longer than %d edges", KS_WALK_MAX);
-			}
-			std::swap(prev, cur);
-		}
+		};
+		PGQ_TRY(walk_count(w, L, cnt, bwd, psrc, AllEdges(), start, step, &st.levels,
+		                   "a row needs a walk longer than"));
 		if (kg) {
-			PGQ_CUDA(cudaMemcpyAsync(h_total.data() + b0, total, (size_t)cnt * sizeof(u64), cudaMemcpyDeviceToHost, s));
+			PGQ_CUDA(cudaMemcpyAsync(h_total.data() + b0, w.total, (size_t)cnt * sizeof(u64), cudaMemcpyDeviceToHost, s));
 			PGQ_CUDA(cudaMemcpyAsync(h_lg.data() + b0, lg, (size_t)cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
 			st.d2h_bytes += cnt * (int64_t)(sizeof(u64) + sizeof(int64_t));
 		}
 	}
 	// ---- the rows' walk counts and element counts; their first walk and first element ----
 	std::vector<int64_t> h_np((size_t)p), h_el((size_t)p), h_last((size_t)p);
-	PGQ_CUDA(cudaMemcpyAsync(h_np.data(), npaths, b8, cudaMemcpyDeviceToHost, s));
-	PGQ_CUDA(cudaMemcpyAsync(h_el.data(), elems_row, b8, cudaMemcpyDeviceToHost, s));
-	PGQ_CUDA(cudaMemcpyAsync(h_last.data(), last, b8, cudaMemcpyDeviceToHost, s));
+	PGQ_CUDA(cudaMemcpyAsync(h_np.data(), w.npaths, b8, cudaMemcpyDeviceToHost, s));
+	PGQ_CUDA(cudaMemcpyAsync(h_el.data(), w.elems_row, b8, cudaMemcpyDeviceToHost, s));
+	PGQ_CUDA(cudaMemcpyAsync(h_last.data(), w.last, b8, cudaMemcpyDeviceToHost, s));
 	PGQ_CUDA(cudaStreamSynchronize(s));
+	st.h2d_bytes += 2 * (int64_t)b8 + S * (int64_t)sizeof(int32_t);
+	st.d2h_bytes += 3 * (int64_t)b8;
 	if (kg) { // the rows' groups: NULL rows have none and are complete
 		std::vector<int64_t> h_count((size_t)p, 0);
 		for (int64_t i = 0; i < p; i++) {
@@ -481,17 +536,10 @@ static int ks_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 			memcpy(kg->count, h_count.data(), b8);
 		}
 		if (kg->count_only) {
-			PGQ_CUDA(cudaEventRecord(ws->ev_end, s));
-			PGQ_CUDA(cudaStreamSynchronize(s));
-			g.settled = true;
-			float ms = 0.f;
-			PGQ_CUDA(cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end));
+			PGQ_TRY(walk_end(g, &st, "walk counts"));
 			for (int64_t i = 0; i < p; i++) {
 				out_valid[i] = h_count[(size_t)i] > 0;
 			}
-			st.total_ms = ms;
-			st.h2d_bytes += 2 * (int64_t)b8 + S * (int64_t)sizeof(int32_t);
-			st.d2h_bytes += 3 * (int64_t)b8;
 			if (stats) {
 				*stats = st;
 			}
@@ -505,112 +553,18 @@ static int ks_run(pgq_csr *csr, int64_t p, const int64_t *src, const int64_t *ds
 			kg->complete[i] = h_np[(size_t)i] == h_count[(size_t)i];
 		}
 	}
-	u64 walks = 0, elem_total = 0;
-	for (int64_t i = 0; i < p; i++) {
-		walks = sat_add_host(walks, (u64)h_np[(size_t)i]);
-		elem_total = sat_add_host(elem_total, (u64)h_el[(size_t)i]);
-	}
-	if (elem_total > (AS_MAX / sizeof(int64_t)) || walks > (AS_MAX / sizeof(int64_t)) - 1) {
-		return pgq_fail(PGQ_ERR_OOM, "the walks of one call hold too many elements (%llu)",
-		                (unsigned long long)elem_total);
-	}
-	int64_t *d_total;
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_SCAN_TOTAL, sizeof(int64_t), (void **)&d_total));
-	pgq_path_offsets(0, 0, p, elem_off, elems_row, d_valid, d_total, s);
-	pgq_path_offsets(0, 0, p, first, npaths, d_valid, d_total, s); // (out_valid = a row has a walk)
-	PGQ_CUDA(cudaGetLastError());
-	st.kernel_launches += 2;
-	int64_t *walk_off, *d_elems;
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_WALK_OFF, (size_t)(walks + 1) * sizeof(int64_t), (void **)&walk_off));
-	PGQ_TRY(pgq_ws_reserve(ws, WS_KS_ELEMS, (size_t)elem_total * sizeof(int64_t), (void **)&d_elems));
-	// ---- the storing pass and the unranking, group by group ----
-	std::vector<int32_t> grp;
-	int64_t grp_h = 0;
-	auto layer_bytes = [&](int64_t h, int64_t rows) { return (double)(h + 1) * (double)n_ab * (double)rows * 8.0; };
-	auto run_group = [&]() -> int {
-		const int ng = (int)grp.size();
-		if (ng == 0) {
-			return PGQ_OK;
-		}
-		u64 *layers;
-		PGQ_TRY(pgq_ws_reserve(ws, WS_KS_LAYERS, (size_t)std::max<int64_t>(grp_h, 1) * n_ab * ng * sizeof(u64),
-		                       (void **)&layers));
-		PGQ_CUDA(cudaMemcpyAsync(glane, grp.data(), (size_t)ng * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-		k_ks_group_src<<<ks_grid((ng + 255) / 256, 64), 256, 0, s>>>(ng, glane, psrc, gsrc);
-		PGQ_CUDA(cudaGetLastError());
-		st.kernel_launches++;
-		if (grp_h > 0) {
-			PGQ_CUDA(cudaMemsetAsync(layers, 0, (size_t)grp_h * n_ab * ng * sizeof(u64), s));
-		}
-		for (int64_t h = 1; h <= grp_h && m > 0; h++) {
-			u64 *lcur = layers + (h - 1) * n_ab * ng;
-			const u64 *lprev = h >= 2 ? layers + (h - 2) * n_ab * ng : nullptr;
-			k_ks_omega<<<chunk_grid, 256, 0, s>>>((int)h, m, n_ab, ng, ng, csr->in.off, csr->in.adj, gsrc, lprev, lcur,
-			                                      nullptr, nullptr, 0, nullptr);
-			st.kernel_launches++;
-		}
-		k_ks_unrank<<<ks_grid(ng, (int64_t)sms * 16), 256, 0, s>>>(
-		    ng, ng, n, n_ab, glane, d_lane_row, psrc, pdst, d_src, d_dst, layers, csr->in.off, step_key, step_pos,
-		    csr->perm, csr->edge_ids, npaths, last, first, elem_off, walk_off, d_elems);
-		PGQ_CUDA(cudaGetLastError());
-		st.kernel_launches++;
-		// (the next group reuses the group buffers)
-		PGQ_CUDA(cudaStreamSynchronize(s));
-		grp.clear();
-		grp_h = 0;
-		return PGQ_OK;
-	};
+	PGQ_TRY(walk_offsets(w, 0, p, h_np.data(), h_el.data(), d_valid));
+	// ---- the storing pass and the unranking, group by group over the call's lanes ----
+	std::vector<WalkLane> listed;
 	for (int64_t ln = 0; ln < S; ln++) {
 		const int64_t row = lane_row[(size_t)ln];
-		if (h_np[(size_t)row] == 0) {
-			continue;
+		if (h_np[(size_t)row] > 0) {
+			listed.push_back({(int32_t)ln, row, h_last[(size_t)row]});
 		}
-		const int64_t h = h_last[(size_t)row];
-		if (layer_bytes(h, 1) > (double)budget) {
-			return pgq_fail(PGQ_ERR_UNSUPPORTED, "the walks of row %lld need %.0f bytes of count layers, over the budget of "
-			                "%lld", (long long)row, layer_bytes(h, 1), (long long)budget);
-		}
-		const int64_t gh = std::max(grp_h, h);
-		if (!grp.empty() && ((int64_t)grp.size() == W || layer_bytes(gh, (int64_t)grp.size() + 1) > (double)budget)) {
-			PGQ_TRY(run_group());
-		}
-		grp.push_back((int32_t)ln);
-		grp_h = std::max(grp_h, h);
 	}
-	PGQ_TRY(run_group());
-	// ---- back to the host ----
-	int64_t *h_off = (int64_t *)malloc((size_t)(walks + 1) * sizeof(int64_t));
-	int64_t *h_elems = (int64_t *)malloc((size_t)std::max<u64>(elem_total, 1) * sizeof(int64_t));
-	if (!h_off || !h_elems) {
-		free(h_off);
-		free(h_elems);
-		return pgq_fail(PGQ_ERR_OOM, "host allocation of %llu walk elements failed", (unsigned long long)elem_total);
-	}
-	cudaError_t e = cudaSuccess;
-	if (walks > 0) e = cudaMemcpyAsync(h_off, walk_off, (size_t)walks * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
-	if (e == cudaSuccess && elem_total > 0)
-		e = cudaMemcpyAsync(h_elems, d_elems, (size_t)elem_total * sizeof(int64_t), cudaMemcpyDeviceToHost, s);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(out_first_path, first, b8, cudaMemcpyDeviceToHost, s);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(out_valid, d_valid, (size_t)p, cudaMemcpyDeviceToHost, s);
-	if (e == cudaSuccess) e = cudaEventRecord(ws->ev_end, s);
-	if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-	float ms = 0.f;
-	if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ws->ev_begin, ws->ev_end);
-	g.settled = (e == cudaSuccess);
-	if (e != cudaSuccess) {
-		cudaGetLastError();
-		free(h_off);
-		free(h_elems);
-		return pgq_fail(PGQ_ERR_CUDA, "copying the walks back failed: %s", cudaGetErrorString(e));
-	}
-	h_off[walks] = (int64_t)elem_total;
+	PGQ_TRY(walk_store(w, listed, W, budget, [](const int32_t *) { return AllEdges(); }));
+	PGQ_TRY(walk_lists(w, g, p, d_valid, out_first_path, out_valid, out_path_offsets, out_elems, out_total_paths));
 	memcpy(out_npaths, h_np.data(), b8);
-	st.total_ms = ms;
-	st.h2d_bytes += 2 * (int64_t)b8 + S * (int64_t)sizeof(int32_t);
-	st.d2h_bytes += 3 * (int64_t)b8 + p + (int64_t)(walks + elem_total) * (int64_t)sizeof(int64_t);
-	*out_path_offsets = h_off;
-	*out_elems = h_elems;
-	*out_total_paths = (int64_t)walks;
 	if (stats) {
 		*stats = st;
 	}
