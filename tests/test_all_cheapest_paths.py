@@ -274,8 +274,11 @@ def compare(ctx, n, src, dst, w, ps, pd, max_paths, sv=None, dv=None):
     opaths, ocnt2, ost2 = oac.all_cheapest_paths(n, v, e, ids, ww, ps, pd, max_paths, sv, dv, st["lanes"])
     assert cnt.tolist() == ocnt.tolist() and cnt2.tolist() == ocnt2.tolist() and valid.tolist() == ovalid.tolist()
     assert paths == opaths
+    # (the number of sweeps varies from call to call with the order of the parallel relaxations; each sweep is one
+    # launch, so launches - sweeps is fixed: three launches per batch for cheapest_path_length)
+    assert lst["kernel_launches"] - lst["levels"] == 3 * lst["batches"]
     for s_ in (cst, st):
-        assert (s_["batches"], s_["levels"], s_["lanes"]) == (lst["batches"], lst["levels"], lst["lanes"])
+        assert (s_["batches"], s_["lanes"]) == (lst["batches"], lst["lanes"])
         assert (s_["batches"], s_["push_levels"]) == (ost["batches"], ost["push_levels"])
     assert cst["pull_levels"] == ost["pull_levels"] and st["pull_levels"] == ost2["pull_levels"]
     assert [x[0] if x else None for x in paths] == cpaths  # path 0 is cheapest_path's

@@ -77,7 +77,7 @@ class Graph:
         m = len(self.e)
         row = np.repeat(np.arange(n), np.diff(self.v[:n + 1]))
         order = np.lexsort((np.arange(m), row, self.e))  # by target, then parent, then adjacency position
-        self.st_par, self.st_eid = row[order], self.ids[order]
+        self.st_par, self.st_eid, self.st_idx = row[order], self.ids[order], order
         self.st_off = np.searchsorted(self.e[order], np.arange(n + 1))
         self.in_deg = self.lay["ind"]
 
@@ -105,9 +105,10 @@ def sat(x):
     return min(x, INT64_MAX)
 
 
-def unrank(g, lay, s, t, h, r, rec):
+def unrank(g, lay, s, t, h, r, rec, admit=None):
     """Walk r (exact rank) of the h-edge walks s -> t, whose w_j are lay[j] -> [s, e1, v1, ..., t].  Appends the work
-    of every step to rec."""
+    of every step to rec.  admit (optional): per step-list entry, whether the walk may take it; an entry it refuses
+    stays in its in-list as a zero term."""
     out = [0] * (2 * h + 1)
     out[-1] = t
     if h == 0:
@@ -115,7 +116,8 @@ def unrank(g, lay, s, t, h, r, rec):
     cur = t
     for k in range(h, 0, -1):
         par, eid = g.steps(cur)
-        terms = [lay[k - 1].get(p, 0) for p in par.tolist()]
+        o = int(g.st_off[cur])
+        terms = [lay[k - 1].get(p, 0) if admit is None or admit[o + i] else 0 for i, p in enumerate(par.tolist())]
         pre, j = 0, None
         for i, x in enumerate(terms):
             if pre + x > r:
@@ -227,10 +229,18 @@ def kwalk_row(g, s, t, k, groups=False, max_paths=0):
     return res
 
 
-def chunk_work(g, lay, B, H):
-    """Per layer 1..H, the in-lists of the rows of B (internal ids) that span more than one chunk: their parts"""
+def chunk_work(g, lay, B, H, in_adj=None, admit=None):
+    """Per layer 1..H, the in-lists of the rows of B (internal ids) that span more than one chunk: their parts.
+    in_adj (optional): the in-lists walked, internal parent ids by in-CSC position (g.in_adj by default); admit
+    (optional): per position, whether its edge counts."""
     out = []
     inv = g.lay["inv"]
+    if in_adj is None:
+        in_adj = g.in_adj
+
+    def part(a, b, prev):
+        return sum(prev.get(int(inv[p]), 0) for i, p in enumerate(in_adj[a:b].tolist(), a)
+                   if admit is None or admit[i])
     for u_int in range(g.n_ab):
         rs, re_ = int(g.in_off[u_int]), int(g.in_off[u_int + 1])
         u = int(inv[u_int])
@@ -239,13 +249,13 @@ def chunk_work(g, lay, B, H):
         for h in range(1, H + 1):
             prev = lay[h - 1]
             if rs // CHUNK == (re_ - 1) // CHUNK:
-                total = sum(prev.get(int(inv[p]), 0) for p in g.in_adj[rs:re_].tolist())
+                total = part(rs, re_, prev)
                 out.append(dict(u=u_int, h=h, split=False, parts=[total], rs=rs, re=re_, middle=False))
                 continue
             parts, middle = [], False
             for c0 in range(rs // CHUNK * CHUNK, re_, CHUNK):
                 a, b = max(rs, c0), min(re_, c0 + CHUNK)
-                parts.append(sum(prev.get(int(inv[p]), 0) for p in g.in_adj[a:b].tolist()))
+                parts.append(part(a, b, prev))
                 middle |= rs < c0 and re_ > c0 + CHUNK
             out.append(dict(u=u_int, h=h, split=True, parts=parts, rs=rs, re=re_, middle=middle))
     return out
