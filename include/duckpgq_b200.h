@@ -519,15 +519,20 @@ int pgq_shortest_k_paths_mode(pgq_csr *csr, int64_t n_pairs, const int64_t *src,
  *   - cost(P) = P's weights added left to right from 0 in the weight type's arithmetic (int64 addition; double addition
  *     rounded to nearest).  A list is not a path when its cost is NaN or reaches pgq_cheapest_path_length's sentinel
  *     (INT64_MAX / 2; DBL_MAX / 2), tested before each addition (for BIGINT w < sentinel - c), so nothing overflows.
- *     Prefix costs never decrease, so a row has a path exactly when pgq_cheapest_path_length's cost is not NULL.
+ *     Prefix costs never decrease, so a row has a path exactly when pgq_cheapest_path_length's cost is not NULL, as
+ *     long as every BIGINT weight is at most 2^62.  Above that pgq_cheapest_path_length's sums are the reference's
+ *     and are not defined (DESIGN.md §3): they can wrap on a route from s (0 -> 1 -> 2 over weights [1, INT64_MAX]
+ *     gets a negative cost there and NULL here) or from a vertex s does not reach, whose sentinel plus the weight
+ *     wraps into t (a negative cost there, t's own cheapest path here).
  *   - format, modes and NULL rows are pgq_shortest_k_paths_mode's: a path is [s, e1, v1, ..., eh, t]; WALK, TRAIL,
  *     ACYCLIC and SIMPLE admit paths by the same rules, TRAIL's adjacency-entry edges and the s == t cases included;
  *     NULL (out_valid 0, no paths): a NULL id, or no admitted path.
  *   - order: by cost ascending (compared as values), then by h, then by the steps from t back to s as
  *     pgq_shortest_k_paths orders them.  The result is the first min(k, total) admitted paths in that order; with
  *     weights >= 0 that prefix exists even when zero-cost cycles make WALK's total infinite.  s == t: path 0 is [s]
- *     with cost 0.  k = 1 gives pgq_cheapest_path's path in every mode, with pgq_cheapest_path_length's cost; with every
- *     weight 0 or every weight 1 (BIGINT) the paths are pgq_shortest_k_paths_mode's.
+ *     with cost 0.  With no BIGINT weight above 2^62, k = 1 gives pgq_cheapest_path's path in every mode, with
+ *     pgq_cheapest_path_length's cost; with every weight 0 or every weight 1 (BIGINT) the paths are
+ *     pgq_shortest_k_paths_mode's.
  *   - DOUBLE: the order above is exact for BIGINT.  For DOUBLE it holds whenever every sum involved is exact (dyadic
  *     weights, for example); when a sum rounds, the construction below is the contract, as the tight-edge rule is for
  *     pgq_all_cheapest_paths.  With edges 0 -> 1 (0.1), 1 -> 2 (0.2) and 0 -> 2 (0.3), WALK's two paths from 0 to 2 are
